@@ -1098,7 +1098,8 @@ extern "C" int apus_get_stats(apus_replica_t *r, apus_stats_t *out)
     out->kernel_launches = r->launches;
     out->lat_samples = c.lat_count;
     out->auto_heads = c.auto_heads;
-    out->entries_published = c.published;
+    /* published-but-uncommitted entries count too (`published` itself follows the commit) */
+    out->entries_published = c.pub_seen > c.published ? c.pub_seen : c.published;
     for (int i = 0; i < 8; i++) { out->phase_ns[i] = c.phase_ns[i]; out->turn_ns[i] = c.turn_ns[i]; }
     return APUS_OK;
 }
@@ -1420,6 +1421,9 @@ extern "C" int apus_ctl_adjust_follower(apus_replica_t *r, uint8_t peer, uint64_
     if (peer_write(r, peer, offsetof(apus_ctrl_t, acked), &mine, 8) != APUS_OK) return APUS_ERROR;
     const uint64_t none = L;
     if (peer_write(r, peer, offsetof(apus_ctrl_t, pend_head_end), &none, 8) != APUS_OK) return APUS_ERROR;
+    /* my commit offset as a commit publish of my term: the follower's kernel follows it as far as it holds entries */
+    const uint64_t pc[2] = { mh.commit, r->cfg.term };
+    if (peer_write(r, peer, offsetof(apus_ctrl_t, pub_commit), pc, 16) != APUS_OK) return APUS_ERROR;
     if (own_write(r, offsetof(apus_ctrl_t, ack) + 8u * peer, &mine, 8) != APUS_OK) return APUS_ERROR;
     const uint64_t adj[3] = { sid, mh.end, mine };
     if (peer_write(r, peer, APUS_CTL_OFF + offsetof(apus_ctlwords_t, adj_end), &adj[1], 16) != APUS_OK) return APUS_ERROR;
@@ -1489,7 +1493,7 @@ extern "C" int apus_replica_set_role(apus_replica_t *r, uint8_t leader_idx, uint
             if (unc > (1u << 20)) return fail("too many uncommitted entries to take over");
         }
     }
-    c.next_idx = last + 1; c.published = last; c.committed = last - unc;
+    c.next_idx = last + 1; c.published = last; c.pub_seen = last; c.committed = last - unc;
     c.consumed = 0; c.committed_tickets = 0;
     c.hwm = L;                       /* treat every range as written before: prefill reads the log (zeros where it was never written) */
     for (int i = 0; i < 16; i++) { c.ack[i] = 0; c.apply_off[i] = h.head; c.fbeat[i] = 0; }   /* dare_server.c:1507-1510 */

@@ -430,9 +430,11 @@ __device__ void leader_commit_warp(const apus_devctx_t *__restrict__ cx)
     uint32_t spins = 0, hb_spins = 0;
     uint64_t last_hb = 0, hb_beat = globaltimer_ns() >> 10;   // beats keep growing across launches
     bool S_rec_ok = false;
-    volatile uint64_t *peer_commit = nullptr;
+    // commit publish into the follower's control block, stamped with my term: the follower's header `commit` is the
+    // follower's own (clamped to what it holds, I4), and a deposed leader's offsets are dropped by the term fence
+    uint64_t *peer_commit = nullptr;
     if (lane < N && lane != me && cx->peer[lane])
-        peer_commit = &reinterpret_cast<apus_loghdr_t *>(cx->peer[lane] + APUS_HDR_OFF)->commit;
+        peer_commit = reinterpret_cast<apus_ctrl_t *>(cx->peer[lane])->pub_commit;
 
     for (;;) {
         // every lane looks at one 16 B pair of the next four publish records (lane>>3 = record, lane&7 = pair)
@@ -449,6 +451,7 @@ __device__ void leader_commit_warp(const apus_devctx_t *__restrict__ cx)
             if (nvalid) {
                 published = __shfl_sync(0xffffffffu, rv, 8 * (nvalid - 1) + PR_CUM);
                 seen += nvalid;
+                if (lane == 0) st_relaxed_sys(&ctrl->pub_seen, published);
             }
             S_rec_ok = nvalid != 0;
         }
@@ -506,7 +509,7 @@ __device__ void leader_commit_warp(const apus_devctx_t *__restrict__ cx)
                 if (nc < 4) break;
             }
             if (any) {
-                if (peer_commit) st_relaxed_sys(peer_commit, off);          // dare_ibv_rc.c:1810
+                if (peer_commit) st_relaxed_sys_2x64(peer_commit, off, cx->term);   // dare_ibv_rc.c:1810
                 if (lane == 0) {
                     // {commit offset, committed tickets}: ONE 16 B store into pinned host memory -- this is what
                     // releases the proxy.c:160 spinners; a 16 B host load sees a consistent pair
@@ -1623,7 +1626,7 @@ __device__ void follower_main(const apus_devctx_t *__restrict__ cx)
     for (;;) {
         if (tid < 32) {
             // warp 0 polls: lane 0 the tail publish {end, entries|term} (one 16 B acquire load), lane 1 its certificate half,
-            // lane 2 the commit offset, lane 3 the heartbeat word
+            // lane 2 the commit publish {offset, term}, lane 3 the heartbeat word
             const int lane = tid;
             uint64_t e = 0, cumt = 0, c = 0, cert_start = 0;
             uint32_t done = 0, is_cert = 0;
@@ -1637,13 +1640,14 @@ __device__ void follower_main(const apus_devctx_t *__restrict__ cx)
                 uint4 spec = make_uint4(0, 0, 0, 0);
                 if (lane == 0) ld_acquire_sys_2x64(&ctrl->pub_end, x0, x1);
                 else if (lane == 1) ld_relaxed_sys_2x64(&ctrl->pub_csum, x0, x1);
-                else if (lane == 2) x0 = ld_relaxed_sys(&hdr->commit);
+                else if (lane == 2) ld_relaxed_sys_2x64(ctrl->pub_commit, x0, x1);
                 else if (lane == 3) x0 = ld_relaxed_sys(&ctrl->hb);
                 else if (lane < 16 && spec_lo + 16 <= L) spec = ld_relaxed_sys_v4(entries + spec_lo);
                 e = __shfl_sync(0xffffffffu, x0, 0); cumt = __shfl_sync(0xffffffffu, x1, 0);
                 const uint64_t csum = __shfl_sync(0xffffffffu, x0, 1);
                 cert_start = __shfl_sync(0xffffffffu, x1, 1);
                 c = __shfl_sync(0xffffffffu, x0, 2);
+                if (__shfl_sync(0xffffffffu, x1, 2) != cx->term) c = applied;     // term fence on the commit publish too
                 const uint64_t hbw = __shfl_sync(0xffffffffu, x0, 3);
                 // term fence: a publish stamped with another term (a deposed leader still storing) is not looked at
                 uint64_t cum = cumt & APUS_PUB_CUM_MASK;
@@ -1879,6 +1883,7 @@ __device__ void follower_main(const apus_devctx_t *__restrict__ cx)
                 }
                 applied = to;
                 if (tid == 0) {
+                    hdr->commit = applied;              // what this replica knows committed AND holds (I4)
                     if (!host_apply) {
                         hdr->apply = applied;           // library use: nothing replays the log on the host
                         st_relaxed_sys(&lctrl->apply_off[me], applied);

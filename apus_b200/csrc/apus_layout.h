@@ -28,7 +28,7 @@
  *   leader  -> follower.entries[range]       entry bytes           (replaces RDMA WRITE dare_ibv_rc.c:1606)
  *   leader  -> follower.index[..]            entry offsets, 4 B per entry
  *   leader  -> follower.ctrl.pub_{end,cum}   tail publish, 16 B    (dare_ibv_rc.c:1549-1573)
- *   leader  -> follower.hdr.commit           commit publish, 8 B   (dare_ibv_rc.c:1810)
+ *   leader  -> follower.ctrl.pub_commit      commit publish {offset, term}, 16 B (dare_ibv_rc.c:1810)
  *   follower-> leader.entries[e+28+idx]      reply byte, 1 B       (dare_ibv_rc.c:1833-1854)
  *   follower-> leader.ctrl.ack[idx]          ack word, 8 B         (the word the quorum ballot polls)
  *   follower-> leader.ctrl.apply_off[idx]    apply offset, 8 B     (push form of rc_get_remote_apply_offsets :1970)
@@ -94,7 +94,9 @@ typedef struct apus_ctrl {
     uint64_t auto_heads;         /* leader: HEAD entries appended by the device-side pruning rule */
     uint64_t pend_head_val;      /* follower: head carried by the last HEAD entry seen ... */
     uint64_t pend_head_end;      /* ... and the offset right after that entry (len = none) */
-    uint64_t pad0[3];
+    uint64_t pub_seen;           /* leader: entries published as the commit warp has seen them (stats only; `published`
+                                    follows the commit) */
+    uint64_t pad0[2];
     /* --- written by the LEADER into each follower's region --- */
     uint64_t fin_entries;        /* end of a launch: entries the leader has published in total */
     uint64_t fin_target;         /* ... and the launch (its ticket target) this refers to */
@@ -104,7 +106,10 @@ typedef struct apus_ctrl {
     uint64_t pub_csum;           /* self-certifying publish (APUS_PUB_CERT): checksum of the bytes [start, end), keyed
                                     with pub_cum ... */
     uint64_t pub_start;          /* ... and the offset of the (single) entry; one 16 B store, NO fence before either */
-    uint64_t pad2[4];
+    uint64_t pub_commit[2];      /* commit publish {leader's commit offset, term}: one 16 B store.  The follower drops
+                                    other terms, clamps the offset to what it holds (I4) and keeps the result in its
+                                    own header's `commit` */
+    uint64_t pad2[2];
     uint64_t hb;                 /* leader -> follower heartbeat: term << 48 | beat counter (dare_ibv_rc.c:868-958 writes
                                     the leader's SID into ctrl_data.hb[]); its own 64 B half line */
     uint64_t pad3[7];

@@ -1,9 +1,28 @@
 """Helpers for the GPU parity tests: run one request stream through the CUDA
 engine (via the C ABI) and through the CPU oracle, then compare everything
 observable (SURVEY.md s8c "Masking rule for parity")."""
+import ctypes as C
+
 import numpy as np
 
 import orc as O
+
+FOREVER = (1 << 64) - 1
+
+
+def launch_each(eng, reps, target=FOREVER):
+    """one launch per replica (followers first): a replica can then be stopped on its own even when several share a GPU"""
+    from apus_b200 import engine as E
+    for r in sorted(reps, key=lambda r: r.is_leader):
+        arr = (C.c_void_p * 1)(r.h)
+        E._ck(eng.lib().apus_replicas_launch(arr, 1, target), "apus_replicas_launch")
+
+
+def stop_each(eng, reps):
+    """stop the launches of `reps` (each launched on its own by launch_each)"""
+    from apus_b200 import engine as E
+    arr = (C.c_void_p * len(reps))(*[r.h for r in reps])
+    E._ck(eng.lib().apus_replicas_stop(arr, len(reps)), "apus_replicas_stop")
 
 
 def oracle_cluster(orc, n, length, stream, rules=O.RULES_ENGINE, prologue=True, leader=0, term=1):

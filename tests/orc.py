@@ -174,8 +174,24 @@ class Cluster:
     def prologue(self):
         return self.o.prologue(self.h)
 
-    def round(self):
-        self.o.round(self.h)
+    def round(self, live=None):
+        """One round of SIM(round) (oracle/cluster_sim.inc).  With `live` (follower indices), only those followers
+        are up: they receive, ack, get the commit offset pushed and apply; the others keep their state.  The steps run
+        in SIM(round)'s order, the commit scan once."""
+        if live is None:
+            self.o.round(self.h)
+            return
+        up = [i for i in range(self.n) if i == self.leader or i in set(live)]
+        self.leader_persist()
+        for i in up:
+            self.replicate(i)
+        for i in up:
+            self.follower_persist(i)
+        self.commit_scan()
+        for i in up:
+            self.push_commit(i)
+        for i in up:
+            self.apply(i)
 
     def offsets(self, i):
         out = (u64 * 8)()

@@ -110,6 +110,14 @@ def _run_once(n, nconn, nreq, plen, threads=1, prune=None, timeout=120, keep=Non
     removed = [i for i in range(n) if res[i].get("log_marks", {}).get("removals", 0)]
     if removed:
         raise Disturbed(f"the reference removed a server from the group while it ran (logs of {removed}); not a quiet run")
+    # a follower the leader never reached at start-up (it did not grant log access within the settle time) waits in vain
+    # for the leader's end and reports an empty log, while the other followers make the majority
+    lead_o = res[leaders[0]].get("offsets", {})
+    empty = [i for i in range(n) if i != leaders[0] and lead_o.get("end") != lead_o.get("len")
+             and res[i].get("offsets", {}).get("end") == res[i].get("offsets", {}).get("len")]
+    if empty:
+        raise Disturbed(f"followers {empty} hold an empty log while the leader holds entries (not reached at start-up); "
+                        "not a quiet run")
     led = sum(r.get("log_marks", {}).get("leaderships", 1 if r["leader"] else 0) for r in res)
     if led != 1:
         raise Disturbed(f"{led} leaderships in one run (a leader was deposed during start-up: one CONFIG entry per term); not a quiet run")

@@ -17,18 +17,8 @@ from test_gpu_parity import MODES, devices_for, eng, prune_both, check_replica_i
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(240)]
 
-FOREVER = (1 << 64) - 1
+FOREVER = EU.FOREVER
 F_NO_EXPRESS, F_HOST_APPLY, F_AUTOPRUNE, F_STATS = 0x20, 0x10, 0x4, 0x2
-
-
-def launch_each(eng, reps, target=FOREVER):
-    """one launch per replica (followers first): a replica can then be stopped on its own even when several share a GPU"""
-    import ctypes as C
-    from apus_b200 import engine as E
-    for r in sorted(reps, key=lambda r: r.is_leader):
-        arr = (C.c_void_p * 1)(r.h)
-        E._ck(eng.lib().apus_replicas_launch(arr, 1, target), "apus_replicas_launch")
-
 
 def closed_loop(g, stream, timeout_us=5_000_000):
     t = 0
@@ -364,7 +354,7 @@ def test_heartbeats_and_failure_detector(eng):
     is gone reports the suspicion within its timeout, not before."""
     n, L = 3, 1 << 20
     with eng.Group(n, devices=devices_for(eng, n), log_size=L, flags=F_STATS, hb_period_us=100, hb_timeout_us=20_000) as g:
-        launch_each(eng, g.replicas)
+        EU.launch_each(eng, g.replicas)
         g.leader.wait_committed(g.prologue())
         time.sleep(0.15)                                    # many timeouts' worth of beats
         for r in g.replicas[1:]:
@@ -401,6 +391,7 @@ def test_term_fence_ignores_a_deposed_leader(eng, orc):
             E._ck(eng.lib().apus_replicas_launch(arr, len(rs), FOREVER), "launch")
         lead = reps[0]
         stream = S.ragged_stream(200, 100, conns=2, seed=3)
+        fenced0 = reps[2].offsets()
         t = lead.submit(E.CONFIG, 0, 0, E.cid_image(n))
         for typ, clt, rid, payload in stream:
             t = lead.submit(typ, clt, rid, payload)
@@ -408,7 +399,11 @@ def test_term_fence_ignores_a_deposed_leader(eng, orc):
         time.sleep(0.05)
         assert reps[1].stats()["entries_acked"] == t
         assert reps[2].stats()["entries_acked"] == 0
-        assert reps[2].offsets()["end"] == L                # still the empty-log sentinel
+        fo = reps[2].offsets()
+        assert fo["end"] == L                               # still the empty-log sentinel
+        # the deposed leader's commit offsets are fenced off too: the follower's commit and apply stay where they were
+        assert (fo["commit"], fo["apply"]) == (fenced0["commit"], fenced0["apply"]), (fenced0, fo)
+        assert reps[1].offsets()["commit"] == lead.offsets()["commit"]
     finally:
         arr = (C.c_void_p * n)(*[r.h for r in reps])
         eng.lib().apus_replicas_stop(arr, n)
