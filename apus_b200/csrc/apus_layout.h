@@ -145,15 +145,13 @@ typedef struct apus_ctlwords {
 typedef struct apus_seq {
     uint64_t claimed_slots;      /* slots handed to workers so far (>= ctrl.consumed); compare-and-swap */
     uint64_t pad_c[15];
-    uint64_t place_seq;      uint64_t pad_d[15];   /* next claim allowed to place */
     uint64_t pub_turn[2];    uint64_t pad_e[14];   /* {next claim allowed to publish, next record number}: one 16 B word */
-    uint64_t pub_head;       uint64_t pad_f[15];   /* publish ring: next record written */
-    uint64_t pub_tail;       uint64_t pad_g[15];   /* ... next record the commit warp reads */
+    uint64_t pub_tail;       uint64_t pad_g[15];   /* publish ring: next record the commit warp reads */
     uint64_t workers_done;
     uint64_t abort_flag;
     uint64_t ready_epoch;        /* == devctx.epoch once worker 0 has reset the block */
     uint64_t pad_h[13];
-    /* placement state handed from claim to claim: three 16 B {stamp, value} pairs, each written
+    /* placement state handed from claim to claim: four 16 B {stamp, value} pairs, each written
      * with ONE 16 B store and read with one 16 B load.  stamp == the claim sequence number whose
      * turn it is: the hand-over needs no fence (a system/gpu fence is expensive and the turn is
      * the only serialized part of the leader) */
