@@ -1097,6 +1097,13 @@ struct LeaderProf {
 // claimed-slots counter.  The claimed range [slot0, slot0+n) is also the worker's place in the order: the place and
 // publish turns are stamped with slot numbers.  A lone request is taken by the express path right here; a claim for the
 // tile machine leaves with S->n_fetch > 0, a stop or an abort with S->finish.
+//
+// Every worker contends for the counter, so a claim costs as few dependent round trips as possible (DESIGN.md §3a): a
+// pass issues its loads together (counter, doorbell, claim-sizing averages, w0_idle, every 64th pass the abort flag),
+// then, only when there is something to claim, the compare-and-swap with an acquire re-read of the doorbell beside it.
+// A failed compare-and-swap returns the current counter: lane 0 decides the claim again from that value and the
+// doorbell already read, and retries at once.  That retry loop reads the abort flag; a stop and the watchdog are
+// checked by the passes around it, and the loop ends because every lost attempt moves the counter towards `t`.
 __device__ __forceinline__ void t0_claim(const apus_devctx_t *__restrict__ cx, LeaderShared *S, Express &X,
                                          uint64_t &xguess, uint4 &pf, uint64_t &pf_pos, uint64_t &last_progress,
                                          LeaderProf &P, const uint32_t wid, const int lane)
@@ -1127,16 +1134,20 @@ __device__ __forceinline__ void t0_claim(const apus_devctx_t *__restrict__ cx, L
             if (lane < 12) pf = ld_relaxed_sys_v4(entries + X.rec.end + 16ull * lane);
             pf_pos = X.rec.end;
         }
-        uint32_t ctl = 0;
-        uint64_t t = 0, w0i = 0;
+        // lane 0: one round trip of independent loads (the averages are small: their low 32 bits hold them); the
+        // doorbell is read relaxed here and with acquire next to the compare-and-swap
+        uint32_t ctl = 0, aes = 0, axb = 0;
+        uint64_t t = 0, w0i = 0, ab = 0;
         if (lane == 0) {
-            if ((spins & 0x3fu) == 0 && ld_relaxed_sys(&seq->abort_flag)) ctl = 1;
-            // (relaxed: a doorbell that shows requests is re-read with acquire before anything is fetched)
+            if ((spins & 0x3fu) == 0) ab = ld_relaxed_sys(&seq->abort_flag);
             t = cx->doorbell_relay ? ld_relaxed_sys(&seq->doorbell) : ld_relaxed_sys(cx->sub_tail);
             claimed = ld_relaxed_sys(&seq->claimed_slots);
-            if (claimed >= cx->target) ctl = 1;
             if (wid != 0) w0i = ld_relaxed_sys(&seq->w0_idle);
-            if (t > claimed) t = cx->doorbell_relay ? ld_acquire_gpu(&seq->doorbell) : ld_acquire_sys(cx->sub_tail);
+            aes = ld_relaxed_sys_u32(&seq->avg_es); axb = ld_relaxed_sys_u32(&seq->avg_xb);
+            // worker 0 waits for its slot poll (a PCIe round trip) in every pass anyway: there, a doorbell that shows
+            // requests is re-read with acquire at once, under the poll, and not beside the compare-and-swap
+            if (poll_slot && t > claimed) t = cx->doorbell_relay ? ld_acquire_gpu(&seq->doorbell) : ld_acquire_sys(cx->sub_tail);
+            if (ab || claimed >= cx->target) ctl = 1;
         }
         ctl = __shfl_sync(0xffffffffu, ctl, 0);
         claimed = __shfl_sync(0xffffffffu, claimed, 0);
@@ -1159,40 +1170,61 @@ __device__ __forceinline__ void t0_claim(const apus_devctx_t *__restrict__ cx, L
         // lone requests belong to worker 0 while it is polling (express path)
         if (avail == 1 && wid != 0 && w0i) avail = 0;
         if (avail) {
-            const uint64_t room = cx->target - claimed;
-            if (avail > room) avail = room;
             uint32_t nn = 0, won = 0;
             if (lane == 0) {
-                // share a shallow queue between the workers instead of one big tile
-                uint64_t want = (avail + cx->n_workers - 1) / cx->n_workers;
-                if (want < 32) want = avail < 32 ? avail : 32;
-                // a claim should fit ONE tile image / staging buffer (else it is placed in pieces
-                // while holding the place turn, which serializes the workers)
-                uint64_t aes = ld_relaxed_sys(&seq->avg_es), axb = ld_relaxed_sys(&seq->avg_xb);
+                // a claim should fit ONE tile image / staging buffer (else it is placed in pieces while holding the
+                // place turn, which serializes the workers)
                 if (aes < 64) aes = 128;
-                uint64_t fit = (APUS_LEADER_IMG_BYTES - 256u) / aes;
-                if (axb) { const uint64_t xf = APUS_LEADER_EXT_BYTES / axb; if (xf < fit) fit = xf; }
+                uint32_t fit = (APUS_LEADER_IMG_BYTES - 256u) / aes;
+                if (axb) { const uint32_t xf = APUS_LEADER_EXT_BYTES / axb; if (xf < fit) fit = xf; }
                 if (fit < 1) fit = 1;
-                if (want > fit) want = fit;
-                nn = want > MAXB ? MAXB : (uint32_t)want;
-                won = atomicCAS(reinterpret_cast<unsigned long long *>(&seq->claimed_slots), (unsigned long long)claimed,
-                                (unsigned long long)(claimed + nn)) == (unsigned long long)claimed;
-            }
-            nn = __shfl_sync(0xffffffffu, nn, 0);
-            won = __shfl_sync(0xffffffffu, won, 0);
-            if (!won) continue;                   // somebody else took these slots: look again
-            if (nn == 1 && express_on) {
-                const int rc = leader_express(cx, S, X, claimed, sv, slot_ok, smem_raw + L_IMG_OFF, lane, pf, pf_pos);
-                if (rc == 0) {
-                    xguess = claimed + 1; last_progress = globaltimer_ns();
-                    if (P.on) { P.tn[5]++; P.ph[7]++; for (int q = 0; q < 5; q++) P.ph[1 + q] += X.dt[q]; }
-                    continue;
+                const uint32_t cap = fit > MAXB ? MAXB : fit;
+                // claim; a lost compare-and-swap returns the counter: decide again from it and the doorbell already
+                // read.  This loop ends: every lost attempt moved the counter towards `t`.  It reads the abort flag
+                // every 64 attempts; a stop and the watchdog are looked at by the passes around it.  (`lost`, not
+                // `spins`: the pass counter must stay the same in every lane, the stop check below is warp-wide.)
+                for (uint32_t lost = 0;; lost++) {
+                    const uint64_t room = cx->target - claimed;
+                    if (avail > room) avail = room;
+                    // share a shallow queue between the workers instead of one big tile
+                    uint64_t want = (avail + cx->n_workers - 1) / cx->n_workers;
+                    if (want < 32) want = avail < 32 ? avail : 32;
+                    nn = want > cap ? cap : (uint32_t)want;
+                    const uint64_t was = atomicCAS(reinterpret_cast<unsigned long long *>(&seq->claimed_slots),
+                                                   (unsigned long long)claimed, (unsigned long long)(claimed + nn));
+                    // the doorbell again, with acquire, in flight with the compare-and-swap: it shows at least `t` and
+                    // orders the fetch of the claimed slots after it (not for a lone request that only the slot poll
+                    // has shown: its stamp is what publishes it; not for worker 0, which has read `t` with acquire)
+                    if (t > claimed && !poll_slot) (void)(cx->doorbell_relay ? ld_acquire_gpu(&seq->doorbell) : ld_acquire_sys(cx->sub_tail));
+                    if (was == claimed) { won = 1; break; }
+                    claimed = was;
+                    if (claimed >= cx->target) break;
+                    if ((lost & 0x3fu) == 0x3fu && ld_relaxed_sys(&seq->abort_flag)) break;
+                    avail = t > claimed ? t - claimed : 0;
+                    // a lone request: worker 0 waits for its slot poll (the next pass), the others leave it to worker 0
+                    if (avail == 1 && ((poll_slot && express_on) || (wid != 0 && w0i))) avail = 0;
+                    if (!avail) break;
                 }
-                if (rc == 2) { fin = 1; break; }
-                // rc == 1: the tile machine places this claim; the cached placement state is still what the records hold
             }
-            n = nn;
-            break;
+            won = __shfl_sync(0xffffffffu, won, 0);
+            claimed = __shfl_sync(0xffffffffu, claimed, 0);
+            if (won) {
+                nn = __shfl_sync(0xffffffffu, nn, 0);
+                if (X.hold && claimed != X.next_seq) express_release(seq, X, lane);   // won after a lost attempt
+                if (nn == 1 && express_on) {
+                    const int rc = leader_express(cx, S, X, claimed, sv, slot_ok && claimed == sv_for, smem_raw + L_IMG_OFF,
+                                                  lane, pf, pf_pos);
+                    if (rc == 0) {
+                        xguess = claimed + 1; last_progress = globaltimer_ns();
+                        if (P.on) { P.tn[5]++; P.ph[7]++; for (int q = 0; q < 5; q++) P.ph[1 + q] += X.dt[q]; }
+                        continue;
+                    }
+                    if (rc == 2) { fin = 1; break; }
+                    // rc == 1: the tile machine places this claim; the cached placement state is still what the records hold
+                }
+                n = nn;
+                break;
+            }
         }
         if ((++spins & 0x1ffu) == 0) {
             // stop / watchdog (the abort flag is not raised on a stop: this worker holds no turn)

@@ -38,6 +38,10 @@ __global__ void k_single(volatile uint64_t *target, uint8_t *buf, int mode, int 
         else if (mode == 13) { acc += gt(); }
         else if (mode == 14) { acc += clock64(); }
         else if (mode == 12) { st16(buf + ((i & 63) * 512) + threadIdx.x * 16, make_uint4(i, i, i, i)); }
+        else if (mode == 15 && threadIdx.x == 0) {
+            const uint64_t o = atomicCAS((unsigned long long *)target, acc, acc + 1);
+            acc = o == acc ? acc + 1 : o;
+        }
     }
     uint64_t t1 = gt();
     long long c1 = clock64();
@@ -133,6 +137,64 @@ __global__ void k_interfere(volatile uint64_t *target, uint8_t *buf, int mode, i
     }
 }
 
+// claim counter (the leader's T0, DESIGN.md §3a): k CTAs take claims of `step` slots from one counter until `total`
+// slots are claimed.  w[0] = counter, w[16] = doorbell (== total), w[32..33] = claim-sizing words, each on its own line.
+// proto 0: load counter + doorbell, re-read the doorbell with acquire, load the sizing words, then the compare-and-swap;
+//          a lost compare-and-swap starts over.
+// proto 1: the sequence of t0_claim: counter, doorbell (relaxed) and sizing words in one round trip, then the
+//          compare-and-swap with an acquire re-read of the doorbell issued beside it; a lost compare-and-swap is retried
+//          at once from the value it returned (each retry again with its acquire).
+__global__ void k_claim(uint64_t *w, int proto, uint64_t total, uint64_t step, uint64_t *out)
+{
+    if (threadIdx.x != 0) return;
+    unsigned long long *ctr = (unsigned long long *)w;
+    uint64_t won = 0, tries = 0;
+    const uint64_t t0 = gt();
+    for (;;) {
+        uint64_t c, t, a, b;
+        if (proto == 0) {
+            t = ldr(w + 16); c = ldr(w);
+            if (t > c) asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(t) : "l"(w + 16) : "memory");
+            if (c >= total) break;
+            a = ldr(w + 32); b = ldr(w + 33);
+            const uint64_t nn = step + ((a + b) & 1);   // (a, b are 0: the sizing loads are a dependency, as in T0)
+            tries++;
+            if (atomicCAS(ctr, c, c + nn) == c) won++;
+        } else {
+            c = ldr(w); t = ldr(w + 16); a = ldr(w + 32); b = ldr(w + 33);
+            const uint64_t nn = step + ((a + b) & 1);
+            while (c < t && c < total) {
+                tries++;
+                const uint64_t was = atomicCAS(ctr, c, c + nn);
+                uint64_t ta;
+                asm volatile("ld.acquire.gpu.global.u64 %0, [%1];" : "=l"(ta) : "l"(w + 16) : "memory");
+                if (was == c) { won++; break; }
+                c = was;
+            }
+            if (c >= total) break;
+        }
+    }
+    const uint64_t t1 = gt();
+    atomicAdd((unsigned long long *)out, (unsigned long long)won);
+    atomicAdd((unsigned long long *)out + 1, (unsigned long long)tries);
+    atomicMax((unsigned long long *)out + 2, (unsigned long long)(t1 - t0));
+}
+
+static void run_claim(uint64_t *dflag, int proto, int k)
+{
+    const uint64_t total = 1ull << 20, step = 256;
+    uint64_t *o; CK(cudaMallocManaged(&o, 64));
+    for (int rep = 0; rep < 2; rep++) {                     // first launch warms up
+        CK(cudaMemset(dflag, 0, 4096)); memset(o, 0, 64);
+        CK(cudaMemcpy(dflag + 16, &total, 8, cudaMemcpyHostToDevice));
+        k_claim<<<k, 32>>>(dflag, proto, total, step, o); CK(cudaDeviceSynchronize());
+    }
+    printf("claims, %2d CTAs, %s: %.2f claims/us, %.2f compare-and-swaps per claim\n", k,
+           proto == 0 ? "load/acquire/load/CAS, restart on loss" : "one load round, CAS + acquire, retry from returned value",
+           (double)o[0] * 1000.0 / (double)o[2], (double)o[1] / (double)o[0]);
+    cudaFree(o);
+}
+
 static void run_interfere(volatile uint64_t *target, uint8_t *buf, const char *name, int mode, int nblk)
 {
     uint64_t *ns; int *stop;
@@ -180,6 +242,12 @@ int main()
     printf("read %%globaltimer: "); printf("%.1f ns\n", run_single(dflag, dbuf, 13, 20000, 32));
     printf("read clock64: "); printf("%.1f ns\n", run_single(dflag, dbuf, 14, 20000, 32));
     printf("warp 512 B local stores only (issue rate): "); printf("%.1f ns\n", run_single(dflag, dbuf, 12, 20000, 32));
+    CK(cudaMemset(dflag, 0, 4096));
+    printf("atomicCAS local L2 (dependent chain): "); printf("%.1f ns\n", run_single(dflag, dbuf, 15, 20000, 32));
+    CK(cudaMemset(dflag, 0, 4096));
+    for (int proto = 0; proto < 2; proto++)
+        for (int k = 1; k <= 16; k *= 4) run_claim(dflag, proto, k);
+    CK(cudaMemset(dflag, 0, 4096));
     run_interfere(dflag, dbuf, "do nothing", 0, 1);
     run_interfere(dflag, dbuf, "loop fence.sc.sys", 1, 2);
     run_interfere(dflag, dbuf, "loop fence.sc.sys", 1, 8);
