@@ -195,6 +195,7 @@ typedef struct apus_pubrec {
 #define APUS_SLOT_BYTES   128u
 #define APUS_SLOT_INLINE  80u
 #define APUS_CSLOT_BYTES  96u     /* a slot as the leader keeps it in shared memory: descriptor + inline image */
+/* (how a slot is written -- image placement, the WRAP rule, descriptor and stamps -- is apus_slot.h) */
 #define APUS_SLOT_OFF_MASK 0x00ffffffu
 #define APUS_SLOT_TYPE_SHIFT 24
 #define APUS_SLOT_TYPE_MASK 0x1fu
@@ -227,7 +228,9 @@ typedef struct apus_hostwords {
     volatile uint64_t committed_tickets; /* ... so a 16 B host load sees a consistent pair */
     volatile uint64_t consumed;          /* kernel -> host (ring space) */
     volatile uint64_t last_commit_ns;    /* kernel -> host: %globaltimer of the latest commit */
-    uint64_t pad1[12];
+    volatile uint64_t dev_rejected;      /* packing kernel -> host: requests of device batches written as NOOPs ... */
+    volatile uint64_t dev_first_rejected;/* ... and the ticket of the first of them (0 = none) */
+    uint64_t pad1[10];
     volatile uint32_t stop;              /* host -> kernel */
     uint32_t pad2[31];
     volatile uint64_t host_apply;        /* host -> follower kernel (APUS_FLAG_HOST_APPLY): offset up to which the

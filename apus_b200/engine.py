@@ -62,6 +62,7 @@ EXPORTS = [
     "apus_ctl_read", "apus_ctl_set_sid", "apus_ctl_reset_votes", "apus_ctl_clear_vote_request", "apus_ctl_send_vote_request",
     "apus_ctl_send_vote_ack", "apus_ctl_last_entry", "apus_ctl_adjust_follower", "apus_replica_set_role",
     "apus_replica_disconnect", "apus_follower_beats", "apus_device_numa_node", "apus_group_multicast", "apus_ctl_heartbeat",
+    "apus_submit_device", "apus_device_submit_status", "apus_stream_wait_committed", "apus_committed_word",
 ]
 
 
@@ -114,6 +115,11 @@ def load_library(path=LIB_PATH):
         L.apus_leader_suspect.restype = u64
         L.apus_last_commit_ns.argtypes = [vp]
         L.apus_last_commit_ns.restype = u64
+        L.apus_submit_device.argtypes = [vp, u32, vp, vp, vp, vp, vp, C.c_size_t, vp, C.POINTER(u64)]
+        L.apus_device_submit_status.argtypes = [vp, C.POINTER(u64), C.POINTER(u64)]
+        L.apus_stream_wait_committed.argtypes = [vp, u64, vp]
+        L.apus_committed_word.argtypes = [vp]
+        L.apus_committed_word.restype = vp
     _lib = L
     return L
 
@@ -215,6 +221,68 @@ class Replica:
         t = u64()
         _ck(lib().apus_submit_synth(self.h, n, typ, conn, first_req_id, length, seed, C.byref(t)), "apus_submit_synth")
         return int(t.value)
+
+    def _stream(self, stream):
+        import torch
+        if stream is None:
+            return torch.cuda.current_stream(self.device)
+        if stream.device != torch.device("cuda", self.device):
+            raise ApusError(f"stream on {stream.device}, the leader is on cuda:{self.device}")
+        return stream
+
+    def submit_device(self, types, conns, req_ids, lens, payloads, stream=None):
+        """n requests whose fields are CUDA tensors on the leader's device, packed into the HBM submission ring in
+        `stream` order (apus_submit_device): types uint8 [n], conns int16/uint16 [n], req_ids int64 [n] (as uint64),
+        lens int16/uint16/int32 [n], payloads uint8 [n, stride].  All contiguous.  Returns the first ticket; the
+        tensors may be overwritten or freed in stream order as soon as this returns.  Invalid requests (a type that
+        is not CSM/CONNECT/SEND/CLOSE, len > stride) become NOOP entries, see device_submit_status()."""
+        import torch
+        dev = torch.device("cuda", self.device)
+        if payloads is None or not isinstance(payloads, torch.Tensor) or payloads.dim() != 2:
+            raise ApusError("submit_device: payloads must be a 2-D uint8 CUDA tensor [n, stride]")
+        n, stride = payloads.shape
+        spec = (("types", types, (torch.uint8,)), ("conns", conns, (torch.int16, torch.uint16)),
+                ("req_ids", req_ids, (torch.int64,)), ("lens", lens, (torch.int16, torch.uint16, torch.int32)),
+                ("payloads", payloads, (torch.uint8,)))
+        for name, t, dtypes in spec:
+            if not isinstance(t, torch.Tensor):
+                raise ApusError(f"submit_device: {name} must be a torch tensor")
+            if t.device != dev:
+                raise ApusError(f"submit_device: {name} is on {t.device}, the leader is on {dev}")
+            if t.dtype not in dtypes:
+                raise ApusError(f"submit_device: {name} has dtype {t.dtype}, expected one of {dtypes}")
+            if t.shape[0] != n or (name != "payloads" and t.dim() != 1):
+                raise ApusError(f"submit_device: {name} has shape {tuple(t.shape)}, expected [{n}]" +
+                                (f" x {stride}" if name == "payloads" else ""))
+            if not t.is_contiguous():
+                raise ApusError(f"submit_device: {name} is not contiguous")
+        s = self._stream(stream)
+        if lens.dtype == torch.int32:
+            # the ABI takes uint16 lengths: a length outside [0, stride] must stay > stride after the narrowing
+            if stride >= 0xFFFF:
+                raise ApusError("submit_device: int32 lengths need stride < 65535 (use uint16 lengths)")
+            with torch.cuda.stream(s):
+                lens = torch.where((lens >= 0) & (lens <= stride), lens, 0xFFFF).to(torch.int16)
+        t = u64()
+        _ck(lib().apus_submit_device(self.h, n, types.data_ptr(), conns.data_ptr(), req_ids.data_ptr(), lens.data_ptr(),
+                                     payloads.data_ptr() if stride else None, stride, s.cuda_stream, C.byref(t)),
+            "apus_submit_device")
+        return int(t.value)
+
+    def device_submit_status(self):
+        """(requests of device batches written as NOOPs, ticket of the first of them or 0)"""
+        rej, first = u64(), u64()
+        _ck(lib().apus_device_submit_status(self.h, C.byref(rej), C.byref(first)), "apus_device_submit_status")
+        return int(rej.value), int(first.value)
+
+    def wait_committed_on_stream(self, ticket, stream=None):
+        """make `stream` (default: the current stream of the leader's device) wait until `ticket` is committed"""
+        s = self._stream(stream)
+        _ck(lib().apus_stream_wait_committed(self.h, ticket, s.cuda_stream), "apus_stream_wait_committed")
+
+    def committed_word(self):
+        """device-visible address of the committed-tickets word (pinned, mapped)"""
+        return int(lib().apus_committed_word(self.h) or 0)
 
     def release(self, ticket):
         _ck(lib().apus_submit_release(self.h, ticket), "apus_submit_release")
@@ -428,6 +496,14 @@ class Group:
         t0 = self.leader.submit_batch(types, conns, req_ids, lens, payloads, length)
         self.tickets = t0 + n_req - 1
         return self.tickets
+
+    def submit_device(self, types, conns, req_ids, lens, payloads, stream=None):
+        """Replica.submit_device on the leader; keeps `tickets` up to date so that run() covers the batch."""
+        n = payloads.shape[0]
+        t0 = self.leader.submit_device(types, conns, req_ids, lens, payloads, stream)
+        if n:
+            self.tickets = t0 + n - 1
+        return t0
 
     def run(self, timeout_ms=60_000):
         """Launch for everything submitted so far and wait until it is committed everywhere."""

@@ -61,7 +61,8 @@ extern "C" {
 
 /* where the leader's submission ring lives */
 #define APUS_RING_HOST_MAPPED 0   /* pinned host memory, read by the kernel over PCIe */
-#define APUS_RING_DEVICE      1   /* HBM; the host fills it with cudaMemcpyAsync batches */
+#define APUS_RING_DEVICE      1   /* HBM; the host fills it with cudaMemcpyAsync batches, or a kernel does
+                                     (apus_submit_synth, apus_submit_device) */
 
 /* apus_config_t.flags */
 #define APUS_F_FENCED_ACK   0x1u  /* follower: reply bytes visible before the ack word; off = ack as soon as
@@ -192,6 +193,29 @@ int  apus_submit_uniform(apus_replica_t *leader, uint32_t n, uint8_t type, uint1
 int  apus_submit_synth(apus_replica_t *leader, uint32_t n, uint8_t type, uint16_t connection_id,
                        uint64_t first_req_id, uint16_t len, uint32_t seed, uint64_t *first_ticket);
 uint8_t apus_synth_byte(uint32_t seed, uint64_t req_id, uint32_t k);
+/* Requests in device memory (APUS_RING_DEVICE only), packed into the HBM submission ring by a kernel in stream order.
+ * The five arrays are device memory on the leader's GPU; payload k is at payloads + k*stride (payloads may be NULL
+ * when stride is 0).  `stream` is a cudaStream_t (NULL = the legacy default stream).  Returns once the work is
+ * enqueued, without synchronising the host:
+ *   - tickets are decided here: *first_ticket .. *first_ticket + n - 1, in log order like every other submit;
+ *   - the payload ring reserves the worst case, n * round16(2 + stride) bytes (nothing when 2 + stride <= 80), and
+ *     frees it when the whole batch has been consumed;
+ *   - the packing runs after everything enqueued on `stream` before the call, and `stream` waits for the packing, so
+ *     the arrays may be overwritten or freed in stream order as soon as the call returns;
+ *   - host submissions that follow are ordered behind the packing, so their own synchronisation now also waits for
+ *     whatever the caller's stream ran before the batch;
+ *   - unless apus_submit_defer is on, the doorbell is raised to *first_ticket + n - 1 after the packing.
+ * A request whose type is not CSM, CONNECT, SEND or CLOSE, or whose len exceeds stride, is written as the NOOP that
+ * apus_submit(APUS_NOOP, conn, req_id, NULL, 0) would write at its ticket, and counted (apus_device_submit_status).
+ * APUS_RETRY, with nothing reserved, when the slot ring or the payload ring has no room now; APUS_ERROR on a follower,
+ * without a device ring, for a null array, or for a batch that could never fit (n > ring_slots, or a reservation
+ * larger than ring_bytes). */
+int  apus_submit_device(apus_replica_t *leader, uint32_t n, const uint8_t *types, const uint16_t *connection_ids,
+                        const uint64_t *req_ids, const uint16_t *lens, const void *payloads, size_t stride,
+                        void *stream, uint64_t *first_ticket);
+/* requests of device batches rejected so far (written as NOOPs) and the ticket of the first of them (0 = none); a
+ * batch is counted once its packing has run (e.g. after synchronising the stream it was submitted on) */
+int  apus_device_submit_status(apus_replica_t *leader, uint64_t *rejected, uint64_t *first_rejected_ticket);
 /* make everything submitted so far visible to the kernel (doorbell); apus_submit*
  * ring it themselves unless the replica was put in deferred mode */
 int  apus_submit_defer(apus_replica_t *leader, int defer);
@@ -208,6 +232,17 @@ uint64_t apus_committed_tickets(apus_replica_t *leader);
 int  apus_progress(apus_replica_t *r, uint64_t *offset, uint64_t *count);
 /* spin until ticket is committed; APUS_RETRY on timeout */
 int  apus_wait_committed(apus_replica_t *leader, uint64_t ticket, int64_t timeout_us);
+/* Make `stream` (a cudaStream_t on the leader's GPU) wait, without the host, until `ticket` is committed: one
+ * cuStreamWaitValue64 (>=) on the committed-tickets word the commit warp keeps in pinned, mapped memory.  Needs
+ * CU_DEVICE_ATTRIBUTE_CAN_USE_64_BIT_STREAM_MEM_OPS (APUS_ERROR without it; there is no spin-kernel fallback).  A wait
+ * on a ticket that never commits while the replica lives stays pending.  apus_replica_destroy releases pending waits
+ * before it frees the word: it stops the kernels, raises the word to at least every ticket waited on and waits for the
+ * streams to pass their waits.  The word cannot tell such a release from a commit; the caller knows it destroyed the
+ * replica. */
+int  apus_stream_wait_committed(apus_replica_t *leader, uint64_t ticket, void *stream);
+/* device-visible address of that word (tickets committed; pinned and mapped, so the same address works in host and
+ * device code), for kernels that look at the commit count themselves */
+const volatile uint64_t *apus_committed_word(apus_replica_t *leader);
 
 /* n requests of payload_len bytes, ONE in flight at a time: submit, spin until committed
  * (what a proxy thread does, proxy.c:108-161); lat_ns[i] = host-clock nanoseconds of request i */
