@@ -210,6 +210,9 @@ struct LeaderShared {
     uint32_t static_cut;       // first k > 0 whose payload image restarted the payload ring (else n_fetch)
     uint32_t first_ext_all;    // first entry with an external payload image (else 0xffffffff)
     uint32_t host_head_k;      // last HEAD entry submitted by the host in this batch (else 0xffffffff): it carries the new head
+    // the batch's descriptors, reduced while they are fetched (t1_fetch) and turned into the words above by t1_scan
+    uint32_t r_es_min, r_es_max, r_xb_min, r_xb_max, r_cut, r_fext, r_hh1;
+    uint32_t part_es[MAXB / 32], part_xb[MAXB / 32];   // per-32-entry totals of the CTA-wide scan (non-uniform batches)
     uint64_t idx_base;         // idx of an entry = idx_base + its 1-based position in the placement order
     uint8_t  ty[MAXB];
     uint8_t  flg[MAXB];        // bit0 EXT, bit1 WRAP
@@ -226,6 +229,7 @@ struct LeaderShared {
     uint64_t ext_base, auto_head_val, a, b, idx0, cum_after, new_end, tail_after, hwm_after;
     uint8_t  *peer_entries[APUS_MAX_SERVERS];
     uint32_t *peer_index[APUS_MAX_SERVERS];
+    uint64_t prof_ph[8], prof_tn[8];  // worker 0's profile (LeaderProf), thread 0 alone
 };
 
 #define LS_BYTES ((sizeof(LeaderShared) + 127u) & ~127u)
@@ -233,6 +237,7 @@ struct LeaderShared {
 #define L_EXT_OFF   (L_SLOTS_OFF + MAXB * APUS_CSLOT_BYTES)
 #define L_IMG_OFF   (L_EXT_OFF + APUS_LEADER_EXT_BYTES)
 #define L_TOTAL     (L_IMG_OFF + APUS_LEADER_IMG_BYTES + 16)
+static_assert(L_TOTAL <= 232448u, "leader shared memory exceeds the sm_90 opt-in limit per CTA (227 KiB)");
 
 struct FollowerShared {
     uint32_t off[APUS_FOLLOWER_WIN_BYTES / 64 + 8];   // entry offsets found in the window (relative to win_lo)
@@ -384,51 +389,82 @@ __device__ __noinline__ void cta_fetch_chunks(uint8_t *dst, const uint8_t *src, 
     for (; c < nchunks; c += nthr) reinterpret_cast<uint4 *>(dst)[c] = ld_relaxed_sys_v4(src + 16ull * c);
 }
 
-// the descriptor chunk of a slot -> compact per-entry arrays
-__device__ __forceinline__ void note_desc(LeaderShared *S, uint32_t k, const uint4 v)
+// What T2 needs to know about the whole fetched batch, reduced by every producer thread over the descriptors it
+// fetched (t1_fetch) and then over the CTA: whether every entry has the same stride and staged size (then the prefix
+// sums are closed-form), the first payload-ring restart, the first external image and the last host HEAD entry.
+struct DescReduce {
+    uint32_t es_min, es_max, xb_min, xb_max, cut, fext, hh1;
+    __device__ __forceinline__ void init()
+    {
+        es_min = xb_min = cut = fext = 0xffffffffu;
+        es_max = xb_max = hh1 = 0;
+    }
+};
+
+// the descriptor chunk of entry k -> compact per-entry arrays, and into the thread's reduction
+__device__ __forceinline__ void note_desc(LeaderShared *S, DescReduce &R, uint32_t k, const uint4 v)
 {
     const uint32_t to = v.z, ty = (to >> APUS_SLOT_TYPE_SHIFT) & APUS_SLOT_TYPE_MASK, len = v.w & 0xffffu;
+    const uint32_t es = entry_stride(ty, len), xb = (to & APUS_SLOT_EXT) ? ((data_bytes(ty, len) + 15u) & ~15u) : 0u;
     S->ty[k] = (uint8_t)ty;
     S->flg[k] = (uint8_t)(((to & APUS_SLOT_EXT) ? 1u : 0u) | ((to & APUS_SLOT_WRAP) ? 2u : 0u));
-    S->es[k] = entry_stride(ty, len);
-    S->xb[k] = (to & APUS_SLOT_EXT) ? ((data_bytes(ty, len) + 15u) & ~15u) : 0u;
+    S->es[k] = es;
+    S->xb[k] = xb;
+    R.es_min = min(R.es_min, es); R.es_max = max(R.es_max, es);
+    R.xb_min = min(R.xb_min, xb); R.xb_max = max(R.xb_max, xb);
+    if (k > 0 && (to & APUS_SLOT_WRAP)) R.cut = min(R.cut, k);
+    if (to & APUS_SLOT_EXT) R.fext = min(R.fext, k);
+    if (ty == T_HEAD) R.hh1 = max(R.hh1, k + 1u);
 }
 
 // fetch `cnt` slots starting at ring slot `s` into shared slot `k0` onward.  A 128 B ring slot is kept as a
 // 96 B compact slot: its two stamp chunks (3 and 7) are neither loaded nor stored, so that the inline image
-// is contiguous in shared memory (and a quarter of the PCIe / HBM read traffic is saved).
+// is contiguous in shared memory (and a quarter of the PCIe / HBM read traffic is saved).  8 loads in flight per
+// thread: a 512-slot claim is 3072 chunks, one round for every producer thread and a second for a few.
 __device__ __noinline__ void cta_fetch_slots(LeaderShared *S, uint8_t *slots, const apus_slot_t *ring, uint64_t s, uint32_t k0,
                                                 uint32_t cnt, int tid)
 {
+    DescReduce R;
+    R.init();
     const uint8_t *src = reinterpret_cast<const uint8_t *>(ring + s);
     uint8_t *dst = slots + (size_t)k0 * APUS_CSLOT_BYTES;
     const uint32_t nq = cnt * 6u;                                  // compact chunks
-    uint32_t q = (tid >= 32) ? tid - 32 : tid + NT - 32;           // warp 1 takes the first chunks (warp 0 is busy with the turns)
-#define SRC_OF(qq, kk, rr) const uint32_t kk = (qq) / 6u, rr = (qq) - 6u * kk; const uint8_t *p_##qq = src + (size_t)kk * APUS_SLOT_BYTES + 16u * (rr < 3u ? rr : rr + 1u)
-    for (; q + 3u * NT < nq; q += 4u * NT) {
-        const uint32_t q0 = q, q1 = q + NT, q2 = q + 2u * NT, q3 = q + 3u * NT;
-        SRC_OF(q0, ka, ra); SRC_OF(q1, kb, rb); SRC_OF(q2, kc, rc); SRC_OF(q3, kd, rd);
-        const uint4 v0 = ld_relaxed_sys_v4(p_q0);
-        const uint4 v1 = ld_relaxed_sys_v4(p_q1);
-        const uint4 v2 = ld_relaxed_sys_v4(p_q2);
-        const uint4 v3 = ld_relaxed_sys_v4(p_q3);
-        reinterpret_cast<uint4 *>(dst)[q0] = v0;
-        reinterpret_cast<uint4 *>(dst)[q1] = v1;
-        reinterpret_cast<uint4 *>(dst)[q2] = v2;
-        reinterpret_cast<uint4 *>(dst)[q3] = v3;
-        if (ra == 0) note_desc(S, k0 + ka, v0);
-        if (rb == 0) note_desc(S, k0 + kb, v1);
-        if (rc == 0) note_desc(S, k0 + kc, v2);
-        if (rd == 0) note_desc(S, k0 + kd, v3);
+    // warp 1 takes the first chunks (warp 0 is busy with the turns).  NT is a multiple of 6: a thread's chunks are
+    // all the same chunk of their slots, so only the threads of the descriptor chunks decode descriptors.
+    const uint32_t q0 = (tid >= 32) ? tid - 32 : tid + NT - 32;
+    const bool desc = (q0 % 6u) == 0;
+    for (uint32_t q = q0; q < nq; q += 8u * NT) {
+        uint4 v[8];
+#pragma unroll
+        for (uint32_t i = 0; i < 8; i++) {
+            // zeroed first: a register that a predicated load leaves undefined on the other path makes ptxas keep the
+            // eight values in local memory, one load after the other (issuing the surplus loads at a clamped address
+            // instead costs real reads -- over PCIe, hundreds of them at one host address)
+            const uint32_t qi = q + i * NT, k = qi / 6u, r = qi - 6u * k;
+            v[i] = make_uint4(0, 0, 0, 0);
+            if (qi < nq) v[i] = ld_relaxed_sys_v4(src + (size_t)k * APUS_SLOT_BYTES + 16u * (r < 3u ? r : r + 1u));
+        }
+#pragma unroll
+        for (uint32_t i = 0; i < 8; i++) {
+            const uint32_t qi = q + i * NT;
+            if (qi < nq) {
+                reinterpret_cast<uint4 *>(dst)[qi] = v[i];
+                if (desc) note_desc(S, R, k0 + qi / 6u, v[i]);
+            }
+        }
     }
-    for (; q < nq; q += NT) {
-        const uint32_t q0 = q;
-        SRC_OF(q0, ka, ra);
-        const uint4 v = ld_relaxed_sys_v4(p_q0);
-        reinterpret_cast<uint4 *>(dst)[q0] = v;
-        if (ra == 0) note_desc(S, k0 + ka, v);
+    // each warp folds its lanes', lane 0 folds the warp's into the r_* words (which t0_claim reset)
+    R.es_min = __reduce_min_sync(0xffffffffu, R.es_min); R.es_max = __reduce_max_sync(0xffffffffu, R.es_max);
+    R.xb_min = __reduce_min_sync(0xffffffffu, R.xb_min); R.xb_max = __reduce_max_sync(0xffffffffu, R.xb_max);
+    R.cut = __reduce_min_sync(0xffffffffu, R.cut); R.fext = __reduce_min_sync(0xffffffffu, R.fext);
+    R.hh1 = __reduce_max_sync(0xffffffffu, R.hh1);
+    if ((tid & 31) == 0 && R.es_max) {       // (a warp that decoded no descriptor has nothing to add)
+        atomicMin(&S->r_es_min, R.es_min); atomicMax(&S->r_es_max, R.es_max);
+        atomicMin(&S->r_xb_min, R.xb_min); atomicMax(&S->r_xb_max, R.xb_max);
+        if (R.cut != 0xffffffffu) atomicMin(&S->r_cut, R.cut);
+        if (R.fext != 0xffffffffu) atomicMin(&S->r_fext, R.fext);
+        if (R.hh1) atomicMax(&S->r_hh1, R.hh1);
     }
-#undef SRC_OF
 }
 
 __device__ void leader_commit_warp(const apus_devctx_t *__restrict__ cx)
@@ -600,52 +636,50 @@ __device__ void leader_commit_warp(const apus_devctx_t *__restrict__ cx)
     }
 }
 
-// T2a (outside the place turn): state-independent part of the placement -- inclusive prefix sums
-// of the log strides and of the staged payload bytes of the fetched batch; apply offsets read ahead
-__device__ __noinline__ void leader_prescan(const apus_devctx_t *__restrict__ cx, LeaderShared *S, int lane)
+// After T1 (all producer threads, between the T1 barrier and T2): the state-independent part of the placement --
+// inclusive prefix sums of the log strides and of the staged payload bytes of the fetched batch, closed-form when every
+// entry has the same shape (the benchmark's, and most applications' bursts), else a CTA-wide scan -- and the batch
+// words T2 reads.  Ends with a barrier of the producer warps.
+__device__ __noinline__ void t1_scan(LeaderShared *S, int tid)
 {
+    const int lane = tid & 31, warp = tid >> 5;
     const uint32_t nf = S->n_fetch;
-    uint32_t carry = 0, xcarry = 0, scut = nf, fext = 0xffffffffu, hhk = 0xffffffffu;
-    // a batch of ONE request shape (the benchmark's, and most applications' bursts) needs no scan: cum[k] = (k+1) * stride
-    const uint32_t es0 = S->es[0], xb0 = S->xb[0];
-    bool uniform = true;
-    for (uint32_t r = 0; r < nf; r += 32) {
-        const uint32_t k = r + lane;
-        if (__ballot_sync(0xffffffffu, k < nf && (S->es[k] != es0 || S->xb[k] != xb0))) { uniform = false; break; }
-    }
-    for (uint32_t r = 0; r < nf; r += 32) {
-        const uint32_t k = r + lane;
-        const bool in = k < nf;
-        uint32_t inc = in ? S->es[k] : 0u, xinc = in ? S->xb[k] : 0u;
-        if (uniform) {
-            if (in) { S->cum_es[k] = (k + 1u) * es0; S->cum_xb[k] = (k + 1u) * xb0; }
-        } else {
+    if (S->r_es_min == S->r_es_max && S->r_xb_min == S->r_xb_max) {
+        const uint32_t es0 = S->r_es_min, xb0 = S->r_xb_min;
+        for (uint32_t k = tid; k < nf; k += NT) { S->cum_es[k] = (k + 1u) * es0; S->cum_xb[k] = (k + 1u) * xb0; }
+    } else {
+        // warp w scans the 32-entry parts w, w + 15, ...; then every entry adds the totals of the parts before its own
+        for (uint32_t c = warp; 32u * c < nf; c += N_PRODUCER_WARPS) {
+            const uint32_t k = 32u * c + lane;
+            uint32_t inc = k < nf ? S->es[k] : 0u, xinc = k < nf ? S->xb[k] : 0u;
 #pragma unroll
             for (int sft = 1; sft < 32; sft <<= 1) {
                 const uint32_t o = __shfl_up_sync(0xffffffffu, inc, sft);
                 const uint32_t xo = __shfl_up_sync(0xffffffffu, xinc, sft);
                 if (lane >= sft) { inc += o; xinc += xo; }
             }
-            if (in) { S->cum_es[k] = carry + inc; S->cum_xb[k] = xcarry + xinc; }
-            carry += __shfl_sync(0xffffffffu, inc, 31);
-            xcarry += __shfl_sync(0xffffffffu, xinc, 31);
+            if (k < nf) { S->cum_es[k] = inc; S->cum_xb[k] = xinc; }
+            if (lane == 31) { S->part_es[c] = inc; S->part_xb[c] = xinc; }
         }
-        const uint32_t hm = __ballot_sync(0xffffffffu, in && S->ty[k] == T_HEAD);
-        if (hm) hhk = r + (31u - (uint32_t)__clz(hm));                 // the LAST host HEAD entry of the batch
-        const uint32_t wm = __ballot_sync(0xffffffffu, in && k > 0 && (S->flg[k] & 2u));
-        const uint32_t em = __ballot_sync(0xffffffffu, in && (S->flg[k] & 1u));
-        if (wm && scut == nf) scut = r + (uint32_t)(__ffs(wm) - 1);
-        if (em && fext == 0xffffffffu) fext = r + (uint32_t)(__ffs(em) - 1);
+        bar_sync(1, NT);
+        for (uint32_t k = 32u + tid; k < nf; k += NT) {
+            uint32_t ce = 0, cx = 0;
+            for (uint32_t c = 0; c < (k >> 5); c++) { ce += S->part_es[c]; cx += S->part_xb[c]; }
+            S->cum_es[k] += ce; S->cum_xb[k] += cx;
+        }
     }
-    if (lane == 0) { S->static_cut = scut; S->first_ext_all = fext; S->host_head_k = hhk; }
-    // (the apply offsets are NOT read here: they are ring offsets, and a snapshot taken before the place turn can be so
-    //  old by the time it is used -- other workers may have pruned in between -- that it falls into the used region of
-    //  the NEXT lap and reads as "almost caught up"; they are read while holding the turn, see leader_main)
+    if (tid == 0) {
+        S->static_cut = S->r_cut < nf ? S->r_cut : nf;
+        S->first_ext_all = S->r_fext;
+        S->host_head_k = S->r_hh1 ? S->r_hh1 - 1u : 0xffffffffu;
+        S->ap_valid = 0;          // apply offsets are read inside the place turn, only if the pruning rule could be due
+    }
+    bar_sync(1, NT);
 }
 
 // T2b (inside the place turn): place the next sub-tile of the fetched batch (entries kbase..nf) --
 // log_append_entry's offset rules, free-space rule E2 and the pruning rule, on the placement
-// state this CTA holds.  Kept short: everything state independent was done by leader_prescan.
+// state this CTA holds.  Kept short: everything state independent was done by t1_scan.
 __device__ __noinline__ void leader_place(const apus_devctx_t *__restrict__ cx, LeaderShared *S, const apus_cslot_t *sl, int lane)
 {
     const int N = cx->group_size;
@@ -1080,11 +1114,12 @@ __device__ __noinline__ int leader_express(const apus_devctx_t *__restrict__ cx,
 // The tile loop of a worker CTA, one function per phase (DESIGN.md §3a): T0 claim, T1 fetch, T2 place, T3 prefill,
 // T4 compose, T5 store, T6 publish.  leader_main runs them in order with a CTA barrier of the producer warps between.
 // ---------------------------------------------------------------------------------
-// Worker 0's profile (APUS_FLAG_STATS, thread 0 alone): the phase_ns / turn_ns slots of apus_ctrl_t, kept in registers
+// Worker 0's profile (APUS_FLAG_STATS, thread 0 alone): the phase_ns / turn_ns slots of apus_ctrl_t, kept in shared memory
 // and written out after every tile and while waiting for requests.
 struct LeaderProf {
     bool on;
-    uint64_t ph[8], tn[8], tprev;
+    uint64_t *ph, *tn, tprev;      // ph / tn: LeaderShared::prof_ph / prof_tn -- only thread 0 uses them; in registers
+                                    // they would take 32 from every producer thread (and the kernel spills)
     // the time since the previous mark goes to phase i
     __device__ __forceinline__ void phase(int i) { if (on) { const uint64_t t = globaltimer_ns(); ph[i] += t - tprev; tprev = t; } }
     __device__ __forceinline__ void flush(apus_ctrl_t *ctrl) const
@@ -1248,11 +1283,16 @@ __device__ __forceinline__ void t0_claim(const apus_devctx_t *__restrict__ cx, L
         if (P.on) { P.tn[0] += globaltimer_ns() - tw0; P.tn[6]++; }
         if (n) S->slot0 = claimed;
         S->n_fetch = n; S->finish = fin;
+        DescReduce R0;
+        R0.init();
+        S->r_es_min = R0.es_min; S->r_es_max = R0.es_max; S->r_xb_min = R0.xb_min; S->r_xb_max = R0.xb_max;
+        S->r_cut = R0.cut; S->r_fext = R0.fext; S->r_hh1 = R0.hh1;
         S->t_dequeue = globaltimer_ns();
     }
 }
 
-// T1 fetch (all producer threads): the claimed slots (descriptor + inline payload), coalesced 16 B loads
+// T1 fetch (all producer threads): the claimed slots (descriptor + inline payload), coalesced 16 B loads; the
+// descriptors are reduced on the way (DescReduce)
 __device__ __forceinline__ void t1_fetch(const apus_devctx_t *__restrict__ cx, LeaderShared *S, int tid)
 {
     uint8_t *slots = smem_raw + L_SLOTS_OFF;
@@ -1342,8 +1382,8 @@ __device__ __forceinline__ void place_fast(const apus_devctx_t *__restrict__ cx,
     S->fast = 1;
 }
 
-// T2 place (warp 0): the next sub-tile of the fetched batch.  For the first one, the state-independent part outside the
-// place turn (leader_prescan), then the turn and the fast path; what the fast path does not place is placed by
+// T2 place (warp 0): the next sub-tile of the fetched batch.  For the first one the turn and the fast path (the
+// state-independent part was done by all producer threads in t1_scan); what the fast path does not place is placed by
 // leader_place while the turn is held, and the state is handed on with the last sub-tile.
 __device__ __forceinline__ void t2_place(const apus_devctx_t *__restrict__ cx, LeaderShared *S, bool have_place_turn,
                                          LeaderProf &P, int lane)
@@ -1353,19 +1393,6 @@ __device__ __forceinline__ void t2_place(const apus_devctx_t *__restrict__ cx, L
     apus_seq_t *seq = reinterpret_cast<apus_seq_t *>(cx->region + APUS_SEQ_OFF);
     apus_loghdr_t *hdr = reinterpret_cast<apus_loghdr_t *>(cx->region + APUS_HDR_OFF);
     if (!have_place_turn) {
-        if (S->n_fetch == 1) {
-            // one request in flight (closed-loop latency path): nothing to scan
-            if (lane == 0) {
-                S->cum_es[0] = S->es[0]; S->cum_xb[0] = S->xb[0];
-                S->static_cut = 1; S->first_ext_all = (S->flg[0] & 1u) ? 0u : 0xffffffffu;
-                S->host_head_k = (S->ty[0] == T_HEAD) ? 0u : 0xffffffffu;
-            }
-            S->ap_valid = 0;          // apply offsets are read only if the pruning rule could be due
-        } else {
-            leader_prescan(cx, S, lane);
-            if (lane == 0) S->ap_valid = 0;
-        }
-        __syncwarp();
         if (lane == 0) place_fast(cx, S, P);
         __syncwarp();
         if (S->fast) return;
@@ -1392,6 +1419,26 @@ __device__ __forceinline__ void t2_place(const apus_devctx_t *__restrict__ cx, L
 // data image ([48 + nb, stride): 14 bytes for a request) -- which keep what the log held (dare_log.h:507-529 never
 // writes them).  For tiles of large entries only the chunks that overlap a hole are brought in; small entries are
 // mostly holes' neighbours, the whole range is read in one coalesced sweep.
+__device__ __forceinline__ void hole_chunks(const LeaderShared *S, const apus_cslot_t *sl, uint32_t j, uint64_t lo[4])
+{
+    uint32_t rel, es_, nb_;
+    if (S->auto_head && j == 0) { rel = 0; es_ = APUS_HDR_BYTES; nb_ = 8; }
+    else {
+        const uint32_t k = S->kbase + j - S->auto_head;
+        rel = S->hbytes + (S->cum_es[k] - S->base_es) - S->es[k];
+        es_ = S->es[k]; nb_ = data_bytes(S->ty[k], sl[k].len);
+    }
+    const uint64_t eo = S->a + rel;
+    const uint64_t h0 = eo + 41, h1 = eo + 47, g0 = eo + 48 + nb_, g1 = eo + es_ - 1;   // hole byte ranges (inclusive)
+    const uint64_t cs[4] = { h0 >> 4, h1 >> 4, g0 >> 4, g1 >> 4 };
+#pragma unroll
+    for (int q = 0; q < 4; q++) {
+        lo[q] = cs[q] << 4;
+        if (q >= 2 && g1 < g0) lo[q] = ~0ull;                     // no slack
+        else if (q > 0 && cs[q] == cs[q - 1]) lo[q] = ~0ull;      // same chunk as the previous hole
+    }
+}
+
 __device__ __noinline__ void t3_prefill(const apus_devctx_t *__restrict__ cx, LeaderShared *S, int tid)
 {
     const apus_cslot_t *sl = reinterpret_cast<const apus_cslot_t *>(smem_raw + L_SLOTS_OFF);
@@ -1404,27 +1451,21 @@ __device__ __noinline__ void t3_prefill(const apus_devctx_t *__restrict__ cx, Le
     const uint32_t nchunks = (uint32_t)(((b + 15ull) & ~15ull) - a16) >> 4;
     const bool holes_only = !gap && (b - a) >= (uint64_t)(m + autoh) * 512ull;
     if (holes_only) {
+        // the (up to four) hole chunks of an entry are loaded together (zeroed first, see cta_fetch_slots)
+        const uint64_t hi16 = a16 + 16ull * nchunks;
+        const bool fresh = S->fresh != 0;
         for (uint32_t j = tid; j < m + autoh; j += NT) {
-            uint32_t rel, es_, nb_;
-            if (autoh && j == 0) { rel = 0; es_ = APUS_HDR_BYTES; nb_ = 8; }
-            else {
-                const uint32_t k = kbase + j - autoh;
-                rel = S->hbytes + (S->cum_es[k] - S->base_es) - S->es[k];
-                es_ = S->es[k]; nb_ = data_bytes(S->ty[k], sl[k].len);
-            }
-            const uint64_t eo = a + rel;
-            const uint64_t h0 = eo + 41, h1 = eo + 47, g0 = eo + 48 + nb_, g1 = eo + es_ - 1;   // hole byte ranges (inclusive)
-            const uint64_t cs[4] = { h0 >> 4, h1 >> 4, g0 >> 4, g1 >> 4 };
+            uint64_t lo[4];
+            hole_chunks(S, sl, j, lo);
+            uint4 v[4];
 #pragma unroll
             for (int q = 0; q < 4; q++) {
-                if (q == 3 && g1 < g0) continue;
-                if (q == 2 && g1 < g0) continue;
-                if (q > 0 && cs[q] == cs[q - 1]) continue;
-                const uint64_t lo = cs[q] << 4;
-                if (lo < a16 || lo >= a16 + 16ull * nchunks) continue;
-                reinterpret_cast<uint4 *>(img)[(lo - a16) >> 4] =
-                    S->fresh ? make_uint4(0, 0, 0, 0) : ld_relaxed_sys_v4(entries + lo);
+                v[q] = make_uint4(0, 0, 0, 0);
+                if (!fresh && lo[q] >= a16 && lo[q] < hi16) v[q] = ld_relaxed_sys_v4(entries + lo[q]);
             }
+#pragma unroll
+            for (int q = 0; q < 4; q++)
+                if (lo[q] >= a16 && lo[q] < hi16) reinterpret_cast<uint4 *>(img)[(lo[q] - a16) >> 4] = v[q];
         }
     } else if (S->fresh) {
         for (uint32_t c = tid; c < nchunks; c += NT) reinterpret_cast<uint4 *>(img)[c] = make_uint4(0, 0, 0, 0);
@@ -1631,7 +1672,8 @@ __device__ void leader_main(const apus_devctx_t *__restrict__ cx, const uint32_t
     uint64_t last_progress = globaltimer_ns();
     LeaderProf P;
     P.on = (cx->flags & APUS_FLAG_STATS) != 0 && tid == 0 && wid == 0;
-    for (int i = 0; i < 8; i++) { P.ph[i] = ctrl->phase_ns[i]; P.tn[i] = ctrl->turn_ns[i]; }
+    P.ph = S->prof_ph; P.tn = S->prof_tn;
+    if (tid == 0) for (int i = 0; i < 8; i++) { P.ph[i] = ctrl->phase_ns[i]; P.tn[i] = ctrl->turn_ns[i]; }
     P.tprev = globaltimer_ns();
     Express X = {};
     uint64_t xguess = ctrl->consumed;          // worker 0: the slot it expects to be claimed next
@@ -1646,13 +1688,12 @@ __device__ void leader_main(const apus_devctx_t *__restrict__ cx, const uint32_t
         P.phase(0);
         t1_fetch(cx, S, tid);
         bar_sync(1, NT);
+        t1_scan(S, tid);
         P.phase(1);
-        if (warp == 1) {
+        if (tid == 32) {
             // entry-size statistics of this claim (sizes the next one)
-            uint32_t se = 0, sx = 0;
-            for (uint32_t k = lane; k < nf; k += 32) { se += S->es[k]; sx += S->xb[k]; }
-            for (int sft = 16; sft > 0; sft >>= 1) { se += __shfl_xor_sync(0xffffffffu, se, sft); sx += __shfl_xor_sync(0xffffffffu, sx, sft); }
-            if (lane == 0) { st_relaxed_sys(&seq->avg_es, (se + nf - 1) / nf); st_relaxed_sys(&seq->avg_xb, (sx + nf - 1) / nf); }
+            st_relaxed_sys(&seq->avg_es, (S->cum_es[nf - 1] + nf - 1) / nf);
+            st_relaxed_sys(&seq->avg_xb, (S->cum_xb[nf - 1] + nf - 1) / nf);
         }
         bool have_pub_turn = false, have_place_turn = false, aborted = false;
         uint64_t gap_bytes = 0;      // bytes of a wrap gap replicated ahead of the next publish

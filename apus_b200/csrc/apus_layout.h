@@ -296,7 +296,7 @@ typedef struct apus_role {
 } apus_role_t;
 
 #define APUS_KERNEL_THREADS    512
-#define APUS_MAX_TILE_ENTRIES  256u             /* slots fetched per tile (32 KiB of shared memory) */
+#define APUS_MAX_TILE_ENTRIES  512u             /* slots fetched per tile (48 KiB of shared memory) */
 #define APUS_LEADER_IMG_BYTES  (80u * 1024u)    /* log bytes composed per tile (>= one maximal entry) */
 #define APUS_LEADER_EXT_BYTES  (66u * 1024u)    /* payload-ring bytes staged per tile (>= one maximal image) */
 #define APUS_FOLLOWER_WIN_BYTES (96u * 1024u)   /* log bytes a follower walks per window */

@@ -8,7 +8,7 @@
  * inline in its 128 B slot when it has at most APUS_SLOT_INLINE bytes, else in the payload byte ring at a 16 B aligned
  * position (APUS_SLOT_EXT).  An image never wraps the payload ring: one that would cross its end starts at 0 instead.
  *
- * The invariant the leader kernel relies on (leader_prescan, leader_place and place_fast stage the range
+ * The invariant the leader kernel relies on (t1_scan, leader_place and place_fast stage the range
  * [ext_base, ext_base + cum_xb) of a claim with one copy): the external images of consecutive tickets lie
  * contiguously in the payload ring, each round16(image) bytes after the previous one, and every discontinuity is
  * marked with APUS_SLOT_WRAP on the image AFTER it.  A WRAP where the images happen to be contiguous is harmless: it
