@@ -86,6 +86,9 @@ class Oracle:
         f("apply", None, [vp, C.c_int])
         f("poll_head", None, [vp, C.c_int, C.POINTER(u64)])
         f("prune", u64, [vp])
+        # newer than the rest of the API: a library built by an older recipe (a prebuilt oracle/_ref kept where the
+        # reference tree is absent) lacks it, and everything else in it still works
+        f("prune_to", u64, [vp, u64], optional=True)
         f("round", None, [vp])
         f("cluster_offsets", None, [vp, C.c_int, C.POINTER(u64)])
         f("cluster_entries", C.POINTER(u8), [vp, C.c_int])
@@ -100,8 +103,15 @@ class Oracle:
             L.orc_set_rules.argtypes = [C.c_int]
             L.orc_set_rules.restype = None
 
-    def _f(self, name, restype, argtypes):
-        fn = getattr(self.lib, f"{self.prefix}_{name}")
+    def _f(self, name, restype, argtypes, optional=False):
+        sym = f"{self.prefix}_{name}"
+        if optional and not hasattr(self.lib, sym):
+            def missing(*_):
+                raise AttributeError(f"{self.lib._name} has no {sym}: it was built from an older oracle/cluster_sim.inc "
+                                     "(make -C oracle port ref)")
+            setattr(self, name, missing)
+            return
+        fn = getattr(self.lib, sym)
         fn.restype = restype
         fn.argtypes = argtypes
         setattr(self, name, fn)
@@ -173,6 +183,11 @@ class Cluster:
 
     def prologue(self):
         return self.o.prologue(self.h)
+
+    def prune_to(self, head):
+        """SIM(prune_to): head := `head` and append <HEAD, head>, without the pruning rule's checks (the replay of a
+        run whose HEAD entries the engine decided, tests/autoprune_replay.py).  Returns the HEAD idx, 0 when full."""
+        return self.o.prune_to(self.h, head)
 
     def round(self, live=None):
         """One round of SIM(round) (oracle/cluster_sim.inc).  With `live` (follower indices), only those followers
