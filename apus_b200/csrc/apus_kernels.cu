@@ -23,7 +23,7 @@
  *            from committed HEAD entries (dare_server.c:2163-2186).
  *
  * Ordering (invariant I1, "data before tail"): all data stores of a tile ->
- * bar.sync -> fence.acq_rel.sys -> 16 B st.relaxed.sys of {end, count}.  The
+ * bar.sync -> fence.sc.sys -> 16 B st.relaxed.sys of {end, count}.  The
  * follower reads the pair, fences, and reads the entry bytes with ld.relaxed.sys
  * (never through a stale L1 line).  Acks mirror this in the other direction.
  *
@@ -1896,13 +1896,27 @@ __device__ void follower_main(const apus_devctx_t *__restrict__ cx)
             const uint64_t n = cum_seen - acked;
             if (tid == 0) S->head_j = 0;
             __syncthreads();
-            for (uint64_t j = tid; j < n; j += nthr) {
-                // (a self-certified publish names its one entry itself: its index word may still be in flight)
-                const uint32_t w = S->cert ? (uint32_t)S->cert_start : ld_relaxed_sys_u32(&index[(uint32_t)(acked + 1 + j) & cx->idx_mask]);
-                const uint64_t at = (uint64_t)(w & ~APUS_IDX_HEAD_FLAG) + E_REPLY + (uint64_t)me;
-                st_relaxed_sys_u8(entries + at, 1);         // reply[me] = 1 in my copy and in the
-                st_relaxed_sys_u8(lentries + at, 1);        // leader's (dare_ibv_rc.c:1833-1854)
-                if (w & APUS_IDX_HEAD_FLAG) atomicMax(&S->head_j, (uint32_t)(j + 1));
+            // FIDX index words per thread are loaded together before any is used: one round trip per FIDX * nthr
+            // entries, not per nthr (a batch of a few tiles is thousands of entries)
+            constexpr int FIDX = 8;
+            for (uint64_t j0 = tid; j0 < n; j0 += (uint64_t)FIDX * nthr) {
+                uint32_t w[FIDX];
+#pragma unroll
+                for (int q = 0; q < FIDX; q++) {
+                    const uint64_t j = j0 + (uint64_t)q * nthr;
+                    w[q] = 0;
+                    // (a self-certified publish names its one entry itself: its index word may still be in flight)
+                    if (j < n) w[q] = S->cert ? (uint32_t)S->cert_start : ld_relaxed_sys_u32(&index[(uint32_t)(acked + 1 + j) & cx->idx_mask]);
+                }
+#pragma unroll
+                for (int q = 0; q < FIDX; q++) {
+                    const uint64_t j = j0 + (uint64_t)q * nthr;
+                    if (j >= n) break;
+                    const uint64_t at = (uint64_t)(w[q] & ~APUS_IDX_HEAD_FLAG) + E_REPLY + (uint64_t)me;
+                    st_relaxed_sys_u8(entries + at, 1);         // reply[me] = 1 in my copy and in the
+                    st_relaxed_sys_u8(lentries + at, 1);        // leader's (dare_ibv_rc.c:1833-1854)
+                    if (w[q] & APUS_IDX_HEAD_FLAG) atomicMax(&S->head_j, (uint32_t)(j + 1));
+                }
             }
             __syncthreads();
             if (S->head_j) {
