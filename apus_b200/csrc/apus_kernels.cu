@@ -24,8 +24,10 @@
  *
  * Ordering (invariant I1, "data before tail"): all data stores of a tile ->
  * bar.sync -> fence.sc.sys -> 16 B st.relaxed.sys of {end, count}.  The
- * follower reads the pair, fences, and reads the entry bytes with ld.relaxed.sys
- * (never through a stale L1 line).  Acks mirror this in the other direction.
+ * follower reads the pair with ld.acquire.sys (or, for a self-certifying publish,
+ * verifies its checksum over the bytes) and then reads the entry bytes with
+ * ld.relaxed.sys (never through a stale L1 line).  Acks mirror this in the other
+ * direction.
  *
  * Pure integer / byte work: no tensor cores, bound by NVLink store bandwidth and
  * by launch-free round-trip latency.
@@ -162,11 +164,23 @@ __device__ __forceinline__ uint64_t adopt_head(uint64_t head, uint64_t carried, 
     const uint64_t ne = (new_end == L) ? 0 : new_end;
     return (ring_dist(head, carried, L) <= ring_dist(head, ne, L)) ? carried : head;     // only forward, only inside the used region
 }
-__device__ __forceinline__ uint64_t slot_head_value(const apus_cslot_t *sl)
+// the little-endian u64 of the 8 bytes at p, any alignment: the head offset a HEAD entry carries
+__device__ __forceinline__ uint64_t le_u64(const uint8_t *p)
 {
     uint64_t v = 0;
 #pragma unroll
-    for (int q = 7; q >= 0; q--) v = (v << 8) | sl->inl[q];
+    for (int q = 7; q >= 0; q--) v = (v << 8) | p[q];
+    return v;
+}
+// the u64 at log offset `at` of any alignment, with system-scope relaxed loads: one 8 B load, or eight byte reads out of
+// 4 B-aligned words
+__device__ __forceinline__ uint64_t ld_relaxed_sys_u64_any(const uint8_t *entries, uint64_t at)
+{
+    uint64_t v = ld_relaxed_sys(entries + (at & ~7ull));
+    if (at & 7ull) {
+        v = 0;
+        for (int q = 7; q >= 0; q--) v = (v << 8) | (uint64_t)(ld_relaxed_sys_u32(entries + ((at + q) & ~3ull)) >> (8 * ((at + q) & 3ull)) & 0xffu);
+    }
     return v;
 }
 
@@ -467,175 +481,6 @@ __device__ __noinline__ void cta_fetch_slots(LeaderShared *S, uint8_t *slots, co
     }
 }
 
-__device__ void leader_commit_warp(const apus_devctx_t *__restrict__ cx)
-{
-    const int lane = threadIdx.x & 31;
-    const int N = cx->group_size, me = cx->idx, quorum = cx->quorum;
-    apus_ctrl_t *ctrl = reinterpret_cast<apus_ctrl_t *>(cx->region);
-    apus_seq_t *seq = reinterpret_cast<apus_seq_t *>(cx->region + APUS_SEQ_OFF);
-    const apus_pubrec_t *ring = reinterpret_cast<const apus_pubrec_t *>(cx->region + APUS_PUBRING_OFF);
-    apus_loghdr_t *hdr = reinterpret_cast<apus_loghdr_t *>(cx->region + APUS_HDR_OFF);
-    apus_hostwords_t *hw = cx->hw;
-    uint64_t committed = ctrl->committed;
-    uint64_t committed_tickets = ctrl->committed_tickets;
-    uint64_t lat_count = ctrl->lat_count;
-    uint64_t bytes_rep = ctrl->bytes_replicated, batches = ctrl->batches;
-    uint64_t tail = 0;                       // next record to commit
-    uint64_t seen = 0;                       // records [tail, seen) are valid and not committed yet
-    uint64_t published = ctrl->published;    // entries published = cum of the newest valid record
-    uint64_t last_progress = globaltimer_ns();
-    uint32_t spins = 0, hb_spins = 0;
-    uint64_t last_hb = 0, hb_beat = globaltimer_ns() >> 10;   // beats keep growing across launches
-    bool S_rec_ok = false;
-    // commit publish into the follower's control block, stamped with my term: the follower's header `commit` is the
-    // follower's own (clamped to what it holds, I4), and a deposed leader's offsets are dropped by the term fence
-    uint64_t *peer_commit = nullptr;
-    if (lane < N && lane != me && cx->peer[lane])
-        peer_commit = reinterpret_cast<apus_ctrl_t *>(cx->peer[lane])->pub_commit;
-
-    for (;;) {
-        // every lane looks at one 16 B pair of the next four publish records (lane>>3 = record, lane&7 = pair)
-        // while lanes 0..N-1 also poll the acks
-        uint64_t st = 0, rv = 0, v = 0;
-        const uint64_t seen_before = seen;
-        {
-            const uint64_t rn = seen + (uint64_t)(lane >> 3);
-            ld_relaxed_sys_2x64(&ring[rn & PUBMASK].w[2 * (lane & 7)], st, rv);
-            const uint32_t okm = __ballot_sync(0xffffffffu, st == rn + 1);
-            // records are valid only in order: count the leading records whose eight pairs all match
-            uint32_t nvalid = 0;
-            while (nvalid < 4 && ((okm >> (8 * nvalid)) & 0xffu) == 0xffu) nvalid++;
-            if (nvalid) {
-                published = __shfl_sync(0xffffffffu, rv, 8 * (nvalid - 1) + PR_CUM);
-                seen += nvalid;
-                if (lane == 0) st_relaxed_sys(&ctrl->pub_seen, published);
-            }
-            S_rec_ok = nvalid != 0;
-        }
-        if (lane < N && lane != me) v = ld_relaxed_sys(&ctrl->ack[lane]);
-        // lane i holds what replica i has acked (entries, monotone); the leader's own vote is
-        // everything it has published (dare_ibv_rc.c:1736 "i == idx")
-        if (lane == me) v = published;
-        // rank: how many replicas hold at least what I hold
-        int cnt = 0;
-        for (int j = 0; j < N; j++) {
-            uint64_t vj = __shfl_sync(0xffffffffu, v, j);
-            cnt += (vj >= v) ? 1 : 0;
-        }
-        uint64_t cand = (lane < N && cnt >= quorum) ? v : 0;
-        // the largest count a majority holds (size/2+1, dare_ibv_rc.c:1741)
-        for (int s = 16; s > 0; s >>= 1) {
-            uint64_t o = __shfl_xor_sync(0xffffffffu, cand, s);
-            cand = o > cand ? o : cand;
-        }
-        const uint64_t Q = cand;
-        if (Q > committed && tail != seen) {
-            // map the entry count to the log offset recorded at publish time; the commit is a
-            // prefix and an entry boundary (invariant I3).  Four records per step.
-            uint64_t off = 0, tickets = committed_tickets, r_tail = 0, r_hwm = 0, r_next = 0;
-            bool any = false;
-            bool reuse = (tail == seen_before);          // the pending records are exactly the ones this iteration loaded
-            while (tail != seen) {
-                const uint64_t rn = tail + (uint64_t)(lane >> 3);
-                uint64_t st2 = 0, val = 0;
-                if (reuse) { val = rv; reuse = false; }
-                else if (rn < seen) ld_relaxed_sys_2x64(&ring[rn & PUBMASK].w[2 * (lane & 7)], st2, val);
-                // how many of these (up to four, in order) are covered by the quorum count
-                const uint32_t cm = __ballot_sync(0xffffffffu, (lane & 7) == PR_CUM && rn < seen && val <= Q);
-                uint32_t nc = 0;
-                while (nc < 4 && ((cm >> (8 * nc)) & 1u)) nc++;
-                if (nc == 0) break;
-                const int base = 8 * (int)(nc - 1);
-                committed = __shfl_sync(0xffffffffu, val, base + PR_CUM);
-                off = __shfl_sync(0xffffffffu, val, base + PR_END);
-                tickets = __shfl_sync(0xffffffffu, val, base + PR_TICKETS);
-                r_tail = __shfl_sync(0xffffffffu, val, base + PR_TAIL);
-                r_hwm = __shfl_sync(0xffffffffu, val, base + PR_HWM);
-                r_next = __shfl_sync(0xffffffffu, val, base + PR_NEXTIDX);
-                for (uint32_t q = 0; q < nc; q++) {
-                    bytes_rep += __shfl_sync(0xffffffffu, val, 8 * q + PR_BYTES);
-                    const uint64_t t0 = __shfl_sync(0xffffffffu, val, 8 * q + PR_T0);
-                    if ((cx->flags & APUS_FLAG_STATS) && cx->lat_ns && lane == 0) {
-                        const uint64_t d = globaltimer_ns() - t0;
-                        cx->lat_ns[(lat_count + q) & (APUS_LAT_RING - 1)] = d > 0xffffffffull ? 0xffffffffu : (uint32_t)d;
-                    }
-                }
-                lat_count += nc; batches += nc;
-                tail += nc;
-                any = true;
-                if (nc < 4) break;
-            }
-            if (any) {
-                if (peer_commit) st_relaxed_sys_2x64(peer_commit, off, cx->term);   // dare_ibv_rc.c:1810
-                if (lane == 0) {
-                    // {commit offset, committed tickets}: ONE 16 B store into pinned host memory -- this is what
-                    // releases the proxy.c:160 spinners; a 16 B host load sees a consistent pair
-                    st_relaxed_sys_2x64(&hw->commit_off, off, tickets);
-                    st_relaxed_sys(&hw->consumed, tickets);                 // submission-ring space
-                    st_relaxed_sys(&hw->last_commit_ns, globaltimer_ns());
-                    st_relaxed_sys(&seq->pub_tail, tail);                   // publish-ring space
-                    // the leader's bookkeeping, in publish order (single writer)
-                    hdr->commit = off;
-                    st_relaxed_sys(&hdr->apply, off);                       // leader applies = update_state
-                    hdr->end = off; hdr->tail = r_tail; hdr->old_end = off;
-                    ctrl->committed = committed; ctrl->committed_tickets = tickets; ctrl->lat_count = lat_count;
-                    ctrl->published = committed; ctrl->consumed = tickets; ctrl->next_idx = r_next; ctrl->hwm = r_hwm;
-                    ctrl->bytes_replicated = bytes_rep; ctrl->batches = batches;
-                }
-                committed_tickets = tickets;
-                last_progress = globaltimer_ns();
-                __syncwarp();
-            }
-        }
-        // heartbeat (dare_ibv_rc.c:868-958: the leader writes its SID into every follower's ctrl_data.hb[]): the
-        // commit warp is the leader's liveness -- when the hosting process dies the context goes with it and the beats stop
-        if (cx->hb_period_ns && (++hb_spins & 0x1fu) == 0) {
-            const uint64_t now = globaltimer_ns();
-            if (now - last_hb >= cx->hb_period_ns) {
-                last_hb = now; hb_beat++;
-                if (lane < N && lane != me && cx->peer[lane])
-                    st_relaxed_sys(&reinterpret_cast<apus_ctrl_t *>(cx->peer[lane])->hb, term_word(hb_beat, cx->term));
-            }
-        }
-        const bool rec_ok = S_rec_ok;
-        // exit: every worker finished and nothing is in flight
-        int ex = 0;
-        if (lane == 0) {
-            if (!rec_ok && tail == seen && committed == published && ld_acquire_gpu(&seq->workers_done) == cx->n_workers) {
-                // one more look at the ring after the workers are known to be done
-                ex = 3;
-            } else if ((++spins & 0x3ffu) == 0) {
-                if (ld_relaxed_sys(&seq->abort_flag)) ex = 2;
-                else if (globaltimer_ns() - last_progress > WATCHDOG_NS && (tail != seen || committed != published) &&
-                         (cx->target != ~0ull || ld_relaxed_sys_u32(&hw->stop))) {
-                    st_relaxed_sys(&hw->error, APUS_KERR_WATCHDOG_COMMIT);
-                    st_relaxed_sys(&seq->abort_flag, 1);
-                    ex = 2;
-                }
-            }
-        }
-        ex = __shfl_sync(0xffffffffu, ex, 0);
-        if (ex == 3) {
-            // workers are done (acquire above): any record they wrote is visible now; re-check once
-            uint64_t st3 = 0, v3 = 0;
-            if (lane >= 16 && lane < 24) ld_relaxed_sys_2x64(&ring[seen & PUBMASK].w[2 * (lane - 16)], st3, v3);
-            const bool more = __ballot_sync(0xffffffffu, lane >= 16 && lane < 24 && st3 == seen + 1) == 0x00ff0000u;
-            ex = more ? 0 : 1;
-        }
-        if (ex) {
-            // clean end of a bounded launch: tell every follower how many entries exist, so
-            // that it can leave once it has acked and applied all of them
-            if (ex == 1 && cx->target != ~0ull && lane < N && lane != me && cx->peer[lane]) {
-                apus_ctrl_t *pc = reinterpret_cast<apus_ctrl_t *>(cx->peer[lane]);
-                st_relaxed_sys(&pc->fin_entries, committed);
-                __threadfence_system();
-                st_relaxed_sys(&pc->fin_target, cx->target);
-            }
-            break;
-        }
-    }
-}
-
 // After T1 (all producer threads, between the T1 barrier and T2): the state-independent part of the placement --
 // inclusive prefix sums of the log strides and of the staged payload bytes of the fetched batch, closed-form when every
 // entry has the same shape (the benchmark's, and most applications' bursts), else a CTA-wide scan -- and the batch
@@ -777,7 +622,7 @@ __device__ __noinline__ void leader_place(const apus_devctx_t *__restrict__ cx, 
             if (autoh) st_relaxed_sys(&hdr->head, new_head);
             if (autoh) S->st.head = new_head;
             if (S->host_head_k != 0xffffffffu && S->host_head_k >= kbase && S->host_head_k < kbase + m) {
-                const uint64_t nh = adopt_head(S->st.head, slot_head_value(&sl[S->host_head_k]), b, L);
+                const uint64_t nh = adopt_head(S->st.head, le_u64(sl[S->host_head_k].inl), b, L);
                 if (nh != S->st.head) { S->st.head = nh; st_relaxed_sys(&hdr->head, nh); }
             }
             if (S->gap) {
@@ -875,6 +720,43 @@ __device__ __forceinline__ void pub_record(apus_pubrec_t *ring, uint64_t h, int 
     const uint64_t val = q == PR_CUM ? cum : q == PR_END ? end : q == PR_TICKETS ? tickets : q == PR_T0 ? t0
                        : q == PR_TAIL ? tail : q == PR_HWM ? hwm : q == PR_NEXTIDX ? next_idx : bytes;
     st_relaxed_sys_2x64(&ring[h & PUBMASK].w[2 * q], h + 1, val);
+}
+// warp: lane l looks at pair l & 7 of record rn0 + l / 8, for the first `nrec` (<= 4) records; v is the lane's value.
+// Returns how many of them, in order from rn0, are valid (all eight pairs stamped with their record number + 1).
+// `known_valid`: the records were found valid before and not committed since, so no writer has reused them (a writer
+// waits for pub_tail, which the commit warp moves only past committed records): nrec, and only the values are loaded.
+__device__ __forceinline__ uint32_t pubrec_probe(const apus_pubrec_t *ring, uint64_t rn0, uint32_t nrec, int lane, uint64_t &v,
+                                                 bool known_valid = false)
+{
+    const uint64_t rn = rn0 + (uint64_t)(lane >> 3);
+    uint64_t st = 0;
+    v = 0;
+    if ((uint32_t)(lane >> 3) < nrec) ld_relaxed_sys_2x64(&ring[rn & PUBMASK].w[2 * (lane & 7)], st, v);
+    if (known_valid) return nrec;
+    const uint32_t okm = __ballot_sync(0xffffffffu, st == rn + 1);
+    uint32_t n = 0;
+    while (n < nrec && ((okm >> (8 * n)) & 0xffu) == 0xffu) n++;
+    return n;
+}
+// field f (PR_*) of record q of a probe, from lane 8q + f, in every lane
+__device__ __forceinline__ uint64_t pubrec_field(uint64_t v, uint32_t q, int f)
+{
+    return __shfl_sync(0xffffffffu, v, 8 * (int)q + f);
+}
+// what the commit warp's bookkeeping takes from the newest committed record
+struct PubRec {
+    uint64_t cum, end, tickets, tail, hwm, next_idx;
+};
+__device__ __forceinline__ PubRec pubrec_decode(uint64_t v, uint32_t q)
+{
+    PubRec r;
+    r.cum = pubrec_field(v, q, PR_CUM);
+    r.end = pubrec_field(v, q, PR_END);
+    r.tickets = pubrec_field(v, q, PR_TICKETS);
+    r.tail = pubrec_field(v, q, PR_TAIL);
+    r.hwm = pubrec_field(v, q, PR_HWM);
+    r.next_idx = pubrec_field(v, q, PR_NEXTIDX);
+    return r;
 }
 
 // the 16 B chunk v of the image at log offset lo (16 B aligned), restricted to [a, b), into the local log and every
@@ -1108,6 +990,254 @@ __device__ __noinline__ int leader_express(const apus_devctx_t *__restrict__ cx,
         if (lane == 0) pub_handoff(seq, claimed + 1, h + 1);
     }
     return 0;
+}
+
+// ---------------------------------------------------------------------------------
+// The self-certifying tail publish, read (the writers: t6_publish and leader_express)
+// ---------------------------------------------------------------------------------
+// {end | APUS_PUB_CERT, count|term} and the certificate half {checksum, start}, decoded.  Term fence: a publish stamped
+// with another term (a deposed leader still storing) counts no entries.
+struct TailPub {
+    uint64_t end, cum, csum, start;
+    uint32_t cert;             // self-certifying: ONE entry at `start`, no writer fence before it
+};
+__device__ __forceinline__ TailPub tail_pub_decode(uint64_t end_w, uint64_t cum_w, uint64_t csum, uint64_t start, uint64_t term)
+{
+    TailPub p;
+    p.cum = term_word_is(cum_w, term) ? cum_w & APUS_PUB_CUM_MASK : 0;
+    p.cert = (end_w & APUS_PUB_CERT) ? 1u : 0u;
+    p.end = end_w & ~APUS_PUB_CERT;
+    p.csum = csum;
+    p.start = start;
+    return p;
+}
+// warp, on a self-certifying publish p: is it exactly the next entry (ONE entry, at the walk position old_end, at most
+// 496 B), and do the bytes there add up to its checksum?  An entry of up to 12 chunks is taken from the speculative read
+// of lanes 4..15 (lane 4 + c holds chunk c, at spec_lo); a longer one is read again.  The key is the publish's
+// count|term: p.cum > acked here, so the term fence passed and term_word rebuilds the word that was stored.
+__device__ __forceinline__ bool tail_pub_verify(const TailPub &p, uint64_t old_end, uint64_t acked, uint64_t L, uint64_t term,
+                                                const uint8_t *entries, const uint4 spec, uint64_t spec_lo, int lane)
+{
+    const uint64_t a = p.start, b = (p.end == 0) ? L : p.end;
+    if (!(p.cum == acked + 1 && a == ((old_end == L) ? 0 : old_end) && b > a && b - a <= 32u * 16u - 16u)) return false;
+    const uint64_t a16 = a & ~15ull;
+    const uint32_t nch = (uint32_t)(((b + 15ull) & ~15ull) - a16) >> 4;
+    uint64_t cs = 0;
+    if (nch <= 12) {
+        if (lane >= 4 && lane < 4 + (int)nch) cs = cs_chunk(spec, spec_lo, a, b);
+    } else if (lane < (int)nch) cs = cs_chunk(ld_relaxed_sys_v4(entries + a16 + 16ull * lane), a16 + 16ull * lane, a, b);
+#pragma unroll
+    for (int sft = 16; sft > 0; sft >>= 1) cs += __shfl_xor_sync(0xffffffffu, cs, sft);
+    return (cs + cs_key(term_word(p.cum, term))) == p.csum;
+}
+
+// ---------------------------------------------------------------------------------
+// Commit warp (worker 0, warp 15): one function per phase (DESIGN.md §3c) -- probe, quorum rank, commit walk, commit
+// stores, heartbeat, exit decision, fin publish -- called in order by leader_commit_warp
+// ---------------------------------------------------------------------------------
+struct CommitWarp {            // addresses derived from cx once, then the state; the same in every lane but `peer`
+    apus_ctrl_t *ctrl; apus_seq_t *seq; const apus_pubrec_t *ring; apus_loghdr_t *hdr; apus_hostwords_t *hw;
+    apus_ctrl_t *peer;         // lane i: follower i's control block (null: not a follower of mine)
+    int N, me, quorum;
+    uint64_t committed, committed_tickets, lat_count, bytes_rep, batches;
+    uint64_t tail;             // next record to commit
+    uint64_t seen;             // records [tail, seen) are valid and not committed yet
+    uint64_t published;        // entries published = cum of the newest valid record
+    uint64_t last_progress;
+    uint32_t spins, hb_spins;
+    uint64_t last_hb, hb_beat; // beats keep growing across launches
+};
+
+// The commit publish {offset, term} in a follower's control block: one 16 B store by cw_commit.  The follower keeps its
+// header `commit` itself (clamped to what it holds, I4); a deposed leader's offsets are dropped by the term fence.
+__device__ __forceinline__ uint64_t commit_pub_offset(uint64_t off, uint64_t term_w, uint64_t term, uint64_t fallback)
+{
+    return term_w == term ? off : fallback;
+}
+
+// End of a bounded launch, into a follower's control block: how many entries exist, a fence, then which launch (its
+// ticket target) that count belongs to -- so that the follower can leave once it has acked and applied all of them
+__device__ __forceinline__ void fin_publish(apus_ctrl_t *pc, uint64_t entries, uint64_t target)
+{
+    st_relaxed_sys(&pc->fin_entries, entries);
+    __threadfence_system();
+    st_relaxed_sys(&pc->fin_target, target);
+}
+// follower warp: has the leader ended the launch `target`?  `entries` is then its count of entries (every lane)
+__device__ __forceinline__ bool fin_read(const apus_ctrl_t *ctrl, uint64_t target, int lane, uint64_t &entries)
+{
+    uint64_t ft = 0;
+    if (lane == 0) ft = ld_acquire_sys(&ctrl->fin_target);
+    if (__shfl_sync(0xffffffffu, ft, 0) != target) return false;
+    entries = ld_relaxed_sys(&ctrl->fin_entries);
+    return true;
+}
+
+// probe: every lane looks at one pair of the next four publish records; lane 0 reports what has been published.
+// Returns the number of new valid records, rv the lane's pair.
+__device__ __forceinline__ uint32_t cw_probe(CommitWarp &C, int lane, uint64_t &rv)
+{
+    const uint32_t nvalid = pubrec_probe(C.ring, C.seen, 4, lane, rv);
+    if (nvalid) {
+        C.published = pubrec_field(rv, nvalid - 1, PR_CUM);
+        C.seen += nvalid;
+        if (lane == 0) st_relaxed_sys(&C.ctrl->pub_seen, C.published);
+    }
+    return nvalid;
+}
+
+// quorum rank: lane i holds what replica i has acked (entries, monotone), the leader's own vote is everything it has
+// published (dare_ibv_rc.c:1736 "i == idx"); returns the largest count a majority (size/2+1, dare_ibv_rc.c:1741) holds
+__device__ __forceinline__ uint64_t cw_quorum(const CommitWarp &C, int lane)
+{
+    uint64_t v = 0;
+    if (lane < C.N && lane != C.me) v = ld_relaxed_sys(&C.ctrl->ack[lane]);
+    if (lane == C.me) v = C.published;
+    // rank: how many replicas hold at least what I hold
+    int cnt = 0;
+    for (int j = 0; j < C.N; j++) {
+        uint64_t vj = __shfl_sync(0xffffffffu, v, j);
+        cnt += (vj >= v) ? 1 : 0;
+    }
+    uint64_t cand = (lane < C.N && cnt >= C.quorum) ? v : 0;
+    for (int s = 16; s > 0; s >>= 1) {
+        uint64_t o = __shfl_xor_sync(0xffffffffu, cand, s);
+        cand = o > cand ? o : cand;
+    }
+    return cand;
+}
+
+// commit walk: map the quorum count Q to the log offset recorded at publish time -- the commit is a prefix and an entry
+// boundary (invariant I3) -- over the records in [tail, seen), four per step.  The first step reuses the probe's pairs
+// (rv, nvalid records) when they are exactly the pending records.  false: Q covers no record; else `last` is the newest
+// covered record.
+__device__ __forceinline__ bool cw_walk(const apus_devctx_t *__restrict__ cx, CommitWarp &C,
+                                        uint64_t Q, uint64_t rv, uint32_t nvalid, int lane, PubRec &last)
+{
+    bool any = false;
+    bool reuse = (C.tail + nvalid == C.seen);
+    while (C.tail != C.seen) {
+        uint64_t val = rv;
+        uint32_t nv = nvalid;
+        if (!reuse) nv = pubrec_probe(C.ring, C.tail, C.seen - C.tail < 4 ? (uint32_t)(C.seen - C.tail) : 4u, lane, val, true);
+        reuse = false;
+        // how many of these (up to four, in order) are covered by the quorum count
+        const uint32_t cm = __ballot_sync(0xffffffffu, (lane & 7) == PR_CUM && (uint32_t)(lane >> 3) < nv && val <= Q);
+        uint32_t nc = 0;
+        while (nc < 4 && ((cm >> (8 * nc)) & 1u)) nc++;
+        if (nc == 0) break;
+        last = pubrec_decode(val, nc - 1);
+        C.committed = last.cum;
+        for (uint32_t q = 0; q < nc; q++) {
+            C.bytes_rep += pubrec_field(val, q, PR_BYTES);
+            const uint64_t t0 = pubrec_field(val, q, PR_T0);
+            if ((cx->flags & APUS_FLAG_STATS) && cx->lat_ns && lane == 0) {
+                const uint64_t d = globaltimer_ns() - t0;
+                cx->lat_ns[(C.lat_count + q) & (APUS_LAT_RING - 1)] = d > 0xffffffffull ? 0xffffffffu : (uint32_t)d;
+            }
+        }
+        C.lat_count += nc; C.batches += nc;
+        C.tail += nc;
+        any = true;
+        if (nc < 4) break;
+    }
+    return any;
+}
+
+// commit stores: {commit offset, term} into every follower (dare_ibv_rc.c:1810), {commit offset, tickets} to the host,
+// and the leader's bookkeeping, in publish order (single writer)
+__device__ __forceinline__ void cw_commit(const apus_devctx_t *__restrict__ cx, CommitWarp &C, const PubRec &r, int lane)
+{
+    apus_ctrl_t *ctrl = C.ctrl;
+    apus_loghdr_t *hdr = C.hdr;
+    const uint64_t off = r.end, tickets = r.tickets;
+    if (C.peer) st_relaxed_sys_2x64(C.peer->pub_commit, off, cx->term);
+    if (lane == 0) {
+        // {commit offset, committed tickets}: ONE 16 B store into pinned host memory -- this is what
+        // releases the proxy.c:160 spinners; a 16 B host load sees a consistent pair
+        st_relaxed_sys_2x64(&C.hw->commit_off, off, tickets);
+        st_relaxed_sys(&C.hw->consumed, tickets);                 // submission-ring space
+        st_relaxed_sys(&C.hw->last_commit_ns, globaltimer_ns());
+        st_relaxed_sys(&C.seq->pub_tail, C.tail);                 // publish-ring space
+        hdr->commit = off;
+        st_relaxed_sys(&hdr->apply, off);                       // leader applies = update_state
+        hdr->end = off; hdr->tail = r.tail; hdr->old_end = off;
+        ctrl->committed = C.committed; ctrl->committed_tickets = tickets; ctrl->lat_count = C.lat_count;
+        ctrl->published = C.committed; ctrl->consumed = tickets; ctrl->next_idx = r.next_idx; ctrl->hwm = r.hwm;
+        ctrl->bytes_replicated = C.bytes_rep; ctrl->batches = C.batches;
+    }
+    C.committed_tickets = tickets;
+    C.last_progress = globaltimer_ns();
+    __syncwarp();
+}
+
+// heartbeat (dare_ibv_rc.c:868-958: the leader writes its SID into every follower's ctrl_data.hb[]): the commit warp
+// is the leader's liveness -- when the hosting process dies the context goes with it and the beats stop
+__device__ __forceinline__ void cw_heartbeat(const apus_devctx_t *__restrict__ cx, CommitWarp &C, int lane)
+{
+    if (cx->hb_period_ns && (++C.hb_spins & 0x1fu) == 0) {
+        const uint64_t now = globaltimer_ns();
+        if (now - C.last_hb >= cx->hb_period_ns) {
+            C.last_hb = now; C.hb_beat++;
+            if (C.peer) st_relaxed_sys(&C.peer->hb, term_word(C.hb_beat, cx->term));
+        }
+    }
+}
+
+// exit decision: 1 every worker finished and nothing is in flight, 2 abort (or the watchdog), 0 go on
+__device__ __forceinline__ int cw_exit(const apus_devctx_t *__restrict__ cx, CommitWarp &C, bool new_records, int lane)
+{
+    apus_seq_t *seq = C.seq;
+    int ex = 0;
+    if (lane == 0) {
+        if (!new_records && C.tail == C.seen && C.committed == C.published && ld_acquire_gpu(&seq->workers_done) == cx->n_workers) {
+            ex = 3;
+        } else if ((++C.spins & 0x3ffu) == 0) {
+            if (ld_relaxed_sys(&seq->abort_flag)) ex = 2;
+            else if (globaltimer_ns() - C.last_progress > WATCHDOG_NS && (C.tail != C.seen || C.committed != C.published) &&
+                     (cx->target != ~0ull || ld_relaxed_sys_u32(&C.hw->stop))) {
+                st_relaxed_sys(&C.hw->error, APUS_KERR_WATCHDOG_COMMIT);
+                st_relaxed_sys(&seq->abort_flag, 1);
+                ex = 2;
+            }
+        }
+    }
+    ex = __shfl_sync(0xffffffffu, ex, 0);
+    if (ex == 3) {
+        // workers are done (acquire above): any record they wrote is visible now; one more look at the ring
+        uint64_t v;
+        ex = pubrec_probe(C.ring, C.seen, 1, lane, v) ? 0 : 1;
+    }
+    return ex;
+}
+
+__device__ void leader_commit_warp(const apus_devctx_t *__restrict__ cx)
+{
+    const int lane = threadIdx.x & 31;
+    const int N = cx->group_size, me = cx->idx;
+    apus_ctrl_t *ctrl = reinterpret_cast<apus_ctrl_t *>(cx->region);
+    CommitWarp C = {ctrl, reinterpret_cast<apus_seq_t *>(cx->region + APUS_SEQ_OFF),
+                    reinterpret_cast<const apus_pubrec_t *>(cx->region + APUS_PUBRING_OFF),
+                    reinterpret_cast<apus_loghdr_t *>(cx->region + APUS_HDR_OFF), cx->hw,
+                    (lane < N && lane != me && cx->peer[lane]) ? reinterpret_cast<apus_ctrl_t *>(cx->peer[lane]) : nullptr,
+                    N, me, cx->quorum,
+                    ctrl->committed, ctrl->committed_tickets, ctrl->lat_count, ctrl->bytes_replicated, ctrl->batches,
+                    0, 0, ctrl->published, globaltimer_ns(), 0, 0, 0, globaltimer_ns() >> 10};
+    for (;;) {
+        uint64_t rv;
+        const uint32_t nvalid = cw_probe(C, lane, rv);
+        const uint64_t Q = cw_quorum(C, lane);
+        if (Q > C.committed && C.tail != C.seen) {
+            PubRec r;
+            if (cw_walk(cx, C, Q, rv, nvalid, lane, r)) cw_commit(cx, C, r, lane);
+        }
+        cw_heartbeat(cx, C, lane);
+        const int ex = cw_exit(cx, C, nvalid != 0, lane);
+        if (ex) {
+            if (ex == 1 && cx->target != ~0ull && C.peer) fin_publish(C.peer, C.committed, cx->target);
+            break;
+        }
+    }
 }
 
 // ---------------------------------------------------------------------------------
@@ -1360,7 +1490,7 @@ __device__ __forceinline__ void place_fast(const apus_devctx_t *__restrict__ cx,
     const bool nw = r.wrapped || b == L;
     uint64_t headv = r.head;
     if (S->host_head_k != 0xffffffffu) {          // a HEAD entry submitted by the host carries the new head
-        const uint64_t nh = adopt_head(headv, slot_head_value(&sl[S->host_head_k]), ne, L);
+        const uint64_t nh = adopt_head(headv, le_u64(sl[S->host_head_k].inl), ne, L);
         if (nh != headv) { headv = nh; st_relaxed_sys(&hdr->head, nh); }
     }
     // hand the turn on at once ...
@@ -1750,301 +1880,311 @@ __device__ void leader_main(const apus_devctx_t *__restrict__ cx, const uint32_t
 }
 
 // ---------------------------------------------------------------------------------
-// FOLLOWER
+// FOLLOWER: one function per phase (DESIGN.md §3c), called in order by follower_main
 // ---------------------------------------------------------------------------------
+struct FollowerAt {           // what the phases address, derived from cx once
+    apus_ctrl_t *ctrl, *lctrl;     // my control block, the leader's
+    apus_loghdr_t *hdr;
+    uint8_t *entries, *lentries;   // my log, the leader's copy of it
+    const uint32_t *index;         // the offset index the leader writes next to my log
+    apus_hostwords_t *hw;
+    uint64_t L;
+    uint32_t flags;
+    int me;
+};
+struct FollowerRep {           // the same in every thread: each updates it from the same shared words
+    uint64_t old_end;          // walk position (dare_server.c:1795)
+    uint64_t acked;            // entries walked (reply byte set) so far
+    uint64_t applied;          // apply offset (== commit as far as I hold the entries)
+    uint64_t pend_val, pend_end;   // head carried by the last HEAD entry held, and the offset right after it (L: none)
+    uint64_t last_progress;
+};
+struct FollowerPoll {          // warp 0's own
+    uint32_t spins;
+    bool suspected;
+    uint64_t host_applied;     // HOST_APPLY: the offset the application has replayed (what the leader may prune behind)
+    uint64_t last_hb, last_hb_t;   // the heartbeat word last seen, and when it changed
+    uint64_t fbeat;            // my liveness counter in the leader's HBM
+    // APUS_FLAG_PROFILE: phase_ns[0] certificates verified, [1] ns from first sight to verified, [2] verify retries
+    uint64_t cert_first_cum, cert_first_t;
+};
+
+// warp 0, every 256 spins of the poll: stop, watchdog, failure detector, host-apply report, liveness beat.  true: leave
+__device__ __forceinline__ bool f_housekeeping(const apus_devctx_t *__restrict__ cx, const FollowerAt &A, const FollowerRep &R, FollowerPoll &W, int lane)
+{
+    uint32_t stopf = 0;
+    uint64_t ha = W.host_applied;
+    if (lane == 0) {
+        if (ld_relaxed_sys_u32(&A.hw->stop)) stopf = 1;
+        else if (cx->target != ~0ull && globaltimer_ns() - R.last_progress > WATCHDOG_NS) {
+            st_relaxed_sys(&A.hw->error, APUS_KERR_WATCHDOG_FOLLOWER);
+            stopf = 1;
+        }
+        // failure detector (hb_receive_cb, dare_server.c:866-993): the leader's beats stopped
+        if (cx->hb_timeout_ns && !W.suspected && globaltimer_ns() - W.last_hb_t > cx->hb_timeout_ns)
+            st_relaxed_sys(&A.hw->leader_suspect, 1 + cx->term);
+        if (A.flags & APUS_FLAG_HOST_APPLY) ha = ld_relaxed_sys(&A.hw->host_apply);
+    }
+    if (cx->hb_timeout_ns && globaltimer_ns() - W.last_hb_t > cx->hb_timeout_ns) W.suspected = true;
+    if (lane == 0) st_relaxed_sys(&A.lctrl->fbeat[A.me], ++W.fbeat);          // I am alive (leader's failure detector)
+    stopf = __shfl_sync(0xffffffffu, stopf, 0);
+    ha = __shfl_sync(0xffffffffu, ha, 0);
+    if ((A.flags & APUS_FLAG_HOST_APPLY) && ha != W.host_applied) {
+        // apply_committed_entries advances `apply` only after do_action (dare_server.c:1939-1962): what this
+        // replica reports to the leader's pruning rule is what the HOST has replayed
+        W.host_applied = ha;
+        if (lane == 0) { A.hdr->apply = ha; st_relaxed_sys(&A.lctrl->apply_off[A.me], ha); }
+    }
+    return stopf != 0;
+}
+
+// warp 0: poll until there is news -- lane 0 the tail publish {end, entries|term} (one 16 B acquire load), lane 1 its
+// certificate half, lane 2 the commit publish {offset, term}, lane 3 the heartbeat word -- then the early ack, and the
+// news into S for the whole CTA
+__device__ __forceinline__ void f_poll(const apus_devctx_t *__restrict__ cx, const FollowerAt &A, FollowerShared *S, const FollowerRep &R,
+                                       FollowerPoll &W, int lane)
+{
+    TailPub p;
+    uint64_t c = 0, cum_seen = 0;
+    uint32_t done = 0;
+    for (;;) {
+        uint64_t x0 = 0, x1 = 0;
+        // lanes 4..15 read, SPECULATIVELY and in the same breath, the bytes where the next entry must land (a
+        // self-certifying publish names exactly that offset): when its certificate shows up the bytes are already
+        // in registers -- verification costs no second trip to memory
+        const uint64_t spec_a = (R.old_end == A.L) ? 0 : R.old_end;
+        const uint64_t spec_lo = (spec_a & ~15ull) + 16ull * (uint64_t)(lane - 4);
+        uint4 spec = make_uint4(0, 0, 0, 0);
+        if (lane == 0) ld_acquire_sys_2x64(&A.ctrl->pub_end, x0, x1);
+        else if (lane == 1) ld_relaxed_sys_2x64(&A.ctrl->pub_csum, x0, x1);
+        else if (lane == 2) ld_relaxed_sys_2x64(A.ctrl->pub_commit, x0, x1);
+        else if (lane == 3) x0 = ld_relaxed_sys(&A.ctrl->hb);
+        else if (lane < 16 && spec_lo + 16 <= A.L) spec = ld_relaxed_sys_v4(A.entries + spec_lo);
+        const uint64_t e = __shfl_sync(0xffffffffu, x0, 0), cumt = __shfl_sync(0xffffffffu, x1, 0);
+        const uint64_t csum = __shfl_sync(0xffffffffu, x0, 1), start = __shfl_sync(0xffffffffu, x1, 1);
+        p = tail_pub_decode(e, cumt, csum, start, cx->term);
+        const uint64_t coff = __shfl_sync(0xffffffffu, x0, 2), cterm = __shfl_sync(0xffffffffu, x1, 2);
+        c = commit_pub_offset(coff, cterm, cx->term, R.applied);
+        const uint64_t hbw = __shfl_sync(0xffffffffu, x0, 3);
+        uint64_t cum = p.cum;
+        bool new_entries = cum > R.acked;
+        if (new_entries && p.cert && (A.flags & APUS_FLAG_PROFILE) && cum != W.cert_first_cum) { W.cert_first_cum = cum; W.cert_first_t = globaltimer_ns(); }
+        if (new_entries && p.cert) {
+            // self-certifying publish: the bytes may still be in flight -- read them back from my own HBM until they add
+            // up to the certificate
+            const bool ok = tail_pub_verify(p, R.old_end, R.acked, A.L, cx->term, A.entries, spec, spec_lo, lane);
+            if ((A.flags & APUS_FLAG_PROFILE) && lane == 0) { if (ok) { A.ctrl->phase_ns[0]++; A.ctrl->phase_ns[1] += globaltimer_ns() - W.cert_first_t; } else A.ctrl->phase_ns[2]++; }
+            if (!ok) { new_entries = false; cum = R.acked; }   // not there yet (or not verifiable: a fenced publish will follow);
+                                                               // nothing of it may be acked or walked
+        }
+        // commit moved, and I hold entries beyond what I applied
+        const bool new_commit = (c != R.applied) && (R.old_end != A.L) && (R.applied != R.old_end);
+        if (new_entries || new_commit) { cum_seen = cum; break; }
+        // bounded launch: the leader says how many entries exist in total
+        uint64_t fe;
+        if (cx->target != ~0ull && fin_read(A.ctrl, cx->target, lane, fe) &&
+            R.acked >= fe && (R.old_end == A.L || (R.applied == R.old_end && c == R.old_end))) { done = 1; cum_seen = R.acked; break; }
+        if (hbw != W.last_hb) { W.last_hb = hbw; W.last_hb_t = globaltimer_ns(); if (lane == 0) st_relaxed_sys(&A.hw->hb_seen, hbw); }
+        if ((++W.spins & 0xffu) == 0 && f_housekeeping(cx, A, R, W, lane)) { done = 1; cum_seen = R.acked; break; }
+    }
+    // early ack: the tail publish was observed with acquire semantics (or its certificate verified), so every
+    // entry up to it is resident and visible here (invariant I2); the reply bytes follow behind the ack word
+    // unless APUS_F_FENCED_ACK asks for them first
+    if (lane == 0) {
+        if (!done && !(A.flags & APUS_FLAG_FENCED_ACK) && cum_seen > R.acked) st_relaxed_sys(&A.lctrl->ack[A.me], cum_seen);
+        S->end_seen = p.end; S->cum_seen = cum_seen; S->commit_seen = c; S->done = done;
+        S->cert = (cum_seen > R.acked) ? p.cert : 0u; S->cert_start = p.start;
+    }
+}
+
+// all threads, index mode: the entries in (acked, cum_seen] are found through the offset index the leader wrote next to
+// the bytes; reply[me] = 1 in my copy and in the leader's (dare_ibv_rc.c:1833-1854)
+__device__ __forceinline__ void f_ack_index(const apus_devctx_t *__restrict__ cx, const FollowerAt &A, FollowerShared *S, FollowerRep &R,
+                                            uint64_t cum_seen, uint64_t end_seen, int tid, int nthr)
+{
+    const uint64_t n = cum_seen - R.acked;
+    if (tid == 0) S->head_j = 0;
+    __syncthreads();
+    // FIDX index words per thread are loaded together before any is used: one round trip per FIDX * nthr
+    // entries, not per nthr (a batch of a few tiles is thousands of entries)
+    constexpr int FIDX = 8;
+    for (uint64_t j0 = tid; j0 < n; j0 += (uint64_t)FIDX * nthr) {
+        uint32_t w[FIDX];
+#pragma unroll
+        for (int q = 0; q < FIDX; q++) {
+            const uint64_t j = j0 + (uint64_t)q * nthr;
+            w[q] = 0;
+            // (a self-certified publish names its one entry itself: its index word may still be in flight)
+            if (j < n) w[q] = S->cert ? (uint32_t)S->cert_start : ld_relaxed_sys_u32(&A.index[(uint32_t)(R.acked + 1 + j) & cx->idx_mask]);
+        }
+#pragma unroll
+        for (int q = 0; q < FIDX; q++) {
+            const uint64_t j = j0 + (uint64_t)q * nthr;
+            if (j >= n) break;
+            const uint64_t at = (uint64_t)(w[q] & ~APUS_IDX_HEAD_FLAG) + E_REPLY + (uint64_t)A.me;
+            st_relaxed_sys_u8(A.entries + at, 1);
+            st_relaxed_sys_u8(A.lentries + at, 1);
+            if (w[q] & APUS_IDX_HEAD_FLAG) atomicMax(&S->head_j, (uint32_t)(j + 1));
+        }
+    }
+    __syncthreads();
+    if (S->head_j) {
+        // poll_config_entries (dare_server.c:2163-2170): remember the head this entry carries
+        const uint32_t w = ld_relaxed_sys_u32(&A.index[(uint32_t)(R.acked + S->head_j) & cx->idx_mask]);
+        const uint64_t off = (uint64_t)(w & ~APUS_IDX_HEAD_FLAG);
+        R.pend_val = ld_relaxed_sys_u64_any(A.entries, off + E_DATA);
+        R.pend_end = (off + APUS_HDR_BYTES == A.L) ? 0 : off + APUS_HDR_BYTES;
+    }
+    R.old_end = end_seen;
+}
+
+// all threads, walk mode (APUS_F_FOLLOWER_WALK): parse the new bytes [old_end, end_seen) like the reference follower,
+// window by window through shared memory; reply[me] = 1 in my copy and in the leader's (dare_ibv_rc.c:1833-1854)
+__device__ __forceinline__ void f_ack_walk(const FollowerAt &A, FollowerShared *S, uint8_t *win, FollowerRep &R,
+                                           uint64_t cum_seen, uint64_t end_seen, int tid, int nthr)
+{
+    uint64_t walked = 0;
+    while (R.old_end != end_seen) {
+        // window: contiguous bytes from old_end up to end_seen or the end of the ring
+        if (tid == 0) {
+            uint64_t lo = (R.old_end == A.L) ? 0 : R.old_end;
+            if (A.L - lo < APUS_HDR_BYTES) lo = 0;                 // log_get_entry: header does not fit -> 0
+            uint64_t hi = (end_seen > lo) ? end_seen : A.L;       // wrapped: first run to the ring's end
+            if (lo == end_seen) hi = lo;
+            if (hi - (lo & ~15ull) > APUS_FOLLOWER_WIN_BYTES) hi = (lo & ~15ull) + APUS_FOLLOWER_WIN_BYTES;
+            S->win_lo = lo; S->win_hi = hi;
+        }
+        __syncthreads();
+        const uint64_t lo = S->win_lo, hi = S->win_hi;
+        if (lo == hi) { R.old_end = lo; break; }
+        const uint64_t lo16 = lo & ~15ull;
+        const uint32_t nch = (uint32_t)(((hi + 15ull) & ~15ull) - lo16) >> 4;
+        cta_fetch_chunks(win, A.entries + lo16, nch, tid, nthr);
+        __syncthreads();
+        // serial walk over headers in shared memory (log_get_entry / log_fit_entry / log_entry_len)
+        if (tid == 0) {
+            uint64_t off = lo;
+            uint32_t n = 0;
+            uint64_t next = off;
+            bool wrapped = false;
+            uint64_t hv = 0, he = A.L;
+            while (off < hi) {
+                if (A.L - off < APUS_HDR_BYTES) { next = 0; wrapped = true; break; }   // jump to 0
+                if (hi - off < APUS_HDR_BYTES) { next = off; break; }                // header not in window yet
+                const uint8_t *e = win + (off - lo16);
+                const uint32_t ty = e[E_TYPE];
+                const uint32_t ln = (uint32_t)e[E_DATA] | ((uint32_t)e[E_DATA + 1] << 8);
+                const uint32_t es = entry_stride(ty, ln);
+                if (A.L - off < es) { next = 0; wrapped = true; break; }              // ghost: entry continues at 0
+                if (off + es > hi) { next = off; break; }                            // entry crosses the window
+                if (ty == T_HEAD) {                                                  // poll_config_entries (dare_server.c:2163-2170)
+                    hv = le_u64(e + E_DATA);
+                    he = (off + es == A.L) ? 0 : off + es;
+                }
+                S->off[n++] = (uint32_t)(off - lo);
+                off += es;
+                next = off;
+            }
+            if (!wrapped && next == A.L) next = 0;      // rule E1 on walker offsets
+            S->n = n; S->next = next;
+            S->head_val = hv; S->head_end = he;
+        }
+        __syncthreads();
+        const uint32_t n = S->n;
+        for (uint32_t k = tid; k < n; k += nthr) {
+            const uint64_t at = lo + S->off[k] + E_REPLY + (uint64_t)A.me;
+            st_relaxed_sys_u8(A.entries + at, 1);
+            st_relaxed_sys_u8(A.lentries + at, 1);
+        }
+        __syncthreads();
+        const uint64_t next = S->next;
+        if (n == 0 && next == R.old_end) {
+            // no progress possible inside this window: protocol error
+            if (tid == 0) st_relaxed_sys(&A.hw->error, APUS_KERR_BAD_ENTRY);
+            R.old_end = end_seen;
+            break;
+        }
+        if (S->head_end != A.L) { R.pend_val = S->head_val; R.pend_end = S->head_end; }
+        walked += n;
+        R.old_end = next;
+    }
+    if (R.acked + walked != cum_seen && tid == 0) st_relaxed_sys(&A.hw->error, APUS_KERR_COUNT_MISMATCH);
+}
+
+// either mode, the batch is persisted: the ack word (APUS_F_FENCED_ACK: only now, behind a fence over the reply bytes),
+// then the header and control words
+__device__ __forceinline__ void f_persist(const FollowerAt &A, FollowerRep &R, uint64_t cum_seen,
+                                          uint64_t end_seen, int tid)
+{
+    R.acked = cum_seen;
+    if (tid == 0) {
+        if (A.flags & APUS_FLAG_FENCED_ACK) {
+            __threadfence_system();                      // reply bytes before the ack word
+            st_relaxed_sys(&A.lctrl->ack[A.me], R.acked);   // the word the leader's quorum ranking polls
+        }
+        A.hdr->end = end_seen; A.hdr->old_end = R.old_end;
+        A.ctrl->acked = R.acked;
+        A.ctrl->pend_head_val = R.pend_val; A.ctrl->pend_head_end = R.pend_end;
+    }
+    R.last_progress = globaltimer_ns();
+}
+
+// all threads: follow the commit offset (invariant I4: never beyond what I hold), and adopt the head of a committed
+// HEAD entry
+__device__ __forceinline__ void f_follow_commit(const FollowerAt &A, FollowerRep &R, uint64_t commit_seen, int tid)
+{
+    if (R.old_end == A.L || R.applied == R.old_end || commit_seen == R.applied) return;
+    const uint64_t from = R.applied;
+    const uint64_t held = ring_dist(from, R.old_end, A.L);          // bytes I hold beyond `applied`
+    uint64_t want = ring_dist(from, commit_seen, A.L);
+    uint64_t to = commit_seen;
+    if (want > held) { want = held; to = R.old_end; }             // the leader clamps the same way (dare_ibv_rc.c:1783-1787)
+    if (!want) return;
+    if (R.pend_end != A.L) {
+        const uint64_t dh = ring_dist(from, R.pend_end, A.L);
+        if (dh > 0 && dh <= want) {
+            // the HEAD entry is committed: adopt the head it carries (dare_server.c:2166-2169, 2182-2186)
+            if (tid == 0) { A.hdr->head = R.pend_val; A.ctrl->pend_head_end = A.L; }
+            R.pend_end = A.L;
+        }
+    }
+    R.applied = to;
+    if (tid == 0) {
+        A.hdr->commit = R.applied;              // what this replica knows committed AND holds (I4)
+        if (!(A.flags & APUS_FLAG_HOST_APPLY)) {
+            A.hdr->apply = R.applied;           // library use: nothing replays the log on the host
+            st_relaxed_sys(&A.lctrl->apply_off[A.me], R.applied);
+        }
+        // the host may replay [its apply, applied): everything before `applied` is committed and held here
+        st_relaxed_sys_2x64(&A.hw->commit_off, R.applied, R.acked);
+    }
+    R.last_progress = globaltimer_ns();
+}
+
 __device__ void follower_main(const apus_devctx_t *__restrict__ cx)
 {
     FollowerShared *S = reinterpret_cast<FollowerShared *>(smem_raw);
     uint8_t *win = smem_raw + FS_BYTES;
     const int tid = threadIdx.x, nthr = blockDim.x;
-    const int me = cx->idx, ldr = cx->leader_idx;
     apus_ctrl_t *ctrl = reinterpret_cast<apus_ctrl_t *>(cx->region);
     apus_loghdr_t *hdr = reinterpret_cast<apus_loghdr_t *>(cx->region + APUS_HDR_OFF);
-    uint8_t *entries = cx->region + cx->entries_off;
-    apus_hostwords_t *hw = cx->hw;
-    uint8_t *lregion = cx->peer[ldr];
-    apus_ctrl_t *lctrl = reinterpret_cast<apus_ctrl_t *>(lregion);
-    uint8_t *lentries = lregion + cx->entries_off;
-    const uint64_t L = cx->log_len;
-    const bool fenced = (cx->flags & APUS_FLAG_FENCED_ACK) != 0;
-    const bool walk = (cx->flags & APUS_FLAG_WALK) != 0;
-    const uint32_t *index = reinterpret_cast<const uint32_t *>(cx->region + APUS_INDEX_OFF);
-
-    uint64_t old_end = hdr->old_end;     // walk position (dare_server.c:1795)
-    uint64_t acked = ctrl->acked;        // entries walked (reply byte set) so far
-    uint64_t applied = hdr->apply;       // apply offset (== commit as far as I hold the entries)
-    uint64_t pend_val = ctrl->pend_head_val, pend_end = ctrl->pend_head_end;
-    uint64_t last_progress = globaltimer_ns();
-    uint32_t spins = 0;
-
-    const bool host_apply = (cx->flags & APUS_FLAG_HOST_APPLY) != 0;
-    uint64_t host_applied = hdr->apply;  // HOST_APPLY: the offset the application has replayed (what the leader may prune behind)
-    uint64_t last_hb = ld_relaxed_sys(&ctrl->hb), last_hb_t = globaltimer_ns();
-    bool suspected = false;
-    const bool fstat = (cx->flags & APUS_FLAG_PROFILE) != 0;     // follower profiling: phase_ns[0] certificates verified,
-    uint64_t cert_first_cum = 0, cert_first_t = 0, fbeat = globaltimer_ns() >> 8;               // [1] ns from first sight to verified, [2] verify retries
+    const FollowerAt A = {ctrl, reinterpret_cast<apus_ctrl_t *>(cx->peer[cx->leader_idx]), hdr,
+                          cx->region + cx->entries_off, cx->peer[cx->leader_idx] + cx->entries_off,
+                          reinterpret_cast<const uint32_t *>(cx->region + APUS_INDEX_OFF), cx->hw, cx->log_len, cx->flags, cx->idx};
+    FollowerRep R = {hdr->old_end, ctrl->acked, hdr->apply, ctrl->pend_head_val, ctrl->pend_head_end, globaltimer_ns()};
+    FollowerPoll W = {0, false, hdr->apply, ld_relaxed_sys(&ctrl->hb), globaltimer_ns(), globaltimer_ns() >> 8, 0, 0};
 
     for (;;) {
-        if (tid < 32) {
-            // warp 0 polls: lane 0 the tail publish {end, entries|term} (one 16 B acquire load), lane 1 its certificate half,
-            // lane 2 the commit publish {offset, term}, lane 3 the heartbeat word
-            const int lane = tid;
-            uint64_t e = 0, cumt = 0, c = 0, cert_start = 0;
-            uint32_t done = 0, is_cert = 0;
-            for (;;) {
-                uint64_t x0 = 0, x1 = 0;
-                // lanes 4..15 read, SPECULATIVELY and in the same breath, the bytes where the next entry must land (a
-                // self-certifying publish names exactly that offset): when its certificate shows up the bytes are already
-                // in registers -- verification costs no second trip to memory
-                const uint64_t spec_a = (old_end == L) ? 0 : old_end;
-                const uint64_t spec_lo = (spec_a & ~15ull) + 16ull * (uint64_t)(lane - 4);
-                uint4 spec = make_uint4(0, 0, 0, 0);
-                if (lane == 0) ld_acquire_sys_2x64(&ctrl->pub_end, x0, x1);
-                else if (lane == 1) ld_relaxed_sys_2x64(&ctrl->pub_csum, x0, x1);
-                else if (lane == 2) ld_relaxed_sys_2x64(ctrl->pub_commit, x0, x1);
-                else if (lane == 3) x0 = ld_relaxed_sys(&ctrl->hb);
-                else if (lane < 16 && spec_lo + 16 <= L) spec = ld_relaxed_sys_v4(entries + spec_lo);
-                e = __shfl_sync(0xffffffffu, x0, 0); cumt = __shfl_sync(0xffffffffu, x1, 0);
-                const uint64_t csum = __shfl_sync(0xffffffffu, x0, 1);
-                cert_start = __shfl_sync(0xffffffffu, x1, 1);
-                c = __shfl_sync(0xffffffffu, x0, 2);
-                if (__shfl_sync(0xffffffffu, x1, 2) != cx->term) c = applied;     // term fence on the commit publish too
-                const uint64_t hbw = __shfl_sync(0xffffffffu, x0, 3);
-                // term fence: a publish stamped with another term (a deposed leader still storing) is not looked at
-                uint64_t cum = term_word_is(cumt, cx->term) ? cumt & APUS_PUB_CUM_MASK : 0;
-                is_cert = (e & APUS_PUB_CERT) ? 1u : 0u;
-                e &= ~APUS_PUB_CERT;
-                bool new_entries = cum > acked;
-                if (new_entries && is_cert && fstat && cum != cert_first_cum) { cert_first_cum = cum; cert_first_t = globaltimer_ns(); }
-                if (new_entries && is_cert) {
-                    // self-certifying publish of ONE entry at cert_start: the bytes may still be in flight -- read them back
-                    // from my own HBM until they add up to the certificate
-                    const uint64_t a = cert_start, b = (e == 0) ? L : e;
-                    bool ok = cum == acked + 1 && a == ((old_end == L) ? 0 : old_end) && b > a && b - a <= 32u * 16u - 16u;
-                    if (ok) {
-                        const uint64_t a16 = a & ~15ull;
-                        const uint32_t nch = (uint32_t)(((b + 15ull) & ~15ull) - a16) >> 4;
-                        uint64_t cs = 0;
-                        if (nch <= 12) {                  // the speculative read covers it (lane 4 + c holds chunk c)
-                            if (lane >= 4 && lane < 4 + (int)nch) cs = cs_chunk(spec, spec_lo, a, b);
-                        } else if (lane < (int)nch) cs = cs_chunk(ld_relaxed_sys_v4(entries + a16 + 16ull * lane), a16 + 16ull * lane, a, b);
-#pragma unroll
-                        for (int sft = 16; sft > 0; sft >>= 1) cs += __shfl_xor_sync(0xffffffffu, cs, sft);
-                        ok = (cs + cs_key(cumt)) == csum;
-                    }
-                    if (fstat && lane == 0) { if (ok) { ctrl->phase_ns[0]++; ctrl->phase_ns[1] += globaltimer_ns() - cert_first_t; } else ctrl->phase_ns[2]++; }
-                    if (!ok) { new_entries = false; cum = acked; }   // not there yet (or not verifiable: a fenced publish will follow);
-                                                                     // nothing of it may be acked or walked
-                }
-                // commit moved, and I hold entries beyond what I applied
-                const bool new_commit = (c != applied) && (old_end != L) && (applied != old_end);
-                if (new_entries || new_commit) { cumt = cum; break; }
-                // bounded launch: the leader says how many entries exist in total
-                if (cx->target != ~0ull) {
-                    uint64_t ft = 0;
-                    if (lane == 0) ft = ld_acquire_sys(&ctrl->fin_target);
-                    ft = __shfl_sync(0xffffffffu, ft, 0);
-                    if (ft == cx->target) {
-                        const uint64_t fe = ld_relaxed_sys(&ctrl->fin_entries);
-                        if (acked >= fe && (old_end == L || (applied == old_end && c == old_end))) { done = 1; cumt = acked; break; }
-                    }
-                }
-                if (hbw != last_hb) { last_hb = hbw; last_hb_t = globaltimer_ns(); if (lane == 0) st_relaxed_sys(&hw->hb_seen, hbw); }
-                if ((++spins & 0xffu) == 0) {
-                    uint32_t stopf = 0;
-                    uint64_t ha = host_applied;
-                    if (lane == 0) {
-                        if (ld_relaxed_sys_u32(&hw->stop)) stopf = 1;
-                        else if (cx->target != ~0ull && globaltimer_ns() - last_progress > WATCHDOG_NS) {
-                            st_relaxed_sys(&hw->error, APUS_KERR_WATCHDOG_FOLLOWER);
-                            stopf = 1;
-                        }
-                        // failure detector (hb_receive_cb, dare_server.c:866-993): the leader's beats stopped
-                        if (cx->hb_timeout_ns && !suspected && globaltimer_ns() - last_hb_t > cx->hb_timeout_ns)
-                            st_relaxed_sys(&hw->leader_suspect, 1 + cx->term);
-                        if (host_apply) ha = ld_relaxed_sys(&hw->host_apply);
-                    }
-                    if (cx->hb_timeout_ns && globaltimer_ns() - last_hb_t > cx->hb_timeout_ns) suspected = true;
-                    if (lane == 0) st_relaxed_sys(&lctrl->fbeat[me], ++fbeat);          // I am alive (leader's failure detector)
-                    stopf = __shfl_sync(0xffffffffu, stopf, 0);
-                    ha = __shfl_sync(0xffffffffu, ha, 0);
-                    if (host_apply && ha != host_applied) {
-                        // apply_committed_entries advances `apply` only after do_action (dare_server.c:1939-1962): what this
-                        // replica reports to the leader's pruning rule is what the HOST has replayed
-                        host_applied = ha;
-                        if (lane == 0) { hdr->apply = ha; st_relaxed_sys(&lctrl->apply_off[me], ha); }
-                    }
-                    if (stopf) { done = 1; cumt = acked; break; }
-                }
-            }
-            // early ack: the tail publish was observed with acquire semantics (or its certificate verified), so every
-            // entry up to it is resident and visible here (invariant I2); the reply bytes follow behind the ack word
-            // unless APUS_F_FENCED_ACK asks for them first
-            if (lane == 0) {
-                if (!done && !fenced && cumt > acked) st_relaxed_sys(&lctrl->ack[me], cumt);
-                S->end_seen = e; S->cum_seen = cumt; S->commit_seen = c; S->done = done;
-                S->cert = (cumt > acked) ? is_cert : 0u; S->cert_start = cert_start;
-            }
-        }
+        if (tid < 32) f_poll(cx, A, S, R, W, tid);
         __syncthreads();
         if (S->done) break;
         const uint64_t end_seen = S->end_seen, cum_seen = S->cum_seen, commit_seen = S->commit_seen;
-
-        // ---- persist + ack every new entry in [old_end, end_seen) -----------------------
-        if (cum_seen > acked && !walk) {
-            // entry boundaries come from the offset index the leader wrote next to the bytes
-            const uint64_t n = cum_seen - acked;
-            if (tid == 0) S->head_j = 0;
-            __syncthreads();
-            // FIDX index words per thread are loaded together before any is used: one round trip per FIDX * nthr
-            // entries, not per nthr (a batch of a few tiles is thousands of entries)
-            constexpr int FIDX = 8;
-            for (uint64_t j0 = tid; j0 < n; j0 += (uint64_t)FIDX * nthr) {
-                uint32_t w[FIDX];
-#pragma unroll
-                for (int q = 0; q < FIDX; q++) {
-                    const uint64_t j = j0 + (uint64_t)q * nthr;
-                    w[q] = 0;
-                    // (a self-certified publish names its one entry itself: its index word may still be in flight)
-                    if (j < n) w[q] = S->cert ? (uint32_t)S->cert_start : ld_relaxed_sys_u32(&index[(uint32_t)(acked + 1 + j) & cx->idx_mask]);
-                }
-#pragma unroll
-                for (int q = 0; q < FIDX; q++) {
-                    const uint64_t j = j0 + (uint64_t)q * nthr;
-                    if (j >= n) break;
-                    const uint64_t at = (uint64_t)(w[q] & ~APUS_IDX_HEAD_FLAG) + E_REPLY + (uint64_t)me;
-                    st_relaxed_sys_u8(entries + at, 1);         // reply[me] = 1 in my copy and in the
-                    st_relaxed_sys_u8(lentries + at, 1);        // leader's (dare_ibv_rc.c:1833-1854)
-                    if (w[q] & APUS_IDX_HEAD_FLAG) atomicMax(&S->head_j, (uint32_t)(j + 1));
-                }
-            }
-            __syncthreads();
-            if (S->head_j) {
-                // poll_config_entries (dare_server.c:2163-2170): remember the head this entry carries
-                const uint32_t w = ld_relaxed_sys_u32(&index[(uint32_t)(acked + S->head_j) & cx->idx_mask]);
-                const uint64_t off = (uint64_t)(w & ~APUS_IDX_HEAD_FLAG);
-                pend_val = ld_relaxed_sys(entries + ((off + E_DATA) & ~7ull));
-                if ((off + E_DATA) & 7ull) {
-                    uint64_t hv = 0;
-                    for (int q = 7; q >= 0; q--) hv = (hv << 8) | (uint64_t)(ld_relaxed_sys_u32(entries + ((off + E_DATA + q) & ~3ull)) >> (8 * ((off + E_DATA + q) & 3ull)) & 0xffu);
-                    pend_val = hv;
-                }
-                pend_end = (off + APUS_HDR_BYTES == L) ? 0 : off + APUS_HDR_BYTES;
-            }
-            old_end = end_seen;
-        } else if (cum_seen > acked) {
-            uint64_t walked = 0;
-            while (old_end != end_seen) {
-                // window: contiguous bytes from old_end up to end_seen or the end of the ring
-                if (tid == 0) {
-                    uint64_t lo = (old_end == L) ? 0 : old_end;
-                    if (L - lo < APUS_HDR_BYTES) lo = 0;                 // log_get_entry: header does not fit -> 0
-                    uint64_t hi = (end_seen > lo) ? end_seen : L;       // wrapped: first run to the ring's end
-                    if (lo == end_seen) hi = lo;
-                    if (hi - (lo & ~15ull) > APUS_FOLLOWER_WIN_BYTES) hi = (lo & ~15ull) + APUS_FOLLOWER_WIN_BYTES;
-                    S->win_lo = lo; S->win_hi = hi;
-                }
-                __syncthreads();
-                const uint64_t lo = S->win_lo, hi = S->win_hi;
-                if (lo == hi) { old_end = lo; break; }
-                const uint64_t lo16 = lo & ~15ull;
-                const uint32_t nch = (uint32_t)(((hi + 15ull) & ~15ull) - lo16) >> 4;
-                cta_fetch_chunks(win, entries + lo16, nch, tid, nthr);
-                __syncthreads();
-                // serial walk over headers in shared memory (log_get_entry / log_fit_entry / log_entry_len)
-                if (tid == 0) {
-                    uint64_t off = lo;
-                    uint32_t n = 0;
-                    uint64_t next = off;
-                    bool wrapped = false;
-                    uint64_t hv = 0, he = L;
-                    while (off < hi) {
-                        if (L - off < APUS_HDR_BYTES) { next = 0; wrapped = true; break; }   // jump to 0
-                        if (hi - off < APUS_HDR_BYTES) { next = off; break; }                // header not in window yet
-                        const uint8_t *e = win + (off - lo16);
-                        const uint32_t ty = e[E_TYPE];
-                        const uint32_t ln = (uint32_t)e[E_DATA] | ((uint32_t)e[E_DATA + 1] << 8);
-                        const uint32_t es = entry_stride(ty, ln);
-                        if (L - off < es) { next = 0; wrapped = true; break; }              // ghost: entry continues at 0
-                        if (off + es > hi) { next = off; break; }                            // entry crosses the window
-                        if (ty == T_HEAD) {                                                  // poll_config_entries (dare_server.c:2163-2170)
-                            hv = 0;
-                            for (int q = 7; q >= 0; q--) hv = (hv << 8) | e[E_DATA + q];
-                            he = (off + es == L) ? 0 : off + es;
-                        }
-                        S->off[n++] = (uint32_t)(off - lo);
-                        off += es;
-                        next = off;
-                    }
-                    if (!wrapped && next == L) next = 0;      // rule E1 on walker offsets
-                    S->n = n; S->next = next;
-                    S->head_val = hv; S->head_end = he;
-                }
-                __syncthreads();
-                const uint32_t n = S->n;
-                // reply[me] = 1 in my copy and in the leader's copy (dare_ibv_rc.c:1833-1854)
-                for (uint32_t k = tid; k < n; k += nthr) {
-                    const uint64_t at = lo + S->off[k] + E_REPLY + (uint64_t)me;
-                    st_relaxed_sys_u8(entries + at, 1);
-                    st_relaxed_sys_u8(lentries + at, 1);
-                }
-                __syncthreads();
-                const uint64_t next = S->next;
-                if (n == 0 && next == old_end) {
-                    // no progress possible inside this window: protocol error
-                    if (tid == 0) st_relaxed_sys(&hw->error, APUS_KERR_BAD_ENTRY);
-                    old_end = end_seen;
-                    break;
-                }
-                if (S->head_end != L) { pend_val = S->head_val; pend_end = S->head_end; }
-                walked += n;
-                old_end = next;
-            }
-            if (acked + walked != cum_seen && tid == 0) st_relaxed_sys(&hw->error, APUS_KERR_COUNT_MISMATCH);
+        if (cum_seen > R.acked) {
+            if (A.flags & APUS_FLAG_WALK) f_ack_walk(A, S, win, R, cum_seen, end_seen, tid, nthr);
+            else f_ack_index(cx, A, S, R, cum_seen, end_seen, tid, nthr);
+            f_persist(A, R, cum_seen, end_seen, tid);
         }
-        if (cum_seen > acked) {     // either mode: the batch is persisted
-            acked = cum_seen;
-            if (tid == 0) {
-                if (fenced) {
-                    __threadfence_system();                  // reply bytes before the ack word
-                    st_relaxed_sys(&lctrl->ack[me], acked);  // the word the leader's quorum ranking polls
-                }
-                hdr->end = end_seen; hdr->old_end = old_end;
-                ctrl->acked = acked;
-                ctrl->pend_head_val = pend_val; ctrl->pend_head_end = pend_end;
-            }
-            last_progress = globaltimer_ns();
-        }
-
-        // ---- follow the commit offset (invariant I4: never beyond what I hold) ----------
-        if (old_end != L && applied != old_end && commit_seen != applied) {
-            const uint64_t from = applied;
-            const uint64_t held = ring_dist(from, old_end, L);          // bytes I hold beyond `applied`
-            uint64_t want = ring_dist(from, commit_seen, L);
-            uint64_t to = commit_seen;
-            if (want > held) { want = held; to = old_end; }             // the leader clamps the same way (dare_ibv_rc.c:1783-1787)
-            if (want) {
-                if (pend_end != L) {
-                    const uint64_t dh = ring_dist(from, pend_end, L);
-                    if (dh > 0 && dh <= want) {
-                        // the HEAD entry is committed: adopt the head it carries (dare_server.c:2166-2169, 2182-2186)
-                        if (tid == 0) { hdr->head = pend_val; ctrl->pend_head_end = L; }
-                        pend_end = L;
-                    }
-                }
-                applied = to;
-                if (tid == 0) {
-                    hdr->commit = applied;              // what this replica knows committed AND holds (I4)
-                    if (!host_apply) {
-                        hdr->apply = applied;           // library use: nothing replays the log on the host
-                        st_relaxed_sys(&lctrl->apply_off[me], applied);
-                    }
-                    // the host may replay [its apply, applied): everything before `applied` is committed and held here
-                    st_relaxed_sys_2x64(&hw->commit_off, applied, acked);
-                }
-                last_progress = globaltimer_ns();
-            }
-        }
+        f_follow_commit(A, R, commit_seen, tid);
         __syncthreads();
     }
 }
