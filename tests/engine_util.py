@@ -73,3 +73,20 @@ def compare_group_to_oracle(group, c, exact=True):
                 if i != lead:
                     assert limg[off + 28 + i] == 1
     return eo, oo
+
+
+def host_apply_replicas(eng, n, L, mode, ring_mode, ring_slots, ring_bytes, leader_ctas=4):
+    """n connected replicas that prune on the device (APUS_F_AUTOPRUNE) with followers whose host applies the log
+    (APUS_F_HOST_APPLY): what a follower's host reports as applied is the apply offset the leader's pruning rule
+    reads.  `mode`: the follower mode flags, given to every replica."""
+    from apus_b200 import engine as E
+    nd = eng.lib().apus_device_count()
+    base = E.F_DEVICE_STATS | E.F_AUTOPRUNE | mode
+    reps = [E.Replica(i % nd, i, n, 0, 1, L, ring_mode, ring_slots, ring_bytes,
+                      base if i == 0 else base | E.F_HOST_APPLY, leader_ctas) for i in range(n)]
+    blobs = [r.export() for r in reps]
+    for r in reps:
+        for j, b in enumerate(blobs):
+            if j != r.idx:
+                r.connect(j, b)
+    return reps

@@ -87,3 +87,13 @@ def ragged_stream(n_req: int, max_len: int, conns: int = 3, leader: int = 0, see
 def stream_bytes(stream):
     """Log bytes the stream occupies (64 + len per request), ignoring wrap waste."""
     return sum(64 + len(p) for _, _, _, p in stream)
+
+
+def sized_stream(n_req: int, lo: int, hi: int, conn: int = 0, seed: int = 1234):
+    """One CONNECT, then n_req SENDs with lengths drawn from [lo, hi]."""
+    rng = np.random.default_rng(seed)
+    out = [(CONNECT, conn, 1, b"")]
+    for i in range(n_req):
+        ln = int(rng.integers(lo, hi + 1))
+        out.append((SEND, conn, 2 + i, rng.integers(0, 256, size=ln, dtype=np.uint8).tobytes()))
+    return out

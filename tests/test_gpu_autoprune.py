@@ -18,7 +18,7 @@ from test_gpu_parity import MODES, devices_for, submit_part, wrap_stream
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(240)]
 
 FOREVER = EU.FOREVER
-F_HOST_APPLY, F_AUTOPRUNE, F_STATS = 0x10, 0x4, 0x2
+F_AUTOPRUNE, F_STATS = 0x4, 0x2
 
 
 @pytest.fixture(scope="module")
@@ -158,14 +158,7 @@ def test_autoprune_head_is_the_lagging_application(eng, orc):
     stream = wrap_stream("u200", 98, L)
     requests = [(O.CONFIG, 0, 0, b"")] + stream
     step = int(0.3 * L / 264)
-    devs = devices_for(eng, n)
-    reps = [E.Replica(devs[i], i, n, 0, 1, L, eng.RING_HOST_MAPPED, 1 << 14, 4 << 20,
-                      (F_STATS | F_AUTOPRUNE) if i == 0 else (F_STATS | F_AUTOPRUNE | F_HOST_APPLY), 4) for i in range(n)]
-    blobs = [r.export() for r in reps]
-    for r in reps:
-        for j, b in enumerate(blobs):
-            if j != r.idx:
-                r.connect(j, b)
+    reps = EU.host_apply_replicas(eng, n, L, 0, eng.RING_HOST_MAPPED, 1 << 14, 4 << 20)
     lead = reps[0]
 
     class G:                                   # what EU.compare_group_to_oracle and settle() need of a Group
@@ -228,7 +221,7 @@ def test_autoprune_head_is_the_lagging_application(eng, orc):
         settle(G, t)
         end = lead.offsets()["end"]
         lc = AR.read_launch(lead, ends[-1], end, L)
-        rp.launch(lc, requests, allow_two=True)
+        rp.launch(lc, requests)             # two HEADs in a row only where the placement blocked between them
         heads = [e.value for e in lc.entries if e.typ == O.HEAD]
         assert heads == [pins[1], release], (heads, pins[1], release)
         check_heads(reps, rp, "after the release")

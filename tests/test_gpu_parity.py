@@ -400,10 +400,18 @@ def test_against_reference_golden(eng, name, n, seed):
         assert g.leader.stats()["bytes_replicated"] == gold["bytes_replicated"]
 
 
-def check_replica_images_consistent(g, L):
+def check_replica_images_consistent(g, L, request=None):
     """Size-independent properties for runs too long for the oracle: every follower
     holds exactly the leader's live log bytes (modulo reply[]), entries parse from
-    head to end with consecutive idx, HEAD entries carry offsets inside the ring."""
+    head to end with consecutive idx, HEAD entries carry offsets inside the ring.
+    With `request` (ticket -> (type, clt_id, req_id, payload)) the live region is also
+    checked against the submitted stream: counting tickets back from the last one,
+    every entry that is not a HEAD must be its request; the last HEAD carries the
+    leader's head, which every follower holds; every HEAD whose head lies in the region
+    carries an entry boundary of it not past the HEAD itself; consecutive HEADs move
+    the head by at least L/8.  The holes (bytes no append writes) and what the
+    overwritten laps held cannot be checked without those laps: the replays of
+    tests/test_gpu_prune_in_launch.py do that on smaller rings."""
     lo = g.leader.offsets()
     limg = g.leader.image()
     assert lo["commit"] == lo["end"]
@@ -417,6 +425,8 @@ def check_replica_images_consistent(g, L):
             h = int.from_bytes(limg[o + 48:o + 56].tobytes(), "little")
             assert 0 <= h < L
         assert limg[o + 27] == g.leader_idx
+    if request is not None:
+        _check_live_region(g, L, limg, lo, ents, request)
     lm = O.mask_replies(limg, ents)
     for i, r in enumerate(g.replicas):
         if i == g.leader_idx:
@@ -431,34 +441,92 @@ def check_replica_images_consistent(g, L):
     return len(ents), idx[-1]
 
 
-@pytest.mark.parametrize("n,L,payload", [(3, 1 << 20, 64), (5, 1 << 20, 200), (3, 1 << 18, 1000)])
+def _check_live_region(g, L, limg, lo, ents, request):
+    """check_replica_images_consistent's content checks of the leader's [head, end)"""
+    head = lo["head"]
+    rel = {o: (o - head) % L for o, _ in ents}                    # position in the region
+    bounds = {head} | {o for o, _ in ents} | {(o + s) % L for o, s in ents}      # head: also where a wrap skipped
+    ticket = g.tickets
+    heads = []
+    for o, stride in reversed(ents):
+        typ = int(limg[o + 26])
+        if typ == O.HEAD:
+            heads.append((o, int.from_bytes(limg[o + 48:o + 56].tobytes(), "little")))
+            continue
+        want_typ, clt, rid, payload = request(ticket)
+        got = (typ, int.from_bytes(limg[o + 24:o + 26].tobytes(), "little"),
+               int.from_bytes(limg[o + 16:o + 24].tobytes(), "little"))
+        assert got == (want_typ, clt, rid), f"entry at {o}: (type, clt_id, req_id) {got}, ticket {ticket} is {(want_typ, clt, rid)}"
+        if typ != O.CONFIG:
+            ln = int(limg[o + 48]) | int(limg[o + 49]) << 8
+            assert ln == len(payload) and stride == 64 + ln, f"entry at {o}: len {ln}, ticket {ticket} has {len(payload)}"
+            assert limg[o + 50:o + 50 + ln].tobytes() == payload, f"entry at {o}: data image of ticket {ticket}"
+        ticket -= 1
+    heads.reverse()
+    assert heads, "no HEAD entry in the live region: the leader's head was carried by none"
+    assert heads[-1][1] == head, f"the last HEAD carries {heads[-1][1]}, the leader's head is {head}"
+    for k, (o, v) in enumerate(heads):
+        if (v - head) % L <= rel[o]:                              # its head lies in the region
+            assert v in bounds, f"HEAD at {o} carries {v}, not an entry boundary of [{head}, {lo['end']})"
+        if k:
+            pv, po = heads[k - 1][1], heads[k - 1][0]
+            adv = (v - pv) % L
+            assert L // 8 <= adv <= (o - pv) % L, f"HEAD at {o}: head {pv} -> {v} moves by {adv}"
+    for i, r in enumerate(g.replicas):
+        if i != g.leader_idx:
+            assert r.offsets()["head"] == head, f"replica {i} head {r.offsets()['head']}, the last HEAD carries {head}"
+
+
+@pytest.mark.parametrize("n,L,payload", [(3, 1 << 20, 64), (5, 1 << 20, 200), (3, 1 << 18, 1000),
+                                         pytest.param(5, O.LOG_SIZE, 64, id="bench-shape-n5-64M-synth64-ctas16")])
 def test_sustained_autoprune_many_laps(eng, n, L, payload):
     """Device-side pruning (APUS_F_AUTOPRUNE): 40+ laps around a small ring in a few
-    launches, no host-side HEAD submission."""
+    launches, no host-side HEAD submission; the live region against the submitted
+    requests.  The ring of the reference's LOG_SIZE runs the benchmark's configuration:
+    five replicas, 16 leader CTAs, 2^20 device-generated 64 B requests per launch in
+    the HBM ring, two launches (four laps)."""
     from apus_b200 import engine as E
     flags = E.F_DEVICE_STATS | E.F_AUTOPRUNE
-    per, rounds = 20000, 4
+    bench = L == O.LOG_SIZE
+    per, rounds = (1 << 20, 2) if bench else (20000, 4)
+    seed = 0xA5A50000 + payload
     with eng.Group(n, devices=devices_for(eng, n), log_size=L, ring_mode=eng.RING_DEVICE,
-                   ring_slots=1 << 17, ring_bytes=64 << 20, flags=flags) as g:
+                   ring_slots=(1 << 21) if bench else 1 << 17, ring_bytes=64 << 20, flags=flags,
+                   leader_ctas=16 if bench else 0) as g:
         g.prologue()
         g.submit(S.CONNECT, 0, 1, b"")
         req = 2
         rng = np.random.default_rng(5)
+        sent = {}                                    # first req_id of a round -> its payloads
         for _ in range(rounds):
-            pl = rng.integers(0, 256, size=per * payload, dtype=np.uint8)
-            g.submit_uniform(per, payload, 0, req, pl)
+            if bench:
+                g.tickets = g.leader.submit_synth(per, S.SEND, 0, req, payload, seed) + per - 1
+            else:
+                pl = rng.integers(0, 256, size=per * payload, dtype=np.uint8)
+                sent[req] = pl
+                g.submit_uniform(per, payload, 0, req, pl)
             req += per
             g.run(timeout_ms=120_000)
         st = g.leader.stats()
         assert st["tickets_committed"] == g.tickets
         assert st["auto_heads"] > 0
         laps = (per * rounds * (64 + payload)) / L
-        assert laps > 4
-        n_live, last_idx = check_replica_images_consistent(g, L)
+        assert laps > (3.9 if bench else 4)
+
+        def request(ticket):                         # ticket 1 the CONFIG prologue, 2 the CONNECT, then req_id + 1
+            if ticket == 1:
+                return (O.CONFIG, 0, 0, b"")
+            if ticket == 2:
+                return (S.CONNECT, 0, 1, b"")
+            rid = ticket - 1
+            if bench:
+                return (S.SEND, 0, rid, E.synth_payload(seed, rid, payload))
+            first = 2 + (rid - 2) // per * per
+            k = rid - first
+            return (S.SEND, 0, rid, sent[first][k * payload:(k + 1) * payload].tobytes())
+
+        n_live, last_idx = check_replica_images_consistent(g, L, request)
         assert last_idx == g.tickets + st["auto_heads"]
-        # followers adopted a head carried by a committed HEAD entry
-        for i in range(1, n):
-            assert g.replicas[i].offsets()["head"] != 0
 
 
 # ---- golden vectors produced by the RUNNING reference (tests/golden/gen_refstack_golden.py) -----------------------
