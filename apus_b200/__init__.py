@@ -8,4 +8,5 @@ importing `apus_b200.engine` fails loudly when the library has not been built.
 from .engine import (  # noqa: F401
     APUS_OK, APUS_ERROR, APUS_RETRY, NOOP, CSM, CONFIG, HEAD, CONNECT, SEND, CLOSE,
     RING_HOST_MAPPED, RING_DEVICE, LOG_SIZE, ApusError, Group, Replica, lib, load_library,
+    F_DEVICE_APPLY, CONSUME_BAD_IDX,
 )

@@ -28,6 +28,8 @@
 
 extern "C" cudaError_t apus_launch_roles(const apus_role_t *d_roles, int n_roles, cudaStream_t stream);
 extern "C" size_t apus_kernel_smem_bytes(void);
+extern "C" cudaError_t apus_consume_load(void);
+extern "C" cudaError_t apus_consume_enqueue(const apus_consume_args_t *a, cudaStream_t stream);
 
 #define MAX_ROLES 160          /* CTAs of one fused launch: leader workers + local followers */
 static __thread char g_err[512];
@@ -171,6 +173,12 @@ struct apus_replica {
     cudaEvent_t *waits;           /* recorded right after each enqueued commit wait, not yet seen complete */
     int      n_waits, cap_waits;
     uint64_t wait_max;            /* highest ticket a stream has been made to wait for */
+    /* device consumers (APUS_F_DEVICE_APPLY, apus_consume_device): their own stream, so that host-synchronous calls on
+     * copy_stream never queue behind them */
+    cudaStream_t cons_stream;
+    cudaEvent_t ev_cons_in, ev_cons_out;   /* caller's stream -> cons_stream -> caller's stream */
+    apus_cons_state_t *cons_st;   /* consume state + 2 words per consume block (index-ring capacity / block size) */
+    pthread_mutex_t cons_mu;      /* one enqueue at a time: the two events are shared by every caller */
 };
 
 extern "C" int apus_abi_version(void) { return APUS_ABI_VERSION; }
@@ -264,6 +272,19 @@ static int replica_init(apus_replica *r, const apus_config_t *cfg, uint64_t log_
     memset(&c, 0, sizeof c);
     c.next_idx = 1;
     c.pend_head_end = log_len;   /* no HEAD entry pending */
+    if (r->cfg.flags & APUS_F_DEVICE_APPLY) {
+        /* the consumers start at offset 0 with idx 1, where the first entry goes; nothing is committed yet */
+        c.cons_cur[1] = 1;
+        c.cons_on = 1;
+        pthread_mutex_init(&r->cons_mu, NULL);
+        CK(cudaStreamCreateWithFlags(&r->cons_stream, cudaStreamNonBlocking));
+        CK(cudaEventCreateWithFlags(&r->ev_cons_in, cudaEventDisableTiming));
+        CK(cudaEventCreateWithFlags(&r->ev_cons_out, cudaEventDisableTiming));
+        const size_t sb = sizeof(apus_cons_state_t) + 16ull * ((cap + APUS_CONS_THREADS - 1) / APUS_CONS_THREADS);
+        CK(cudaMalloc(&r->cons_st, sb));
+        CK(cudaMemset(r->cons_st, 0, sb));
+        CK(apus_consume_load());
+    }
     CK(cudaMemcpy(r->region, &c, sizeof c, cudaMemcpyHostToDevice));
 
     CK(cudaHostAlloc(&r->hw, sizeof(apus_hostwords_t), cudaHostAllocMapped | cudaHostAllocPortable));
@@ -310,6 +331,10 @@ extern "C" int apus_replica_create(const apus_config_t *cfg, apus_replica_t **ou
     if (log_len > (1ull << 31)) return fail("log_size above 2 GiB is not supported (32-bit offset index)");
     uint32_t slots = cfg->ring_slots ? cfg->ring_slots : (1u << 16);
     uint32_t bytes = cfg->ring_bytes ? cfg->ring_bytes : (16u << 20);
+    if ((cfg->flags & APUS_F_DEVICE_APPLY) && (cfg->flags & APUS_F_HOST_APPLY))
+        return fail("APUS_F_DEVICE_APPLY and APUS_F_HOST_APPLY exclude each other: one consumer reports the apply offset");
+    if ((cfg->flags & APUS_F_DEVICE_APPLY) && cfg->server_idx == cfg->leader_idx)
+        return fail("APUS_F_DEVICE_APPLY is for followers");
     if (slots & (slots - 1)) return fail("ring_slots must be a power of two");
     if (bytes % 4096 || bytes < (1u << 17)) return fail("ring_bytes must be a multiple of 4096, >= 128 KiB");
     if (bytes / 16 > 0x00ffffffu) return fail("ring_bytes too large for the 24-bit descriptor offset");
@@ -353,6 +378,7 @@ extern "C" void apus_replica_destroy(apus_replica_t *r)
     }
     free(r->waits);
     if (r->ev_dsub_out) cudaStreamSynchronize(r->copy_stream);      /* device batches still packing into the rings */
+    if (r->cons_stream) cudaStreamSynchronize(r->cons_stream);      /* consume work still reading the region */
     for (int i = 0; i < APUS_MAX_SERVER_COUNT; i++)
         if (r->peer_is_ipc[i] && r->peer_ptr[i]) cudaIpcCloseMemHandle(r->peer_ptr[i]);
     if (r->cfg.ring_mode != APUS_RING_HOST_MAPPED) {
@@ -372,6 +398,10 @@ extern "C" void apus_replica_destroy(apus_replica_t *r)
     if (r->ev_stop) cudaEventDestroy(r->ev_stop);
     if (r->ev_dsub_in) cudaEventDestroy(r->ev_dsub_in);
     if (r->ev_dsub_out) cudaEventDestroy(r->ev_dsub_out);
+    if (r->cons_st) cudaFree(r->cons_st);
+    if (r->ev_cons_in) cudaEventDestroy(r->ev_cons_in);
+    if (r->ev_cons_out) cudaEventDestroy(r->ev_cons_out);
+    if (r->cons_stream) cudaStreamDestroy(r->cons_stream);
     if (r->stream) cudaStreamDestroy(r->stream);
     if (r->copy_stream) cudaStreamDestroy(r->copy_stream);
     if (r->hw) cudaFreeHost((void *)r->hw);
@@ -1387,6 +1417,51 @@ extern "C" int apus_set_applied(apus_replica_t *r, uint64_t offset)
     return APUS_OK;
 }
 
+/* ---- device consumers: committed entries straight into device memory, in stream order ----------------------- */
+extern "C" int apus_consume_device(apus_replica_t *r, uint32_t max_n, uint64_t *idx, uint8_t *types,
+                                   uint16_t *connection_ids, uint64_t *req_ids, uint16_t *lens, void *payloads,
+                                   size_t stride, uint32_t *count, void *stream)
+{
+    if (!r) return fail("null argument");
+    if (is_leader(r)) return fail("apus_consume_device: consumption is a follower's (the leader's log is its own)");
+    if (!(r->cfg.flags & APUS_F_DEVICE_APPLY)) return fail("apus_consume_device needs a replica created with APUS_F_DEVICE_APPLY");
+    if (max_n == 0) return fail("apus_consume_device: max_n is 0");
+    if (!idx || !types || !connection_ids || !req_ids || !lens || !count || (!payloads && stride)) return fail("null argument");
+    /* the kernels store whole elements: a misaligned array would fault on the device, so refuse it here */
+    if (((uintptr_t)idx | (uintptr_t)req_ids) & 7u || ((uintptr_t)connection_ids | (uintptr_t)lens) & 1u || (uintptr_t)count & 3u)
+        return fail("apus_consume_device: misaligned array (idx and req_ids need 8 B, count 4 B, connection_ids and lens 2 B)");
+    /* at most idx_cap entries lie between the cursor and what the follower holds (each is >= 64 B of one lap) */
+    const uint32_t n = max_n < r->idx_cap ? max_n : r->idx_cap;
+    apus_consume_args_t a;
+    memset(&a, 0, sizeof a);
+    a.region = r->region; a.entries_off = r->entries_off; a.log_len = r->log_len; a.stride = stride;
+    a.idx_mask = r->idx_cap - 1; a.max_n = n; a.nblk = (n + APUS_CONS_THREADS - 1) / APUS_CONS_THREADS;
+    a.st = r->cons_st; a.hw = r->hw_dev;
+    a.idx = idx; a.types = types; a.conns = connection_ids; a.req_ids = req_ids; a.lens = lens;
+    a.payloads = (uint8_t *)payloads; a.count = count;
+    DeviceGuard g(r->cfg.device);
+    StageLock sl(&r->cons_mu);
+    cudaStream_t s = (cudaStream_t)stream;
+    CK(cudaEventRecord(r->ev_cons_in, s));
+    CK(cudaStreamWaitEvent(r->cons_stream, r->ev_cons_in, 0));
+    CK(apus_consume_enqueue(&a, r->cons_stream));
+    CK(cudaEventRecord(r->ev_cons_out, r->cons_stream));
+    CK(cudaStreamWaitEvent(s, r->ev_cons_out, 0));
+    return APUS_OK;
+}
+
+extern "C" int apus_consume_status(apus_replica_t *r, uint64_t *cursor_offset, uint64_t *next_idx, uint64_t *need_stride,
+                                   uint64_t *error)
+{
+    if (!r) return fail("null argument");
+    if (!(r->cfg.flags & APUS_F_DEVICE_APPLY)) return fail("apus_consume_status needs a replica created with APUS_F_DEVICE_APPLY");
+    if (cursor_offset) *cursor_offset = r->hw->cons_cursor;
+    if (next_idx) *next_idx = r->hw->cons_next_idx ? r->hw->cons_next_idx : 1;   /* before the first call: idx 1 */
+    if (need_stride) *need_stride = r->hw->cons_need_stride;
+    if (error) *error = r->hw->cons_error;
+    return APUS_OK;
+}
+
 extern "C" uint64_t apus_leader_suspect(apus_replica_t *r) { return r ? r->hw->leader_suspect : 0; }
 extern "C" uint64_t apus_last_commit_ns(apus_replica_t *r) { return r ? r->hw->last_commit_ns : 0; }
 
@@ -1681,6 +1756,7 @@ extern "C" int apus_ctl_adjust_follower(apus_replica_t *r, uint8_t peer, uint64_
     apus_loghdr_t mh, fh; apus_ctrl_t mc, fc;
     if (own_read(r, APUS_HDR_OFF, &mh, sizeof mh) != APUS_OK || own_read(r, 0, &mc, sizeof mc) != APUS_OK) return APUS_ERROR;
     if (peer_read(r, peer, APUS_HDR_OFF, &fh, sizeof fh) != APUS_OK || peer_read(r, peer, 0, &fc, sizeof fc) != APUS_OK) return APUS_ERROR;
+    if (fc.cons_on) return fail("peer %u consumes on the device (APUS_F_DEVICE_APPLY): no log adjustment", (unsigned)peer);
     const uint64_t mine = mc.published, theirs = fc.acked;      /* idx of the last entry each of us holds */
     /* last entry we share: walk down from min(mine, theirs) comparing {offset, idx, term} (the leader's log is the
      * truth, log_find_remote_end_offset, dare_log.h:362-394).  Entries up to the follower's commit are shared by
@@ -1763,6 +1839,7 @@ extern "C" int apus_replica_disconnect(apus_replica_t *r, uint8_t peer_idx)
 extern "C" int apus_replica_set_role(apus_replica_t *r, uint8_t leader_idx, uint64_t term)
 {
     if (!r || leader_idx >= r->cfg.group_size) return fail("bad argument");
+    if (r->cfg.flags & APUS_F_DEVICE_APPLY) return fail("a replica with device consumers (APUS_F_DEVICE_APPLY) keeps its role");
     if (r->in_flight) return fail("stop the kernel first");
     DeviceGuard g(r->cfg.device);
     const bool was_leader = is_leader(r);

@@ -35,6 +35,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "apus_gpu.h"
 #include "apus_layout.h"
 #include "apus_cert.h"
 
@@ -1902,12 +1903,35 @@ struct FollowerRep {           // the same in every thread: each updates it from
 struct FollowerPoll {          // warp 0's own
     uint32_t spins;
     bool suspected;
-    uint64_t host_applied;     // HOST_APPLY: the offset the application has replayed (what the leader may prune behind)
+    uint64_t host_applied;     // HOST_APPLY / DEVICE_APPLY: the offset the application has replayed or the device
+                               // consumers have read (what the leader may prune behind), as last forwarded
     uint64_t last_hb, last_hb_t;   // the heartbeat word last seen, and when it changed
     uint64_t fbeat;            // my liveness counter in the leader's HBM
     // APUS_FLAG_PROFILE: phase_ns[0] certificates verified, [1] ns from first sight to verified, [2] verify retries
     uint64_t cert_first_cum, cert_first_t;
 };
+
+// The consumer record {committed-and-held offset, entries held} in my own control block (APUS_F_DEVICE_APPLY): the
+// bound apus_consume_device's work trusts.  Writer: the follower's thread 0, once per commit advance.  That thread read
+// the tail publish with ld.acquire.sys, which the leader stored on another GPU behind a fence.sc.sys over the entry
+// bytes and index words (or it verified a certificate and stored the entry's index word itself, f_cert_index).  A
+// release is cumulative: everything thread 0 has observed is ordered before the record for whoever acquires it.  The
+// scope is .sys, not .gpu, so that the chain stays at the scope it started at (the writes came from a peer GPU); it
+// costs one store per commit advance.  Reader: the consume work's first kernel on the same GPU, with ld.acquire.sys;
+// the kernels that read the entries run after it in stream order.
+static_assert(offsetof(apus_ctrl_t, cons_rec) == 896 && sizeof(apus_ctrl_t) == APUS_CTL_OFF,
+              "the consumer words use the spare line after turn_ns and end where the control-plane words start");
+static_assert(offsetof(apus_ctrl_t, cons_rec) % 16 == 0 && offsetof(apus_ctrl_t, cons_cur) % 16 == 0,
+              "the consumer record and the cursor are 16 B words");
+__device__ __forceinline__ void cons_publish(apus_ctrl_t *ctrl, uint64_t held_off, uint64_t held_entries)
+{
+    asm volatile("st.release.sys.global.v2.u64 [%0], {%1,%2};" ::"l"(ctrl->cons_rec), "l"(held_off), "l"(held_entries)
+                 : "memory");
+}
+__device__ __forceinline__ void cons_read(const apus_ctrl_t *ctrl, uint64_t &held_off, uint64_t &held_entries)
+{
+    ld_acquire_sys_2x64(ctrl->cons_rec, held_off, held_entries);
+}
 
 // warp 0, every 256 spins of the poll: stop, watchdog, failure detector, host-apply report, liveness beat.  true: leave
 __device__ __forceinline__ bool f_housekeeping(const apus_devctx_t *__restrict__ cx, const FollowerAt &A, const FollowerRep &R, FollowerPoll &W, int lane)
@@ -1924,14 +1948,16 @@ __device__ __forceinline__ bool f_housekeeping(const apus_devctx_t *__restrict__
         if (cx->hb_timeout_ns && !W.suspected && globaltimer_ns() - W.last_hb_t > cx->hb_timeout_ns)
             st_relaxed_sys(&A.hw->leader_suspect, 1 + cx->term);
         if (A.flags & APUS_FLAG_HOST_APPLY) ha = ld_relaxed_sys(&A.hw->host_apply);
+        else if (A.flags & APUS_FLAG_DEVICE_APPLY) ha = ld_relaxed_sys(&A.ctrl->cons_cur[0]);
     }
     if (cx->hb_timeout_ns && globaltimer_ns() - W.last_hb_t > cx->hb_timeout_ns) W.suspected = true;
     if (lane == 0) st_relaxed_sys(&A.lctrl->fbeat[A.me], ++W.fbeat);          // I am alive (leader's failure detector)
     stopf = __shfl_sync(0xffffffffu, stopf, 0);
     ha = __shfl_sync(0xffffffffu, ha, 0);
-    if ((A.flags & APUS_FLAG_HOST_APPLY) && ha != W.host_applied) {
+    if ((A.flags & (APUS_FLAG_HOST_APPLY | APUS_FLAG_DEVICE_APPLY)) && ha != W.host_applied) {
         // apply_committed_entries advances `apply` only after do_action (dare_server.c:1939-1962): what this
-        // replica reports to the leader's pruning rule is what the HOST has replayed
+        // replica reports to the leader's pruning rule is what the HOST has replayed, or what the device consumers
+        // have finished reading (the consume work moves its cursor only after its last read of those entries)
         W.host_applied = ha;
         if (lane == 0) { A.hdr->apply = ha; st_relaxed_sys(&A.lctrl->apply_off[A.me], ha); }
     }
@@ -2129,6 +2155,16 @@ __device__ __forceinline__ void f_persist(const FollowerAt &A, FollowerRep &R, u
     R.last_progress = globaltimer_ns();
 }
 
+// thread 0, APUS_F_DEVICE_APPLY, a verified self-certifying publish: store the index word of its one entry myself.  The
+// leader's store of that word carries no ordering before the publish (it may still be in flight), and device consumers
+// find entries through the index.  The value is the leader's, so the order in which the two stores land does not
+// matter; this one precedes the consumer record (cons_publish, same thread) in program order.
+__device__ __forceinline__ void f_cert_index(const apus_devctx_t *__restrict__ cx, const FollowerAt &A, const FollowerRep &R,
+                                             uint64_t cert_start)
+{
+    const_cast<uint32_t *>(A.index)[(uint32_t)(R.acked + 1) & cx->idx_mask] = (uint32_t)cert_start;
+}
+
 // all threads: follow the commit offset (invariant I4: never beyond what I hold), and adopt the head of a committed
 // HEAD entry
 __device__ __forceinline__ void f_follow_commit(const FollowerAt &A, FollowerRep &R, uint64_t commit_seen, int tid)
@@ -2151,10 +2187,11 @@ __device__ __forceinline__ void f_follow_commit(const FollowerAt &A, FollowerRep
     R.applied = to;
     if (tid == 0) {
         A.hdr->commit = R.applied;              // what this replica knows committed AND holds (I4)
-        if (!(A.flags & APUS_FLAG_HOST_APPLY)) {
+        if (!(A.flags & (APUS_FLAG_HOST_APPLY | APUS_FLAG_DEVICE_APPLY))) {
             A.hdr->apply = R.applied;           // library use: nothing replays the log on the host
             st_relaxed_sys(&A.lctrl->apply_off[A.me], R.applied);
         }
+        if (A.flags & APUS_FLAG_DEVICE_APPLY) cons_publish(A.ctrl, R.applied, R.acked);
         // the host may replay [its apply, applied): everything before `applied` is committed and held here
         st_relaxed_sys_2x64(&A.hw->commit_off, R.applied, R.acked);
     }
@@ -2182,11 +2219,267 @@ __device__ void follower_main(const apus_devctx_t *__restrict__ cx)
         if (cum_seen > R.acked) {
             if (A.flags & APUS_FLAG_WALK) f_ack_walk(A, S, win, R, cum_seen, end_seen, tid, nthr);
             else f_ack_index(cx, A, S, R, cum_seen, end_seen, tid, nthr);
+            if ((A.flags & APUS_FLAG_DEVICE_APPLY) && S->cert && tid == 0) f_cert_index(cx, A, R, S->cert_start);
             f_persist(A, R, cum_seen, end_seen, tid);
         }
         f_follow_commit(A, R, commit_seen, tid);
         __syncthreads();
     }
+}
+
+// ---------------------------------------------------------------------------------
+// DEVICE CONSUMERS (APUS_F_DEVICE_APPLY): the work of one apus_consume_device call, five kernels in stream order on
+// the replica's consume stream -- head (snapshot the record and the cursor), count (per block: rows and the first
+// entry that stops the examination), scan (where the examination stops, row offsets, the new cursor), copy (the rows),
+// tail (the row count, then the cursor and the status words).  Entries are found through the offset index, never
+// by walking bytes; they never wrap (the ghost-header rule places them at 0), so each cmd is one contiguous run.
+// ---------------------------------------------------------------------------------
+#define CONS_OK        0u
+#define CONS_LATER     1u    // not committed (yet): the examination ends here, quietly
+#define CONS_BAD_IDX   2u    // the entry at the index word does not carry the expected idx
+#define CONS_TOO_LONG  3u    // CSM-like with a cmd longer than the row stride
+#define CONS_NONE      0xffffffffu
+
+__device__ __forceinline__ uint32_t ld_relaxed_sys_u8_any(const uint8_t *entries, uint64_t at)
+{
+    return (ld_relaxed_sys_u32(entries + (at & ~3ull)) >> (8 * (at & 3ull))) & 0xffu;
+}
+__device__ __forceinline__ uint32_t ld_relaxed_sys_u16_any(const uint8_t *entries, uint64_t at)
+{
+    return ld_relaxed_sys_u8_any(entries, at) | (ld_relaxed_sys_u8_any(entries, at + 1) << 8);
+}
+
+struct ConsEntry {
+    uint64_t off;
+    uint32_t ty, len, status;
+};
+// entry j of this call: its offset from the index word, then whether it is committed (within [cursor, committed) of
+// the one lap the cursor bounds), carries idx next_idx + j, and fits a row
+__device__ __forceinline__ ConsEntry cons_classify(const apus_consume_args_t &a, const apus_cons_state_t &s, uint64_t j)
+{
+    const uint8_t *entries = a.region + a.entries_off;
+    const uint32_t *index = reinterpret_cast<const uint32_t *>(a.region + APUS_INDEX_OFF);
+    const uint64_t L = a.log_len;
+    ConsEntry e = {0, 0, 0, CONS_OK};
+    e.off = ld_relaxed_sys_u32(&index[(uint32_t)(s.next_idx + j) & a.idx_mask]) & ~APUS_IDX_HEAD_FLAG;
+    if (ring_dist(s.cursor, e.off, L) >= ring_dist(s.cursor, s.committed, L)) { e.status = CONS_LATER; return e; }
+    if (e.off + APUS_HDR_BYTES > L || ld_relaxed_sys_u64_any(entries, e.off + E_IDX) != s.next_idx + j) {
+        e.status = CONS_BAD_IDX;
+        return e;
+    }
+    e.ty = ld_relaxed_sys_u8_any(entries, e.off + E_TYPE);
+    if (has_cmd(e.ty)) {
+        e.len = ld_relaxed_sys_u16_any(entries, e.off + E_DATA);
+        if (e.off + entry_stride(e.ty, e.len) > L) e.status = CONS_BAD_IDX;   // not an entry this log could hold
+        else if (e.len > a.stride) e.status = CONS_TOO_LONG;
+    }
+    return e;
+}
+
+// exclusive prefix count of `flag` over the block (APUS_CONS_THREADS threads); *total = the block's count
+__device__ __forceinline__ uint32_t cons_block_excl(bool flag, uint32_t *total)
+{
+    __shared__ uint32_t warp_n[APUS_CONS_THREADS / 32];
+    const uint32_t lane = threadIdx.x & 31u, w = threadIdx.x >> 5;
+    const uint32_t b = __ballot_sync(0xffffffffu, flag);
+    if (lane == 0) warp_n[w] = __popc(b);
+    __syncthreads();
+    uint32_t before = 0, all = 0;
+    for (uint32_t i = 0; i < APUS_CONS_THREADS / 32; i++) {
+        if (i < w) before += warp_n[i];
+        all += warp_n[i];
+    }
+    __syncthreads();
+    *total = all;
+    return before + __popc(b & ((1u << lane) - 1u));
+}
+
+// 1: snapshot the record (acquire: the entry bytes and index words it covers are visible from here on) and the cursor
+__global__ void apus_consume_head_kernel(apus_consume_args_t a)
+{
+    apus_cons_state_t *s = a.st;
+    const apus_ctrl_t *ctrl = reinterpret_cast<const apus_ctrl_t *>(a.region);
+    uint64_t committed, held;
+    cons_read(ctrl, committed, held);
+    const uint64_t cursor = ld_relaxed_sys(&ctrl->cons_cur[0]), nidx = ld_relaxed_sys(&ctrl->cons_cur[1]);
+    const uint64_t avail = (held + 1 > nidx) ? held + 1 - nidx : 0;
+    s->cursor = cursor; s->next_idx = nidx; s->committed = committed;
+    s->m = s->error ? 0 : (avail < a.max_n ? avail : a.max_n);
+}
+
+// 2: per block, the CSM-like entries before the block's first stop, and that stop {j, reason, len}
+__global__ void __launch_bounds__(APUS_CONS_THREADS) apus_consume_count_kernel(apus_consume_args_t a)
+{
+    __shared__ uint32_t first;
+    const apus_cons_state_t s = *a.st;
+    const uint64_t j = (uint64_t)blockIdx.x * APUS_CONS_THREADS + threadIdx.x;
+    if (threadIdx.x == 0) first = CONS_NONE;
+    __syncthreads();
+    ConsEntry e = {0, 0, 0, CONS_LATER};
+    if (j < s.m) e = cons_classify(a, s, j);
+    if (j < s.m && e.status != CONS_OK) atomicMin(&first, (uint32_t)j);
+    __syncthreads();
+    const uint32_t rows = __syncthreads_count(j < s.m && e.status == CONS_OK && has_cmd(e.ty) && j < first);
+    uint64_t *blk = reinterpret_cast<uint64_t *>(a.st + 1);
+    if (threadIdx.x == 0) blk[2 * blockIdx.x] = rows;
+    if (first == CONS_NONE) {
+        if (threadIdx.x == 0) blk[2 * blockIdx.x + 1] = CONS_NONE;
+    } else if (j == first) {
+        blk[2 * blockIdx.x + 1] = (uint64_t)first | ((uint64_t)e.status << 32) | ((uint64_t)e.len << 40);
+    }
+}
+
+// 3 (one block): the first block with a stop ends the examination; exclusive scan of the rows of the blocks up to it,
+// in place; the examined count, the row count and the new cursor (end of the last examined entry, E1: L is 0)
+__global__ void __launch_bounds__(APUS_CONS_THREADS) apus_consume_scan_kernel(apus_consume_args_t a)
+{
+    __shared__ uint32_t bstop;
+    apus_cons_state_t *s = a.st;
+    uint64_t *blk = reinterpret_cast<uint64_t *>(s + 1);
+    const uint32_t nblk = (uint32_t)((s->m + APUS_CONS_THREADS - 1) / APUS_CONS_THREADS);
+    if (threadIdx.x == 0) bstop = CONS_NONE;
+    __syncthreads();
+    for (uint32_t b = threadIdx.x; b < nblk; b += APUS_CONS_THREADS)
+        if (blk[2 * b + 1] != CONS_NONE) atomicMin(&bstop, b);
+    __syncthreads();
+    const uint32_t last = bstop == CONS_NONE ? nblk : bstop + 1;     // blocks whose rows count
+    uint64_t carry = 0;
+    for (uint32_t b0 = 0; b0 < last; b0 += APUS_CONS_THREADS) {
+        const uint32_t b = b0 + threadIdx.x;
+        const uint64_t v = b < last ? blk[2 * b] : 0;
+        uint64_t incl = v;                                            // block-wide inclusive scan of v
+        __shared__ uint64_t part[APUS_CONS_THREADS / 32];
+        for (uint32_t d = 1; d < 32; d <<= 1) {
+            const uint64_t o = __shfl_up_sync(0xffffffffu, incl, d);
+            if ((threadIdx.x & 31u) >= d) incl += o;
+        }
+        if ((threadIdx.x & 31u) == 31u) part[threadIdx.x >> 5] = incl;
+        __syncthreads();
+        uint64_t before = 0, all = 0;
+        for (uint32_t i = 0; i < APUS_CONS_THREADS / 32; i++) { if (i < (threadIdx.x >> 5)) before += part[i]; all += part[i]; }
+        __syncthreads();
+        if (b < last) blk[2 * b] = carry + before + incl - v;
+        carry += all;
+    }
+    if (threadIdx.x == 0) {
+        uint64_t n_exam = s->m, need = 0;
+        if (bstop != CONS_NONE) {
+            const uint64_t w = blk[2 * bstop + 1];
+            const uint32_t why = (uint32_t)(w >> 32) & 0xffu;
+            n_exam = (uint32_t)w;
+            if (why == CONS_BAD_IDX) s->error = APUS_CONSUME_BAD_IDX;
+            if (why == CONS_TOO_LONG) need = (w >> 40) & 0xffffu;
+        }
+        uint64_t cur = s->cursor;
+        if (n_exam) {
+            const ConsEntry e = cons_classify(a, *s, n_exam - 1);
+            cur = e.off + entry_stride(e.ty, e.len);
+            if (cur == a.log_len) cur = 0;
+        }
+        s->rows = carry; s->n_exam = n_exam; s->new_cursor = cur; s->need_stride = need;
+    }
+}
+
+// `len` bytes from src (log bytes, any alignment) to dst (any alignment), by the `nthr` threads `c` of a group: each
+// writes 16 B-aligned destination chunks, built from the one or two aligned 16 B source chunks that hold them.  Only
+// chunks holding a wanted byte are loaded (they lie inside the entry); destination bytes outside [dst, dst + len) are
+// not written.
+__device__ __forceinline__ void cons_copy_cmd(uint8_t *dst, const uint8_t *src, uint32_t len, uint32_t c, uint32_t nthr)
+{
+    if (!len) return;
+    const uint64_t d = (uint64_t)(uintptr_t)dst, d16 = d & ~15ull, de = d + len;
+    const uint64_t sb = (uint64_t)(uintptr_t)src - (d - d16);         // source address of destination byte d16
+    const uint64_t s_lo = (uint64_t)(uintptr_t)src, s_hi = s_lo + len;
+    const uint32_t nch = (uint32_t)(((de + 15ull) & ~15ull) - d16) >> 4;
+    for (uint32_t q = c; q < nch; q += nthr) {
+        const uint64_t s = sb + 16ull * q, s16 = s & ~15ull;
+        const uint32_t sh = (uint32_t)(s & 15ull);
+        const uint64_t want_lo = s > s_lo ? s : s_lo, want_hi = (s + 16 < s_hi) ? s + 16 : s_hi;
+        uint4 c0 = make_uint4(0, 0, 0, 0), c1 = make_uint4(0, 0, 0, 0);
+        if (want_lo < s16 + 16) c0 = ld_relaxed_sys_v4(reinterpret_cast<const void *>(s16));
+        if (sh && want_hi > s16 + 16) c1 = ld_relaxed_sys_v4(reinterpret_cast<const void *>(s16 + 16));
+        const uint64_t a0 = c0.x | ((uint64_t)c0.y << 32), a1 = c0.z | ((uint64_t)c0.w << 32);
+        const uint64_t a2 = c1.x | ((uint64_t)c1.y << 32), a3 = c1.z | ((uint64_t)c1.w << 32);
+        const uint32_t k = sh >> 3, b = 8u * (sh & 7u);
+        const uint64_t w0 = k ? a1 : a0, w1 = k ? a2 : a1, w2 = k ? a3 : a2;
+        const uint64_t r0 = b ? (w0 >> b) | (w1 << (64u - b)) : w0, r1 = b ? (w1 >> b) | (w2 << (64u - b)) : w1;
+        const uint64_t o = d16 + 16ull * q;
+        if (o >= d && o + 16 <= de) {
+            st_v4(reinterpret_cast<void *>(o), make_uint4((uint32_t)r0, (uint32_t)(r0 >> 32), (uint32_t)r1, (uint32_t)(r1 >> 32)));
+        } else {
+            for (uint32_t i = 0; i < 16; i++)
+                if (o + i >= d && o + i < de) st_u8(reinterpret_cast<void *>(o + i), (uint32_t)(((i < 8 ? r0 : r1) >> (8 * (i & 7))) & 0xffu));
+        }
+    }
+}
+
+// 4: each block writes the rows of its entries (j < examined): one thread per entry for the fields, then eight
+// threads per entry for the cmd bytes
+__global__ void __launch_bounds__(APUS_CONS_THREADS) apus_consume_copy_kernel(apus_consume_args_t a)
+{
+    __shared__ uint64_t s_off[APUS_CONS_THREADS], s_row[APUS_CONS_THREADS];
+    __shared__ uint32_t s_len[APUS_CONS_THREADS];
+    const apus_cons_state_t s = *a.st;
+    const uint64_t *blk = reinterpret_cast<const uint64_t *>(a.st + 1);
+    const uint8_t *entries = a.region + a.entries_off;
+    if ((uint64_t)blockIdx.x * APUS_CONS_THREADS >= s.n_exam) return;          // the whole block is past the stop
+    const uint64_t j = (uint64_t)blockIdx.x * APUS_CONS_THREADS + threadIdx.x;
+    ConsEntry e = {0, 0, 0, CONS_LATER};
+    if (j < s.n_exam) e = cons_classify(a, s, j);
+    const bool live = j < s.n_exam && has_cmd(e.ty);
+    uint32_t tot;
+    const uint64_t row = blk[2 * blockIdx.x] + cons_block_excl(live, &tot);
+    if (live) {
+        a.idx[row] = s.next_idx + j;
+        a.types[row] = (uint8_t)e.ty;
+        a.conns[row] = (uint16_t)ld_relaxed_sys_u16_any(entries, e.off + E_CLTID);
+        a.req_ids[row] = ld_relaxed_sys_u64_any(entries, e.off + E_REQID);
+        a.lens[row] = (uint16_t)e.len;
+    }
+    s_off[threadIdx.x] = e.off; s_row[threadIdx.x] = row; s_len[threadIdx.x] = live ? e.len : CONS_NONE;
+    __syncthreads();
+    const uint32_t c = threadIdx.x & 7u;
+    for (uint32_t i = threadIdx.x >> 3; i < APUS_CONS_THREADS; i += APUS_CONS_THREADS / 8)
+        if (s_len[i] != CONS_NONE)
+            cons_copy_cmd(a.payloads + s_row[i] * a.stride, entries + s_off[i] + E_CMD, s_len[i], c, 8);
+}
+
+// 5: the row count, then -- every read of the examined entries has completed with the copy kernel -- the cursor the
+// follower forwards to the leader's pruning rule, and the status words
+__global__ void apus_consume_tail_kernel(apus_consume_args_t a)
+{
+    const apus_cons_state_t *s = a.st;
+    apus_ctrl_t *ctrl = reinterpret_cast<apus_ctrl_t *>(a.region);
+    *a.count = (uint32_t)s->rows;
+    const uint64_t nidx = s->next_idx + s->n_exam;
+    st_relaxed_sys_2x64(ctrl->cons_cur, s->new_cursor, nidx);
+    st_relaxed_sys(&a.hw->cons_cursor, s->new_cursor);
+    st_relaxed_sys(&a.hw->cons_next_idx, nidx);
+    st_relaxed_sys(&a.hw->cons_need_stride, s->need_stride);
+    st_relaxed_sys(&a.hw->cons_error, s->error);
+}
+
+// Under lazy module loading the first launch of a kernel loads it, and a load may wait for the resident replica
+// kernels: load the consume kernels before any launch
+extern "C" cudaError_t apus_consume_load(void)
+{
+    cudaFuncAttributes fa;
+    cudaError_t e = cudaFuncGetAttributes(&fa, apus_consume_head_kernel);
+    if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, apus_consume_count_kernel);
+    if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, apus_consume_scan_kernel);
+    if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, apus_consume_copy_kernel);
+    if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, apus_consume_tail_kernel);
+    return e;
+}
+
+extern "C" cudaError_t apus_consume_enqueue(const apus_consume_args_t *a, cudaStream_t stream)
+{
+    apus_consume_head_kernel<<<1, 1, 0, stream>>>(*a);
+    apus_consume_count_kernel<<<a->nblk, APUS_CONS_THREADS, 0, stream>>>(*a);
+    apus_consume_scan_kernel<<<1, APUS_CONS_THREADS, 0, stream>>>(*a);
+    apus_consume_copy_kernel<<<a->nblk, APUS_CONS_THREADS, 0, stream>>>(*a);
+    apus_consume_tail_kernel<<<1, 1, 0, stream>>>(*a);
+    return cudaGetLastError();
 }
 
 // ---------------------------------------------------------------------------------

@@ -117,6 +117,13 @@ typedef struct apus_ctrl {
     uint64_t phase_ns[8];        /* [0] wait for requests, [1..6] T1..T6, [7] tiles */
     uint64_t turn_ns[8];         /* worker 0: [0] claim-lock wait, [1] place-turn wait, [2] publish-turn wait (ns),
                                     [3] fast placements, [4] slow placements, [7] place-turn hold (ns) */
+    /* --- device consumers (APUS_F_DEVICE_APPLY, follower): one writer each, on this replica's own GPU --- */
+    uint64_t cons_rec[2];        /* follower kernel -> consume work: {committed-and-held offset, entries held}, one 16 B
+                                    release store per commit advance (cons_publish / cons_read) */
+    uint64_t cons_cur[2];        /* consume work -> follower kernel: {cursor offset, idx of the next entry}; the cursor is
+                                    the apply offset the follower reports to the leader's pruning rule */
+    uint64_t cons_on;            /* 1: this replica was created with APUS_F_DEVICE_APPLY (the control plane refuses it) */
+    uint64_t pad4[11];
 } apus_ctrl_t;
 
 /* Control-plane words (N1: election, votes, log adjustment), at APUS_CTL_OFF inside the ctrl block -- the part of the
@@ -230,7 +237,11 @@ typedef struct apus_hostwords {
     volatile uint64_t last_commit_ns;    /* kernel -> host: %globaltimer of the latest commit */
     volatile uint64_t dev_rejected;      /* packing kernel -> host: requests of device batches written as NOOPs ... */
     volatile uint64_t dev_first_rejected;/* ... and the ticket of the first of them (0 = none) */
-    uint64_t pad1[10];
+    volatile uint64_t cons_cursor;       /* consume work -> host (APUS_F_DEVICE_APPLY): the cursor after the latest call, */
+    volatile uint64_t cons_next_idx;     /* ... the idx of the next entry, */
+    volatile uint64_t cons_need_stride;  /* ... the stride the entry that stopped it needs (0 = none), */
+    volatile uint64_t cons_error;        /* ... and APUS_CONSUME_BAD_IDX (apus_gpu.h; 0 = none; sticky) */
+    uint64_t pad1[6];
     volatile uint32_t stop;              /* host -> kernel */
     uint32_t pad2[31];
     volatile uint64_t host_apply;        /* host -> follower kernel (APUS_FLAG_HOST_APPLY): offset up to which the
@@ -251,7 +262,9 @@ typedef struct apus_hostwords {
 #define APUS_FLAG_PROFILE    0x40u  /* %globaltimer stamps inside the express path and the follower's verification (the reads
                                        lengthen the path: kept out of measured runs) */
 
-#define APUS_PUB_CERT      (1ull << 63)          /* pub_end: this publish is self-certifying (no writer fence) */
+#define APUS_FLAG_DEVICE_APPLY 0x200u /* follower: the apply offset it reports is the device consumers' cursor */
+
+#define APUS_PUB_CERT      (1ull << 63)         /* pub_end: this publish is self-certifying (no writer fence) */
 #define APUS_PUB_TERM_SHIFT 48                   /* pub_cum / hb: term in the top 16 bits */
 #define APUS_PUB_CUM_MASK  ((1ull << 48) - 1)
 
@@ -294,6 +307,33 @@ typedef struct apus_role {
     uint32_t       worker;                /* leader: worker CTA index */
     apus_devctx_t *ctx;
 } apus_role_t;
+
+/* Device consumers (apus_consume_device): the state of one replica's consume work, in device memory ahead of two
+ * words per consume block ({rows, then their exclusive scan; stop}).  The cursor itself is apus_ctrl_t.cons_cur. */
+typedef struct apus_cons_state {
+    uint64_t cursor, next_idx, committed, m;  /* this call: the cursor and the record it starts from, entries to look at */
+    uint64_t rows, n_exam, new_cursor, need_stride;   /* ... and what it found */
+    uint64_t error;                           /* sticky APUS_CONSUME_BAD_IDX */
+    uint64_t pad[7];
+} apus_cons_state_t;
+#define APUS_CONS_THREADS 256u                /* entries per consume block */
+
+/* one apus_consume_device call as the consume kernels see it */
+typedef struct apus_consume_args {
+    uint8_t  *region;                         /* the follower's region (ctrl block, index, entries) */
+    uint64_t  entries_off, log_len, stride;
+    uint32_t  idx_mask, max_n;                /* max_n <= the index ring's capacity */
+    uint32_t  nblk, pad;
+    apus_cons_state_t *st;                    /* followed by 2 * nblk words */
+    apus_hostwords_t  *hw;                    /* status words (device address of the pinned page) */
+    uint64_t *idx;
+    uint8_t  *types;
+    uint16_t *conns;
+    uint64_t *req_ids;
+    uint16_t *lens;
+    uint8_t  *payloads;
+    uint32_t *count;
+} apus_consume_args_t;
 
 #define APUS_KERNEL_THREADS    512
 #define APUS_MAX_TILE_ENTRIES  512u             /* slots fetched per tile (48 KiB of shared memory) */

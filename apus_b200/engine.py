@@ -5,6 +5,7 @@
 """
 import ctypes as C
 import os
+from collections import namedtuple
 
 import numpy as np
 
@@ -18,6 +19,8 @@ LOG_SIZE = 16384 * 4096
 MAX_SERVERS = 13
 F_FENCED_ACK, F_DEVICE_STATS, F_AUTOPRUNE, F_FOLLOWER_WALK, F_EXPLICIT = 0x1, 0x2, 0x4, 0x8, 0x80000000
 F_HOST_APPLY, F_NO_EXPRESS, F_PROFILE, F_FABRIC = 0x10, 0x20, 0x40, 0x100
+F_DEVICE_APPLY = 0x200
+CONSUME_BAD_IDX = 1
 UINT64_MAX = (1 << 64) - 1
 
 u64, u32, u16, u8, i64, i32 = C.c_uint64, C.c_uint32, C.c_uint16, C.c_uint8, C.c_int64, C.c_int32
@@ -48,6 +51,8 @@ class Stats(C.Structure):
                                    "lat_samples", "auto_heads", "entries_published")] + [("phase_ns", u64 * 8), ("turn_ns", u64 * 8)]
 
 
+ConsumeStatus = namedtuple("ConsumeStatus", "cursor next_idx need_stride error")
+
 _lib = None
 
 EXPORTS = [
@@ -63,6 +68,7 @@ EXPORTS = [
     "apus_ctl_send_vote_ack", "apus_ctl_last_entry", "apus_ctl_adjust_follower", "apus_replica_set_role",
     "apus_replica_disconnect", "apus_follower_beats", "apus_device_numa_node", "apus_group_multicast", "apus_ctl_heartbeat",
     "apus_submit_device", "apus_device_submit_status", "apus_stream_wait_committed", "apus_committed_word",
+    "apus_consume_device", "apus_consume_status",
 ]
 
 
@@ -120,6 +126,8 @@ def load_library(path=LIB_PATH):
         L.apus_stream_wait_committed.argtypes = [vp, u64, vp]
         L.apus_committed_word.argtypes = [vp]
         L.apus_committed_word.restype = vp
+        L.apus_consume_device.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp, C.c_size_t, vp, vp]
+        L.apus_consume_status.argtypes = [vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]
     _lib = L
     return L
 
@@ -274,6 +282,54 @@ class Replica:
         rej, first = u64(), u64()
         _ck(lib().apus_device_submit_status(self.h, C.byref(rej), C.byref(first)), "apus_device_submit_status")
         return int(rej.value), int(first.value)
+
+    def consume_device(self, max_n, stride, out=None, stream=None):
+        """Follower created with F_DEVICE_APPLY: the next committed entries, at most max_n of them, into CUDA tensors
+        on this replica's device, in `stream` order (apus_consume_device).  Returns (idx int64 [max_n], types uint8
+        [max_n], conns int16 [max_n], req_ids int64 [max_n], lens int16 [max_n], payloads uint8 [max_n, stride],
+        count int32 [1]): rows 0 .. count-1 are the CSM-like entries examined; NOOP / CONFIG / HEAD entries are
+        skipped, idx shows them.  Read count after synchronising with `stream`.  `out`: those seven tensors to
+        fill (allocated when None); int16 or uint16 for conns and lens, int32 or uint32 for count."""
+        import torch
+        dev = torch.device("cuda", self.device)
+        s = self._stream(stream)
+        if out is None:
+            with torch.cuda.stream(s):
+                out = (torch.empty(max_n, dtype=torch.int64, device=dev), torch.empty(max_n, dtype=torch.uint8, device=dev),
+                       torch.empty(max_n, dtype=torch.int16, device=dev), torch.empty(max_n, dtype=torch.int64, device=dev),
+                       torch.empty(max_n, dtype=torch.int16, device=dev),
+                       torch.empty((max_n, stride), dtype=torch.uint8, device=dev),
+                       torch.empty(1, dtype=torch.int32, device=dev))
+        if len(out) != 7:
+            raise ApusError("consume_device: out must be (idx, types, conns, req_ids, lens, payloads, count)")
+        spec = (("idx", (torch.int64,), (max_n,)), ("types", (torch.uint8,), (max_n,)),
+                ("conns", (torch.int16, torch.uint16), (max_n,)), ("req_ids", (torch.int64,), (max_n,)),
+                ("lens", (torch.int16, torch.uint16), (max_n,)), ("payloads", (torch.uint8,), (max_n, stride)),
+                ("count", (torch.int32, torch.uint32), (1,)))
+        for (name, dtypes, shape), t in zip(spec, out):
+            if not isinstance(t, torch.Tensor):
+                raise ApusError(f"consume_device: {name} must be a torch tensor")
+            if t.device != dev:
+                raise ApusError(f"consume_device: {name} is on {t.device}, the replica is on {dev}")
+            if t.dtype not in dtypes:
+                raise ApusError(f"consume_device: {name} has dtype {t.dtype}, expected one of {dtypes}")
+            if tuple(t.shape) != shape:
+                raise ApusError(f"consume_device: {name} has shape {tuple(t.shape)}, expected {shape}")
+            if not t.is_contiguous():
+                raise ApusError(f"consume_device: {name} is not contiguous")
+        idx, types, conns, req_ids, lens, payloads, count = out
+        _ck(lib().apus_consume_device(self.h, max_n, idx.data_ptr(), types.data_ptr(), conns.data_ptr(),
+                                      req_ids.data_ptr(), lens.data_ptr(), payloads.data_ptr() if stride else None,
+                                      stride, count.data_ptr(), s.cuda_stream), "apus_consume_device")
+        return out
+
+    def consume_status(self):
+        """(cursor offset, idx of the next entry, stride the entry that stopped the latest call needs or 0,
+        CONSUME_* error or 0), as the latest consume call that ran left them"""
+        cur, nidx, need, err = u64(), u64(), u64(), u64()
+        _ck(lib().apus_consume_status(self.h, C.byref(cur), C.byref(nidx), C.byref(need), C.byref(err)),
+            "apus_consume_status")
+        return ConsumeStatus(int(cur.value), int(nidx.value), int(need.value), int(err.value))
 
     def wait_committed_on_stream(self, ticket, stream=None):
         """make `stream` (default: the current stream of the leader's device) wait until `ticket` is committed"""

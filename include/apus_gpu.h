@@ -82,6 +82,9 @@ extern "C" {
 #define APUS_F_FABRIC      0x100u /* the replica's HBM region is a VMM allocation that apus_group_multicast() can bind to an
                                      NVSwitch multicast object (replicas of one process, one GPU each) */
 #define APUS_F_PROFILE      0x40u /* fine-grained device timestamps in the latency path (diagnostic runs only: each is a %globaltimer read) */
+#define APUS_F_DEVICE_APPLY 0x200u /* follower: the apply offset reported to the leader's pruning rule is the cursor of
+                                     the device consumers (apus_consume_device), the device counterpart of
+                                     APUS_F_HOST_APPLY.  Refused together with APUS_F_HOST_APPLY and on a leader */
 #define APUS_F_EXPLICIT     0x80000000u /* flags are exactly as given (no defaults OR-ed in) */
 
 typedef struct apus_replica apus_replica_t;
@@ -262,6 +265,32 @@ int  apus_set_applied(apus_replica_t *r, uint64_t offset);
 /* copy the committed-and-held range [from, to) of the circular log (it may wrap) into dst (capacity cap);
  * *got = bytes copied.  One or two device->host copies through a pinned buffer. */
 int  apus_log_read_range(apus_replica_t *r, uint64_t from, uint64_t to, void *dst, uint64_t cap, uint64_t *got);
+/* Follower, APUS_F_DEVICE_APPLY: deliver committed entries straight into device memory, in stream order.  The arrays
+ * are device memory on the follower's GPU, element types as apus_submit_device's plus idx; row k's cmd goes to
+ * payloads + k*stride (payloads may be NULL when stride is 0).  `stream` is a cudaStream_t (NULL = the legacy default
+ * stream).  Returns once the work is enqueued, without synchronising the host:
+ *   - the work runs after everything enqueued on `stream` before the call, and `stream` waits for it; every call on
+ *     one replica runs on one engine-owned stream, so calls run in call order whatever streams they come from;
+ *   - it examines the next committed entries from the consumer cursor on, at most max_n of them, and writes the
+ *     CSM-like ones (CSM, CONNECT, SEND, CLOSE: what do_action replays) as consecutive rows: idx, type, clt_id,
+ *     req_id, cmd length and the cmd bytes (bytes of a row beyond its length are left untouched).  NOOP, CONFIG and
+ *     HEAD entries are skipped; the idx of the rows shows them.  *count receives the number of rows;
+ *   - the examination stops before the first CSM-like entry whose cmd exceeds `stride` (apus_consume_status tells the
+ *     stride it needs: nothing is truncated or lost) and before an entry that does not carry the idx its index word
+ *     promises (APUS_CONSUME_BAD_IDX, sticky: nothing more is delivered);
+ *   - the cursor moves past every examined entry only after every read of their bytes has completed: the leader may
+ *     prune, then overwrite, everything behind it (the follower's kernel reports it on its idle passes).
+ * It never waits for commits: it delivers what is committed when it runs, which may be nothing.  APUS_ERROR on a
+ * leader, on a replica without APUS_F_DEVICE_APPLY, for a null array, for an array not aligned to its element size
+ * (idx and req_ids 8 B, count 4 B, connection_ids and lens 2 B; payloads may have any alignment), or for max_n == 0. */
+int  apus_consume_device(apus_replica_t *follower, uint32_t max_n, uint64_t *idx, uint8_t *types,
+                         uint16_t *connection_ids, uint64_t *req_ids, uint16_t *lens, void *payloads, size_t stride,
+                         uint32_t *count, void *stream);
+#define APUS_CONSUME_BAD_IDX 1   /* an entry at an index word does not carry the expected idx */
+/* the pinned words the consume work writes: the cursor and the idx of the next entry after the latest call that ran,
+ * the stride the entry that stopped it needs (0 = it did not stop on a long entry), APUS_CONSUME_* (0 = none) */
+int  apus_consume_status(apus_replica_t *follower, uint64_t *cursor_offset, uint64_t *next_idx, uint64_t *need_stride,
+                         uint64_t *error);
 /* failure detector: 0 while the leader's heartbeats arrive, else 1 + the term whose leader fell silent */
 uint64_t apus_leader_suspect(apus_replica_t *follower);
 /* %globaltimer (ns) of the leader kernel's latest commit (device clock; step timing of resident kernels) */
