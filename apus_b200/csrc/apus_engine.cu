@@ -168,7 +168,7 @@ struct apus_replica {
     int      peer_is_ipc[APUS_MAX_SERVERS];
     uint32_t *d_lat;
     /* device batches (apus_submit_device) and stream-ordered commit waits (apus_stream_wait_committed) */
-    uint64_t *pack_blk;           /* per packing block: {external bytes -> their exclusive scan, rejected, first rejected} */
+    uint64_t *pack_blk;           /* per packing block: PACK_BLK_WORDS (apus_pack_sizes_kernel) */
     cudaEvent_t ev_dsub_in, ev_dsub_out;   /* caller's stream -> copy_stream -> caller's stream */
     cudaEvent_t *waits;           /* recorded right after each enqueued commit wait, not yet seen complete */
     int      n_waits, cap_waits;
@@ -177,7 +177,7 @@ struct apus_replica {
      * copy_stream never queue behind them */
     cudaStream_t cons_stream;
     cudaEvent_t ev_cons_in, ev_cons_out;   /* caller's stream -> cons_stream -> caller's stream */
-    apus_cons_state_t *cons_st;   /* consume state + 2 words per consume block (index-ring capacity / block size) */
+    apus_cons_state_t *cons_st;   /* consume state + APUS_CONS_BLK_WORDS per consume block (index-ring capacity / block size) */
     pthread_mutex_t cons_mu;      /* one enqueue at a time: the two events are shared by every caller */
 };
 
@@ -218,7 +218,10 @@ static int ensure_host_ring(apus_replica *r)
     return APUS_OK;
 }
 
-#define PACK_THREADS 256u     /* requests per block of the packing kernels (apus_submit_device) */
+#define PACK_THREADS 256u     /* requests per block of the packing kernels (apus_submit_device, apus_submit_device_packed) */
+/* words per packing block: external bytes (-> their exclusive scan), rejected, first rejected, and the packed layout's
+ * verdict: the block saw offsets that decrease or end past values_bytes (-> the whole batch's verdict) */
+#define PACK_BLK_WORDS 4u
 static inline uint32_t pack_blocks(uint64_t n) { return (uint32_t)((n + PACK_THREADS - 1) / PACK_THREADS); }
 
 /* The kernels that fill the HBM ring run while the replica kernels are resident.  Under lazy module loading
@@ -246,7 +249,7 @@ static int leader_ring_init(apus_replica *r)
         CK(cudaMalloc(&r->sub_tail_dev, 128));
         CK(cudaMemset(r->sub_tail_dev, 0, 128));
         CK(cudaHostAlloc(&r->sub_tail_stage, 64, cudaHostAllocPortable));
-        CK(cudaMalloc(&r->pack_blk, 3 * sizeof(uint64_t) * pack_blocks(r->ring_slots)));
+        CK(cudaMalloc(&r->pack_blk, PACK_BLK_WORDS * sizeof(uint64_t) * pack_blocks(r->ring_slots)));
         if (load_fill_kernels() != APUS_OK) return APUS_ERROR;
     }
     return APUS_OK;
@@ -280,7 +283,7 @@ static int replica_init(apus_replica *r, const apus_config_t *cfg, uint64_t log_
         CK(cudaStreamCreateWithFlags(&r->cons_stream, cudaStreamNonBlocking));
         CK(cudaEventCreateWithFlags(&r->ev_cons_in, cudaEventDisableTiming));
         CK(cudaEventCreateWithFlags(&r->ev_cons_out, cudaEventDisableTiming));
-        const size_t sb = sizeof(apus_cons_state_t) + 16ull * ((cap + APUS_CONS_THREADS - 1) / APUS_CONS_THREADS);
+        const size_t sb = sizeof(apus_cons_state_t) + 8ull * APUS_CONS_BLK_WORDS * ((cap + APUS_CONS_THREADS - 1) / APUS_CONS_THREADS);
         CK(cudaMalloc(&r->cons_st, sb));
         CK(cudaMemset(r->cons_st, 0, sb));
         CK(apus_consume_load());
@@ -981,27 +984,43 @@ extern "C" int apus_submit_synth(apus_replica_t *r, uint32_t n, uint8_t type, ui
 struct PackArgs {
     apus_slot_t *ring;
     uint8_t *pay;
-    uint64_t *blk;                /* 3 words per block: external bytes (-> exclusive scan), rejected, first rejected */
+    uint64_t *blk;                /* PACK_BLK_WORDS per block, see below */
     const uint8_t *types;
     const uint16_t *conns;
     const uint64_t *req_ids;
-    const uint16_t *lens;
+    const uint16_t *lens;         /* strided layout (apus_submit_device): cmd k is payloads[k * stride, + lens[k]) */
+    const uint64_t *offsets;      /* packed layout (apus_submit_device_packed, lens NULL): cmd k is
+                                     payloads[offsets[k], offsets[k + 1]), inside [0, values_bytes) */
     const uint8_t *payloads;
-    uint64_t stride;
+    uint64_t stride, values_bytes;
     uint64_t first_slot;          /* submitted count before the batch: request k gets ticket first_slot + k + 1 */
     uint64_t res_pos;             /* ring position of the batch's payload reservation */
     uint32_t n, mask;
 };
 
-/* what request k becomes: its own type and length, or the NOOP that apus_submit(APUS_NOOP, conn, req_id, NULL, 0)
- * writes when the type is not a request type or len > stride */
-__device__ __forceinline__ bool pack_request(const PackArgs &a, uint32_t k, uint32_t *type, uint32_t *len)
+/* what request k becomes -- its own type and length, or the NOOP that apus_submit(APUS_NOOP, conn, req_id, NULL, 0)
+ * writes when the type is not a request type, the length is above the limit (stride, or 65535 packed) or the packed
+ * batch is `bad` -- and where its cmd starts in payloads, in either layout */
+__device__ __forceinline__ bool pack_request(const PackArgs &a, uint32_t k, bool bad, uint32_t *type, uint32_t *len,
+                                             uint64_t *src)
 {
-    const uint32_t ty = a.types[k], ln = a.lens[k];
-    const bool ok = (ty == APUS_CSM || ty == APUS_CONNECT || ty == APUS_SEND || ty == APUS_CLOSE) && ln <= a.stride;
+    const uint32_t ty = a.types[k];
+    uint64_t ln, at;
+    if (a.offsets) { at = a.offsets[k]; ln = a.offsets[k + 1] - at; }
+    else { at = (uint64_t)k * a.stride; ln = a.lens[k]; }
+    const bool ok = (ty == APUS_CSM || ty == APUS_CONNECT || ty == APUS_SEND || ty == APUS_CLOSE) && !bad &&
+                    ln <= (a.offsets ? 0xffffull : a.stride);
     *type = ok ? ty : (uint32_t)APUS_NOOP;
-    *len = ok ? ln : 0u;
+    *len = ok ? (uint32_t)ln : 0u;
+    *src = at;
     return ok;
+}
+
+/* the packed layout's per-request share of the batch verdict: offsets[k] <= offsets[k + 1] <= values_bytes for every
+ * k is exactly "nondecreasing, and inside values"; valid lengths of such a batch stay inside its reservation */
+__device__ __forceinline__ bool pack_offsets_bad(const PackArgs &a, uint32_t k)
+{
+    return a.offsets && (a.offsets[k + 1] < a.offsets[k] || a.offsets[k + 1] > a.values_bytes);
 }
 
 /* inclusive sum over the block (PACK_THREADS threads) of v; *total = the block's sum */
@@ -1033,41 +1052,54 @@ __global__ void __launch_bounds__(PACK_THREADS) apus_pack_sizes_kernel(PackArgs 
     if (threadIdx.x == 0) first_rej = ~0ull;
     __syncthreads();
     uint32_t ty = 0, len = 0;
-    bool rej = false;
-    uint64_t xb = 0;
+    bool rej = false, bad = false;
+    uint64_t xb = 0, src;
     if (k < a.n) {
-        rej = !pack_request(a, k, &ty, &len);
+        rej = !pack_request(a, k, false, &ty, &len, &src);
+        bad = pack_offsets_bad(a, k);
         xb = slot_ext_bytes(slot_image_bytes(ty, len));
         if (rej) atomicMin(&first_rej, (unsigned long long)k);
     }
     const uint32_t nrej = __syncthreads_count(rej);
+    const uint32_t nbad = __syncthreads_count(bad);
     uint64_t total;
     block_incl_scan(xb, &total);
     if (threadIdx.x == 0) {
-        a.blk[3 * blockIdx.x] = total;
-        a.blk[3 * blockIdx.x + 1] = nrej;
-        a.blk[3 * blockIdx.x + 2] = first_rej;
+        a.blk[PACK_BLK_WORDS * blockIdx.x] = total;
+        a.blk[PACK_BLK_WORDS * blockIdx.x + 1] = nrej;
+        a.blk[PACK_BLK_WORDS * blockIdx.x + 2] = first_rej;
+        a.blk[PACK_BLK_WORDS * blockIdx.x + 3] = nbad != 0;
     }
 }
 
-/* pass 2 (one block): exclusive scan of the blocks' external bytes, in place; the batch's rejections into the host words */
+/* pass 2 (one block): the batch verdict of the packed layout (a bad batch is all NOOPs: no external bytes, every
+ * request rejected), handed to every block; exclusive scan of the blocks' external bytes, in place; the batch's
+ * rejections into the host words.  The verdict is final before pass 3 writes any slot. */
 __global__ void __launch_bounds__(PACK_THREADS) apus_pack_scan_kernel(PackArgs a, uint32_t nblk, apus_hostwords_t *hw)
 {
     __shared__ unsigned long long first_rej;
     __shared__ unsigned int nrej;
-    if (threadIdx.x == 0) { first_rej = ~0ull; nrej = 0; }
+    uint64_t *blk = a.blk;
+    bool mine = false;
+    if (a.offsets)
+        for (uint32_t b = threadIdx.x; b < nblk; b += PACK_THREADS) mine |= blk[PACK_BLK_WORDS * b + 3] != 0;
+    const bool bad = __syncthreads_or(mine) != 0;
+    if (threadIdx.x == 0) { first_rej = bad ? 0ull : ~0ull; nrej = bad ? a.n : 0u; }
     __syncthreads();
     uint64_t carry = 0;
     for (uint32_t b0 = 0; b0 < nblk; b0 += PACK_THREADS) {
         const uint32_t b = b0 + threadIdx.x;
-        const uint64_t v = b < nblk ? a.blk[3 * b] : 0;
-        if (b < nblk && a.blk[3 * b + 1]) {
-            atomicAdd(&nrej, (unsigned int)a.blk[3 * b + 1]);
-            atomicMin(&first_rej, (unsigned long long)a.blk[3 * b + 2]);
+        const uint64_t v = b < nblk && !bad ? blk[PACK_BLK_WORDS * b] : 0;
+        if (b < nblk && !bad && blk[PACK_BLK_WORDS * b + 1]) {
+            atomicAdd(&nrej, (unsigned int)blk[PACK_BLK_WORDS * b + 1]);
+            atomicMin(&first_rej, (unsigned long long)blk[PACK_BLK_WORDS * b + 2]);
         }
         uint64_t total;
         const uint64_t incl = block_incl_scan(v, &total);
-        if (b < nblk) a.blk[3 * b] = carry + incl - v;
+        if (b < nblk) {
+            blk[PACK_BLK_WORDS * b] = carry + incl - v;
+            blk[PACK_BLK_WORDS * b + 3] = bad;
+        }
         carry += total;
     }
     __syncthreads();
@@ -1098,24 +1130,26 @@ __device__ __forceinline__ uint4 image_chunk(const uint8_t *src, uint32_t len, u
 __global__ void __launch_bounds__(PACK_THREADS) apus_pack_kernel(PackArgs a)
 {
     __shared__ uint32_t s_type_off[PACK_THREADS], s_len[PACK_THREADS], s_nb[PACK_THREADS];
-    __shared__ uint64_t s_pos[PACK_THREADS];
+    __shared__ uint64_t s_pos[PACK_THREADS], s_src[PACK_THREADS];
     const uint32_t kb = blockIdx.x * PACK_THREADS;
     {
         const uint32_t k = kb + threadIdx.x;
         uint32_t ty = 0, len = 0, nb = 0;
+        uint64_t src = 0;
         if (k < a.n) {
-            pack_request(a, k, &ty, &len);
+            pack_request(a, k, a.blk[PACK_BLK_WORDS * blockIdx.x + 3] != 0, &ty, &len, &src);
             nb = slot_image_bytes(ty, len);
         }
         const uint64_t xb = slot_ext_bytes(nb);
         uint64_t total;
-        const uint64_t off = a.blk[3 * blockIdx.x] + block_incl_scan(xb, &total) - xb;
+        const uint64_t off = a.blk[PACK_BLK_WORDS * blockIdx.x] + block_incl_scan(xb, &total) - xb;
         const uint64_t pos = a.res_pos + off;
         /* the first external image of the batch starts the reservation: a discontinuity for the leader */
         s_type_off[threadIdx.x] = slot_type_off(ty, xb ? (APUS_SLOT_EXT | (off == 0 ? APUS_SLOT_WRAP : 0u)) : 0u, pos);
         s_len[threadIdx.x] = len;
         s_nb[threadIdx.x] = nb;
         s_pos[threadIdx.x] = pos;
+        s_src[threadIdx.x] = src;
     }
     __syncthreads();
     const uint32_t c = threadIdx.x & 7u;
@@ -1125,7 +1159,7 @@ __global__ void __launch_bounds__(PACK_THREADS) apus_pack_kernel(PackArgs a)
         const uint64_t ticket = a.first_slot + k + 1;
         uint4 *d = reinterpret_cast<uint4 *>(&a.ring[(a.first_slot + k) & a.mask]);
         const uint32_t to = s_type_off[i], len = s_len[i], nb = s_nb[i];
-        const uint8_t *src = a.payloads + (uint64_t)k * a.stride;
+        const uint8_t *src = a.payloads + s_src[i];
         if (live && c == 0) {
             uint32_t w[4];
             slot_desc_words(w, a.req_ids[k], to, len, a.conns[k]);
@@ -1161,22 +1195,16 @@ static int load_fill_kernels(void)
     return APUS_OK;
 }
 
-extern "C" int apus_submit_device(apus_replica_t *r, uint32_t n, const uint8_t *types, const uint16_t *connection_ids,
-                                  const uint64_t *req_ids, const uint16_t *lens, const void *payloads, size_t stride,
-                                  void *stream, uint64_t *first_ticket)
+/* the part of a device batch both layouts share: room in both rings, the placement of the `res`-byte reservation, the
+ * three passes and the doorbell on copy_stream in the caller's stream order, and the space accounting */
+static int submit_packing(apus_replica_t *r, const char *what, PackArgs a, uint64_t res, void *stream,
+                          uint64_t *first_ticket)
 {
-    if (!r) return fail("null argument");
-    if (!is_leader(r)) return fail("submit on a follower");
-    if (r->cfg.ring_mode != APUS_RING_DEVICE) return fail("apus_submit_device needs the device submission ring");
-    if (n == 0) return APUS_OK;
-    if (!types || !connection_ids || !req_ids || !lens || (!payloads && stride)) return fail("null argument");
-    if (n > r->ring_slots) return fail("apus_submit_device: %u requests can never fit a ring of %u slots", n, r->ring_slots);
-    /* lens are unknown here: reserve the worst case, round16(2 + stride) per request (nothing when that is inline) */
-    const uint64_t per = slot_ext_bytes(2u + (uint32_t)(stride < 0xffffu ? stride : 0xffffu));
-    const uint64_t res = (uint64_t)n * per;
+    const uint32_t n = a.n;
+    if (n > r->ring_slots) return fail("%s: %u requests can never fit a ring of %u slots", what, n, r->ring_slots);
     if (res > r->ring_bytes)
-        return fail("apus_submit_device: a reservation of %llu B can never fit a payload ring of %u B",
-                    (unsigned long long)res, r->ring_bytes);
+        return fail("%s: a reservation of %llu B can never fit a payload ring of %u B", what, (unsigned long long)res,
+                    r->ring_bytes);
     const uint64_t consumed = r->hw->consumed;
     if (r->submitted + n - consumed > r->ring_slots) { snprintf(g_err, sizeof g_err, "submission ring full"); return APUS_RETRY; }
     const uint32_t mask = r->ring_slots - 1;
@@ -1192,10 +1220,8 @@ extern "C" int apus_submit_device(apus_replica_t *r, uint32_t n, const uint8_t *
     if (!r->ev_dsub_in) CK(cudaEventCreateWithFlags(&r->ev_dsub_in, cudaEventDisableTiming));
     if (!r->ev_dsub_out) CK(cudaEventCreateWithFlags(&r->ev_dsub_out, cudaEventDisableTiming));
     cudaStream_t s = (cudaStream_t)stream;
-    PackArgs a;
     a.ring = r->ring_desc_dev; a.pay = r->ring_pay_dev; a.blk = r->pack_blk;
-    a.types = types; a.conns = connection_ids; a.req_ids = req_ids; a.lens = lens; a.payloads = (const uint8_t *)payloads;
-    a.stride = stride; a.first_slot = r->submitted; a.res_pos = pos; a.n = n; a.mask = mask;
+    a.first_slot = r->submitted; a.res_pos = pos; a.mask = mask;
     const uint32_t nblk = pack_blocks(n);
     /* the packing sees everything the caller's stream did before this call; the caller's stream sees the packing */
     CK(cudaEventRecord(r->ev_dsub_in, s));
@@ -1221,6 +1247,43 @@ extern "C" int apus_submit_device(apus_replica_t *r, uint32_t n, const uint8_t *
     r->flushed = upto;
     if (!r->defer) r->belled = upto;
     return APUS_OK;
+}
+
+extern "C" int apus_submit_device(apus_replica_t *r, uint32_t n, const uint8_t *types, const uint16_t *connection_ids,
+                                  const uint64_t *req_ids, const uint16_t *lens, const void *payloads, size_t stride,
+                                  void *stream, uint64_t *first_ticket)
+{
+    if (!r) return fail("null argument");
+    if (!is_leader(r)) return fail("submit on a follower");
+    if (r->cfg.ring_mode != APUS_RING_DEVICE) return fail("apus_submit_device needs the device submission ring");
+    if (n == 0) return APUS_OK;
+    if (!types || !connection_ids || !req_ids || !lens || (!payloads && stride)) return fail("null argument");
+    /* lens are unknown here: reserve the worst case, round16(2 + stride) per request (nothing when that is inline) */
+    const uint64_t per = slot_ext_bytes(2u + (uint32_t)(stride < 0xffffu ? stride : 0xffffu));
+    PackArgs a;
+    memset(&a, 0, sizeof a);
+    a.types = types; a.conns = connection_ids; a.req_ids = req_ids; a.lens = lens; a.payloads = (const uint8_t *)payloads;
+    a.stride = stride; a.n = n;
+    return submit_packing(r, "apus_submit_device", a, (uint64_t)n * per, stream, first_ticket);
+}
+
+extern "C" int apus_submit_device_packed(apus_replica_t *r, uint32_t n, const uint8_t *types,
+                                         const uint16_t *connection_ids, const uint64_t *req_ids, const uint64_t *offsets,
+                                         const void *values, uint64_t values_bytes, void *stream, uint64_t *first_ticket)
+{
+    if (!r) return fail("null argument");
+    if (!is_leader(r)) return fail("submit on a follower");
+    if (r->cfg.ring_mode != APUS_RING_DEVICE) return fail("apus_submit_device_packed needs the device submission ring");
+    if (n == 0) return APUS_OK;
+    if (!types || !connection_ids || !req_ids || !offsets || (!values && values_bytes)) return fail("null argument");
+    /* the kernels load whole elements: a misaligned array would fault on the device, so refuse it here */
+    if (((uintptr_t)offsets | (uintptr_t)req_ids) & 7u || (uintptr_t)connection_ids & 1u)
+        return fail("apus_submit_device_packed: misaligned array (offsets and req_ids need 8 B, connection_ids 2 B)");
+    PackArgs a;
+    memset(&a, 0, sizeof a);
+    a.types = types; a.conns = connection_ids; a.req_ids = req_ids; a.offsets = offsets;
+    a.payloads = (const uint8_t *)values; a.values_bytes = values_bytes; a.n = n;
+    return submit_packing(r, "apus_submit_device_packed", a, slot_packed_reserve(n, values_bytes), stream, first_ticket);
 }
 
 extern "C" int apus_device_submit_status(apus_replica_t *r, uint64_t *rejected, uint64_t *first_rejected_ticket)
@@ -1418,6 +1481,26 @@ extern "C" int apus_set_applied(apus_replica_t *r, uint64_t offset)
 }
 
 /* ---- device consumers: committed entries straight into device memory, in stream order ----------------------- */
+/* what both layouts share, once the arguments are checked: max_n clipped to the index ring, and the five kernels on the
+ * consume stream in the caller's stream order */
+static int consume_enqueue(apus_replica_t *r, apus_consume_args_t a, uint32_t max_n, void *stream)
+{
+    /* at most idx_cap entries lie between the cursor and what the follower holds (each is >= 64 B of one lap) */
+    const uint32_t n = max_n < r->idx_cap ? max_n : r->idx_cap;
+    a.region = r->region; a.entries_off = r->entries_off; a.log_len = r->log_len;
+    a.idx_mask = r->idx_cap - 1; a.max_n = n; a.nblk = (n + APUS_CONS_THREADS - 1) / APUS_CONS_THREADS;
+    a.st = r->cons_st; a.hw = r->hw_dev;
+    DeviceGuard g(r->cfg.device);
+    StageLock sl(&r->cons_mu);
+    cudaStream_t s = (cudaStream_t)stream;
+    CK(cudaEventRecord(r->ev_cons_in, s));
+    CK(cudaStreamWaitEvent(r->cons_stream, r->ev_cons_in, 0));
+    CK(apus_consume_enqueue(&a, r->cons_stream));
+    CK(cudaEventRecord(r->ev_cons_out, r->cons_stream));
+    CK(cudaStreamWaitEvent(s, r->ev_cons_out, 0));
+    return APUS_OK;
+}
+
 extern "C" int apus_consume_device(apus_replica_t *r, uint32_t max_n, uint64_t *idx, uint8_t *types,
                                    uint16_t *connection_ids, uint64_t *req_ids, uint16_t *lens, void *payloads,
                                    size_t stride, uint32_t *count, void *stream)
@@ -1430,24 +1513,34 @@ extern "C" int apus_consume_device(apus_replica_t *r, uint32_t max_n, uint64_t *
     /* the kernels store whole elements: a misaligned array would fault on the device, so refuse it here */
     if (((uintptr_t)idx | (uintptr_t)req_ids) & 7u || ((uintptr_t)connection_ids | (uintptr_t)lens) & 1u || (uintptr_t)count & 3u)
         return fail("apus_consume_device: misaligned array (idx and req_ids need 8 B, count 4 B, connection_ids and lens 2 B)");
-    /* at most idx_cap entries lie between the cursor and what the follower holds (each is >= 64 B of one lap) */
-    const uint32_t n = max_n < r->idx_cap ? max_n : r->idx_cap;
     apus_consume_args_t a;
     memset(&a, 0, sizeof a);
-    a.region = r->region; a.entries_off = r->entries_off; a.log_len = r->log_len; a.stride = stride;
-    a.idx_mask = r->idx_cap - 1; a.max_n = n; a.nblk = (n + APUS_CONS_THREADS - 1) / APUS_CONS_THREADS;
-    a.st = r->cons_st; a.hw = r->hw_dev;
+    a.stride = stride;
     a.idx = idx; a.types = types; a.conns = connection_ids; a.req_ids = req_ids; a.lens = lens;
     a.payloads = (uint8_t *)payloads; a.count = count;
-    DeviceGuard g(r->cfg.device);
-    StageLock sl(&r->cons_mu);
-    cudaStream_t s = (cudaStream_t)stream;
-    CK(cudaEventRecord(r->ev_cons_in, s));
-    CK(cudaStreamWaitEvent(r->cons_stream, r->ev_cons_in, 0));
-    CK(apus_consume_enqueue(&a, r->cons_stream));
-    CK(cudaEventRecord(r->ev_cons_out, r->cons_stream));
-    CK(cudaStreamWaitEvent(s, r->ev_cons_out, 0));
-    return APUS_OK;
+    return consume_enqueue(r, a, max_n, stream);
+}
+
+extern "C" int apus_consume_device_packed(apus_replica_t *r, uint32_t max_n, uint64_t *idx, uint8_t *types,
+                                          uint16_t *connection_ids, uint64_t *req_ids, uint64_t *offsets, void *values,
+                                          uint64_t values_cap, uint32_t *count, void *stream)
+{
+    if (!r) return fail("null argument");
+    if (is_leader(r)) return fail("apus_consume_device_packed: consumption is a follower's (the leader's log is its own)");
+    if (!(r->cfg.flags & APUS_F_DEVICE_APPLY))
+        return fail("apus_consume_device_packed needs a replica created with APUS_F_DEVICE_APPLY");
+    if (max_n == 0) return fail("apus_consume_device_packed: max_n is 0");
+    if (!idx || !types || !connection_ids || !req_ids || !offsets || !count || (!values && values_cap))
+        return fail("null argument");
+    if (((uintptr_t)idx | (uintptr_t)req_ids | (uintptr_t)offsets) & 7u || (uintptr_t)connection_ids & 1u ||
+        (uintptr_t)count & 3u)
+        return fail("apus_consume_device_packed: misaligned array (idx, req_ids and offsets need 8 B, count 4 B, "
+                    "connection_ids 2 B)");
+    apus_consume_args_t a;
+    memset(&a, 0, sizeof a);
+    a.idx = idx; a.types = types; a.conns = connection_ids; a.req_ids = req_ids; a.offsets = offsets;
+    a.payloads = (uint8_t *)values; a.values_cap = values_cap; a.count = count;
+    return consume_enqueue(r, a, max_n, stream);
 }
 
 extern "C" int apus_consume_status(apus_replica_t *r, uint64_t *cursor_offset, uint64_t *next_idx, uint64_t *need_stride,

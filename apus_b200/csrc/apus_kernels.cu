@@ -2228,16 +2228,19 @@ __device__ void follower_main(const apus_devctx_t *__restrict__ cx)
 }
 
 // ---------------------------------------------------------------------------------
-// DEVICE CONSUMERS (APUS_F_DEVICE_APPLY): the work of one apus_consume_device call, five kernels in stream order on
-// the replica's consume stream -- head (snapshot the record and the cursor), count (per block: rows and the first
-// entry that stops the examination), scan (where the examination stops, row offsets, the new cursor), copy (the rows),
-// tail (the row count, then the cursor and the status words).  Entries are found through the offset index, never
-// by walking bytes; they never wrap (the ghost-header rule places them at 0), so each cmd is one contiguous run.
+// DEVICE CONSUMERS (APUS_F_DEVICE_APPLY): the work of one apus_consume_device or apus_consume_device_packed call, five
+// kernels in stream order on the replica's consume stream -- head (snapshot the record and the cursor), count (per
+// block: rows, their cmd bytes and the first entry that stops the examination), scan (where the examination stops, row
+// and byte offsets, the new cursor), copy (the rows), tail (the row count and the packed byte total, then the cursor
+// and the status words).  A strided call stops before a cmd longer than its stride; a packed call stops before the
+// first cmd that would end past values_cap, which depends on the running byte sum of the rows before it.  Entries are
+// found through the offset index, never by walking bytes; they never wrap (the ghost-header rule places them at 0), so
+// each cmd is one contiguous run.
 // ---------------------------------------------------------------------------------
 #define CONS_OK        0u
 #define CONS_LATER     1u    // not committed (yet): the examination ends here, quietly
 #define CONS_BAD_IDX   2u    // the entry at the index word does not carry the expected idx
-#define CONS_TOO_LONG  3u    // CSM-like with a cmd longer than the row stride
+#define CONS_TOO_LONG  3u    // CSM-like with a cmd longer than the row stride (strided calls)
 #define CONS_NONE      0xffffffffu
 
 __device__ __forceinline__ uint32_t ld_relaxed_sys_u8_any(const uint8_t *entries, uint64_t at)
@@ -2254,7 +2257,8 @@ struct ConsEntry {
     uint32_t ty, len, status;
 };
 // entry j of this call: its offset from the index word, then whether it is committed (within [cursor, committed) of
-// the one lap the cursor bounds), carries idx next_idx + j, and fits a row
+// the one lap the cursor bounds), carries idx next_idx + j, and fits a row (strided calls; a packed call's capacity
+// stop is the scan kernel's)
 __device__ __forceinline__ ConsEntry cons_classify(const apus_consume_args_t &a, const apus_cons_state_t &s, uint64_t j)
 {
     const uint8_t *entries = a.region + a.entries_off;
@@ -2271,7 +2275,7 @@ __device__ __forceinline__ ConsEntry cons_classify(const apus_consume_args_t &a,
     if (has_cmd(e.ty)) {
         e.len = ld_relaxed_sys_u16_any(entries, e.off + E_DATA);
         if (e.off + entry_stride(e.ty, e.len) > L) e.status = CONS_BAD_IDX;   // not an entry this log could hold
-        else if (e.len > a.stride) e.status = CONS_TOO_LONG;
+        else if (!a.offsets && e.len > a.stride) e.status = CONS_TOO_LONG;
     }
     return e;
 }
@@ -2294,6 +2298,23 @@ __device__ __forceinline__ uint32_t cons_block_excl(bool flag, uint32_t *total)
     return before + __popc(b & ((1u << lane) - 1u));
 }
 
+// inclusive sum of v over the block (APUS_CONS_THREADS threads); *total = the block's sum
+__device__ __forceinline__ uint64_t cons_block_incl(uint64_t v, uint64_t *total)
+{
+    __shared__ uint64_t part[APUS_CONS_THREADS / 32];
+    for (uint32_t d = 1; d < 32; d <<= 1) {
+        const uint64_t o = __shfl_up_sync(0xffffffffu, v, d);
+        if ((threadIdx.x & 31u) >= d) v += o;
+    }
+    if ((threadIdx.x & 31u) == 31u) part[threadIdx.x >> 5] = v;
+    __syncthreads();
+    uint64_t before = 0, all = 0;
+    for (uint32_t i = 0; i < APUS_CONS_THREADS / 32; i++) { if (i < (threadIdx.x >> 5)) before += part[i]; all += part[i]; }
+    __syncthreads();
+    *total = all;
+    return before + v;
+}
+
 // 1: snapshot the record (acquire: the entry bytes and index words it covers are visible from here on) and the cursor
 __global__ void apus_consume_head_kernel(apus_consume_args_t a)
 {
@@ -2307,7 +2328,8 @@ __global__ void apus_consume_head_kernel(apus_consume_args_t a)
     s->m = s->error ? 0 : (avail < a.max_n ? avail : a.max_n);
 }
 
-// 2: per block, the CSM-like entries before the block's first stop, and that stop {j, reason, len}
+// 2: per block, the CSM-like entries before the block's first stop, that stop {j, reason, len}, and (packed) the cmd
+// bytes of those entries
 __global__ void __launch_bounds__(APUS_CONS_THREADS) apus_consume_count_kernel(apus_consume_args_t a)
 {
     __shared__ uint32_t first;
@@ -2319,52 +2341,98 @@ __global__ void __launch_bounds__(APUS_CONS_THREADS) apus_consume_count_kernel(a
     if (j < s.m) e = cons_classify(a, s, j);
     if (j < s.m && e.status != CONS_OK) atomicMin(&first, (uint32_t)j);
     __syncthreads();
-    const uint32_t rows = __syncthreads_count(j < s.m && e.status == CONS_OK && has_cmd(e.ty) && j < first);
-    uint64_t *blk = reinterpret_cast<uint64_t *>(a.st + 1);
-    if (threadIdx.x == 0) blk[2 * blockIdx.x] = rows;
+    const bool row = j < s.m && e.status == CONS_OK && has_cmd(e.ty) && j < first;
+    const uint32_t rows = __syncthreads_count(row);
+    uint64_t *blk = reinterpret_cast<uint64_t *>(a.st + 1) + APUS_CONS_BLK_WORDS * blockIdx.x;
+    if (threadIdx.x == 0) blk[0] = rows;
     if (first == CONS_NONE) {
-        if (threadIdx.x == 0) blk[2 * blockIdx.x + 1] = CONS_NONE;
+        if (threadIdx.x == 0) blk[1] = CONS_NONE;
     } else if (j == first) {
-        blk[2 * blockIdx.x + 1] = (uint64_t)first | ((uint64_t)e.status << 32) | ((uint64_t)e.len << 40);
+        blk[1] = (uint64_t)first | ((uint64_t)e.status << 32) | ((uint64_t)e.len << 40);
+    }
+    if (a.offsets) {
+        uint64_t bytes;
+        cons_block_incl(row ? e.len : 0u, &bytes);
+        if (threadIdx.x == 0) blk[2] = bytes;
     }
 }
 
 // 3 (one block): the first block with a stop ends the examination; exclusive scan of the rows of the blocks up to it,
-// in place; the examined count, the row count and the new cursor (end of the last examined entry, E1: L is 0)
+// in place; the examined count, the row count and the new cursor (end of the last examined entry, E1: L is 0).
+// Packed: exclusive scan of the blocks' cmd bytes, in place; a block whose rows end past values_cap ends the
+// examination too, if it comes first, and inside it the entries are classified again to find the first cmd that ends
+// past values_cap -- the examination stops just before it.
 __global__ void __launch_bounds__(APUS_CONS_THREADS) apus_consume_scan_kernel(apus_consume_args_t a)
 {
-    __shared__ uint32_t bstop;
+    __shared__ uint32_t bstop, bcap, tcap;
+    __shared__ uint64_t s_bytes, s_need;
     apus_cons_state_t *s = a.st;
     uint64_t *blk = reinterpret_cast<uint64_t *>(s + 1);
     const uint32_t nblk = (uint32_t)((s->m + APUS_CONS_THREADS - 1) / APUS_CONS_THREADS);
-    if (threadIdx.x == 0) bstop = CONS_NONE;
+    if (threadIdx.x == 0) { bstop = CONS_NONE; bcap = CONS_NONE; tcap = CONS_NONE; s_bytes = 0; s_need = 0; }
     __syncthreads();
     for (uint32_t b = threadIdx.x; b < nblk; b += APUS_CONS_THREADS)
-        if (blk[2 * b + 1] != CONS_NONE) atomicMin(&bstop, b);
+        if (blk[APUS_CONS_BLK_WORDS * b + 1] != CONS_NONE) atomicMin(&bstop, b);
     __syncthreads();
-    const uint32_t last = bstop == CONS_NONE ? nblk : bstop + 1;     // blocks whose rows count
+    uint32_t last = bstop == CONS_NONE ? nblk : bstop + 1;           // blocks whose rows count
+    if (a.offsets) {
+        uint64_t carry = 0;
+        for (uint32_t b0 = 0; b0 < last; b0 += APUS_CONS_THREADS) {
+            const uint32_t b = b0 + threadIdx.x;
+            const uint64_t v = b < last ? blk[APUS_CONS_BLK_WORDS * b + 2] : 0;
+            uint64_t total;
+            const uint64_t incl = cons_block_incl(v, &total);
+            if (b < last) {
+                blk[APUS_CONS_BLK_WORDS * b + 2] = carry + incl - v;
+                if (carry + incl > a.values_cap) atomicMin(&bcap, b);
+            }
+            carry += total;
+        }
+        __syncthreads();
+        if (bcap == CONS_NONE) {
+            if (threadIdx.x == 0) s_bytes = carry;
+        } else {
+            // every block before bcap ends inside values_cap, and bcap's own stop (if any) comes after its capacity
+            // stop: the bytes the count kernel summed end before that own stop
+            last = bcap + 1;
+            const uint64_t j = (uint64_t)bcap * APUS_CONS_THREADS + threadIdx.x;
+            const uint64_t own = blk[APUS_CONS_BLK_WORDS * bcap + 1], base = blk[APUS_CONS_BLK_WORDS * bcap + 2];
+            ConsEntry e = {0, 0, 0, CONS_LATER};
+            if (j < s->m && j < (uint32_t)own) e = cons_classify(a, *s, j);
+            const uint64_t v = e.status == CONS_OK && has_cmd(e.ty) ? e.len : 0u;
+            uint64_t total;
+            const uint64_t incl = cons_block_incl(v, &total);
+            if (base + incl > a.values_cap && v) atomicMin(&tcap, threadIdx.x);
+            __syncthreads();
+            if (threadIdx.x == tcap) { s_bytes = base + incl - v; s_need = v; }
+        }
+    }
     uint64_t carry = 0;
     for (uint32_t b0 = 0; b0 < last; b0 += APUS_CONS_THREADS) {
         const uint32_t b = b0 + threadIdx.x;
-        const uint64_t v = b < last ? blk[2 * b] : 0;
-        uint64_t incl = v;                                            // block-wide inclusive scan of v
-        __shared__ uint64_t part[APUS_CONS_THREADS / 32];
-        for (uint32_t d = 1; d < 32; d <<= 1) {
-            const uint64_t o = __shfl_up_sync(0xffffffffu, incl, d);
-            if ((threadIdx.x & 31u) >= d) incl += o;
-        }
-        if ((threadIdx.x & 31u) == 31u) part[threadIdx.x >> 5] = incl;
-        __syncthreads();
-        uint64_t before = 0, all = 0;
-        for (uint32_t i = 0; i < APUS_CONS_THREADS / 32; i++) { if (i < (threadIdx.x >> 5)) before += part[i]; all += part[i]; }
-        __syncthreads();
-        if (b < last) blk[2 * b] = carry + before + incl - v;
-        carry += all;
+        const uint64_t v = b < last ? blk[APUS_CONS_BLK_WORDS * b] : 0;
+        uint64_t total;
+        const uint64_t incl = cons_block_incl(v, &total);
+        if (b < last) blk[APUS_CONS_BLK_WORDS * b] = carry + incl - v;
+        carry += total;
     }
+    // rows of the capacity block before its stop (every thread: the count is block-wide)
+    uint32_t cap_rows = 0;
+    if (bcap != CONS_NONE) {
+        const uint64_t j = (uint64_t)bcap * APUS_CONS_THREADS + threadIdx.x;
+        ConsEntry e = {0, 0, 0, CONS_LATER};
+        if (threadIdx.x < tcap) e = cons_classify(a, *s, j);
+        cap_rows = __syncthreads_count(threadIdx.x < tcap && e.status == CONS_OK && has_cmd(e.ty));
+    }
+    __syncthreads();
     if (threadIdx.x == 0) {
-        uint64_t n_exam = s->m, need = 0;
-        if (bstop != CONS_NONE) {
-            const uint64_t w = blk[2 * bstop + 1];
+        uint64_t n_exam = s->m, need = 0, rows = carry;
+        if (bcap != CONS_NONE) {
+            n_exam = (uint64_t)bcap * APUS_CONS_THREADS + tcap;
+            rows = blk[APUS_CONS_BLK_WORDS * bcap] + cap_rows;
+            if (rows == 0) need = s_need;                         // the call's first row: report the bytes it needs
+        } else if (bstop != CONS_NONE) {
+            const uint64_t w = blk[APUS_CONS_BLK_WORDS * bstop + 1];
             const uint32_t why = (uint32_t)(w >> 32) & 0xffu;
             n_exam = (uint32_t)w;
             if (why == CONS_BAD_IDX) s->error = APUS_CONSUME_BAD_IDX;
@@ -2376,7 +2444,7 @@ __global__ void __launch_bounds__(APUS_CONS_THREADS) apus_consume_scan_kernel(ap
             cur = e.off + entry_stride(e.ty, e.len);
             if (cur == a.log_len) cur = 0;
         }
-        s->rows = carry; s->n_exam = n_exam; s->new_cursor = cur; s->need_stride = need;
+        s->rows = rows; s->n_exam = n_exam; s->new_cursor = cur; s->need_stride = need; s->bytes = s_bytes;
     }
 }
 
@@ -2414,13 +2482,14 @@ __device__ __forceinline__ void cons_copy_cmd(uint8_t *dst, const uint8_t *src, 
 }
 
 // 4: each block writes the rows of its entries (j < examined): one thread per entry for the fields, then eight
-// threads per entry for the cmd bytes
+// threads per entry for the cmd bytes -- at row * stride, or (packed) at the row's byte offset: the block's byte base
+// plus the cmd bytes of the rows before it in the block
 __global__ void __launch_bounds__(APUS_CONS_THREADS) apus_consume_copy_kernel(apus_consume_args_t a)
 {
-    __shared__ uint64_t s_off[APUS_CONS_THREADS], s_row[APUS_CONS_THREADS];
+    __shared__ uint64_t s_off[APUS_CONS_THREADS], s_dst[APUS_CONS_THREADS];
     __shared__ uint32_t s_len[APUS_CONS_THREADS];
     const apus_cons_state_t s = *a.st;
-    const uint64_t *blk = reinterpret_cast<const uint64_t *>(a.st + 1);
+    const uint64_t *blk = reinterpret_cast<const uint64_t *>(a.st + 1) + APUS_CONS_BLK_WORDS * blockIdx.x;
     const uint8_t *entries = a.region + a.entries_off;
     if ((uint64_t)blockIdx.x * APUS_CONS_THREADS >= s.n_exam) return;          // the whole block is past the stop
     const uint64_t j = (uint64_t)blockIdx.x * APUS_CONS_THREADS + threadIdx.x;
@@ -2428,29 +2497,37 @@ __global__ void __launch_bounds__(APUS_CONS_THREADS) apus_consume_copy_kernel(ap
     if (j < s.n_exam) e = cons_classify(a, s, j);
     const bool live = j < s.n_exam && has_cmd(e.ty);
     uint32_t tot;
-    const uint64_t row = blk[2 * blockIdx.x] + cons_block_excl(live, &tot);
+    const uint64_t row = blk[0] + cons_block_excl(live, &tot);
+    uint64_t dst = row * a.stride;
+    if (a.offsets) {
+        const uint64_t v = live ? e.len : 0u;
+        uint64_t total;
+        dst = blk[2] + cons_block_incl(v, &total) - v;
+    }
     if (live) {
         a.idx[row] = s.next_idx + j;
         a.types[row] = (uint8_t)e.ty;
         a.conns[row] = (uint16_t)ld_relaxed_sys_u16_any(entries, e.off + E_CLTID);
         a.req_ids[row] = ld_relaxed_sys_u64_any(entries, e.off + E_REQID);
-        a.lens[row] = (uint16_t)e.len;
+        if (a.offsets) a.offsets[row] = dst;
+        else a.lens[row] = (uint16_t)e.len;
     }
-    s_off[threadIdx.x] = e.off; s_row[threadIdx.x] = row; s_len[threadIdx.x] = live ? e.len : CONS_NONE;
+    s_off[threadIdx.x] = e.off; s_dst[threadIdx.x] = dst; s_len[threadIdx.x] = live ? e.len : CONS_NONE;
     __syncthreads();
     const uint32_t c = threadIdx.x & 7u;
     for (uint32_t i = threadIdx.x >> 3; i < APUS_CONS_THREADS; i += APUS_CONS_THREADS / 8)
         if (s_len[i] != CONS_NONE)
-            cons_copy_cmd(a.payloads + s_row[i] * a.stride, entries + s_off[i] + E_CMD, s_len[i], c, 8);
+            cons_copy_cmd(a.payloads + s_dst[i], entries + s_off[i] + E_CMD, s_len[i], c, 8);
 }
 
-// 5: the row count, then -- every read of the examined entries has completed with the copy kernel -- the cursor the
+// 5: the row count and (packed) offsets[rows], then -- every read of the examined entries has completed with the copy kernel -- the cursor the
 // follower forwards to the leader's pruning rule, and the status words
 __global__ void apus_consume_tail_kernel(apus_consume_args_t a)
 {
     const apus_cons_state_t *s = a.st;
     apus_ctrl_t *ctrl = reinterpret_cast<apus_ctrl_t *>(a.region);
     *a.count = (uint32_t)s->rows;
+    if (a.offsets) a.offsets[s->rows] = s->bytes;
     const uint64_t nidx = s->next_idx + s->n_exam;
     st_relaxed_sys_2x64(ctrl->cons_cur, s->new_cursor, nidx);
     st_relaxed_sys(&a.hw->cons_cursor, s->new_cursor);

@@ -308,23 +308,27 @@ typedef struct apus_role {
     apus_devctx_t *ctx;
 } apus_role_t;
 
-/* Device consumers (apus_consume_device): the state of one replica's consume work, in device memory ahead of two
- * words per consume block ({rows, then their exclusive scan; stop}).  The cursor itself is apus_ctrl_t.cons_cur. */
+/* Device consumers (apus_consume_device, apus_consume_device_packed): the state of one replica's consume work, in
+ * device memory ahead of APUS_CONS_BLK_WORDS words per consume block ({rows, then their exclusive scan; stop; cmd
+ * bytes of those rows, then their exclusive scan (packed calls)}).  The cursor itself is apus_ctrl_t.cons_cur. */
 typedef struct apus_cons_state {
     uint64_t cursor, next_idx, committed, m;  /* this call: the cursor and the record it starts from, entries to look at */
     uint64_t rows, n_exam, new_cursor, need_stride;   /* ... and what it found */
     uint64_t error;                           /* sticky APUS_CONSUME_BAD_IDX */
-    uint64_t pad[7];
+    uint64_t bytes;                           /* packed calls: cmd bytes of the rows written (offsets[rows]) */
+    uint64_t pad[6];
 } apus_cons_state_t;
 #define APUS_CONS_THREADS 256u                /* entries per consume block */
+#define APUS_CONS_BLK_WORDS 3u
 
-/* one apus_consume_device call as the consume kernels see it */
+/* one consume call as the consume kernels see it: the strided layout (lens and payloads + row * stride) or, when
+ * offsets is set, the packed one (row r's cmd at payloads + offsets[r], at most values_cap bytes in all; lens NULL) */
 typedef struct apus_consume_args {
     uint8_t  *region;                         /* the follower's region (ctrl block, index, entries) */
     uint64_t  entries_off, log_len, stride;
     uint32_t  idx_mask, max_n;                /* max_n <= the index ring's capacity */
     uint32_t  nblk, pad;
-    apus_cons_state_t *st;                    /* followed by 2 * nblk words */
+    apus_cons_state_t *st;                    /* followed by APUS_CONS_BLK_WORDS * nblk words */
     apus_hostwords_t  *hw;                    /* status words (device address of the pinned page) */
     uint64_t *idx;
     uint8_t  *types;
@@ -333,6 +337,8 @@ typedef struct apus_consume_args {
     uint16_t *lens;
     uint8_t  *payloads;
     uint32_t *count;
+    uint64_t *offsets;                        /* packed: max_n + 1 words */
+    uint64_t  values_cap;
 } apus_consume_args_t;
 
 #define APUS_KERNEL_THREADS    512

@@ -65,6 +65,18 @@ APUS_HD int slot_place(uint64_t R, uint64_t head, uint64_t tail, uint64_t need, 
     return 0;
 }
 
+/* The payload-ring reservation of a packed device batch (apus_submit_device_packed): n requests whose cmds lie in
+ * values_bytes bytes.  The host sees neither the lengths nor the types, so it bounds the external images from n and
+ * values_bytes alone: an image of a valid request (len <= 65535) takes round16(2 + len) <= len + 17 bytes, the lengths
+ * of a batch with nondecreasing offsets sum to at most values_bytes, and no request needs more than round16(2 + 65535). */
+APUS_HD uint64_t slot_packed_reserve(uint64_t n, uint64_t values_bytes)
+{
+    const uint64_t worst = n * slot_ext_bytes(2u + 0xffffu);
+    if (values_bytes >= worst) return worst;
+    const uint64_t sum = (values_bytes + 17u * n + 15u) & ~15ull;
+    return sum < worst ? sum : worst;
+}
+
 /* offset inside the 128 B slot of inline image byte i (i < APUS_SLOT_INLINE): bytes 0..31 in inl0, 32..79 in inl1 */
 APUS_HD uint32_t slot_inline_off(uint32_t i) { return i < 32u ? 16u + i : 32u + i; }
 /* the slot's 16 B chunk that holds inline image chunk q (q < 5); chunk 0 is the descriptor, 3 and 7 the stamps */

@@ -68,7 +68,7 @@ EXPORTS = [
     "apus_ctl_send_vote_ack", "apus_ctl_last_entry", "apus_ctl_adjust_follower", "apus_replica_set_role",
     "apus_replica_disconnect", "apus_follower_beats", "apus_device_numa_node", "apus_group_multicast", "apus_ctl_heartbeat",
     "apus_submit_device", "apus_device_submit_status", "apus_stream_wait_committed", "apus_committed_word",
-    "apus_consume_device", "apus_consume_status",
+    "apus_consume_device", "apus_consume_status", "apus_submit_device_packed", "apus_consume_device_packed",
 ]
 
 
@@ -128,6 +128,8 @@ def load_library(path=LIB_PATH):
         L.apus_committed_word.restype = vp
         L.apus_consume_device.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp, C.c_size_t, vp, vp]
         L.apus_consume_status.argtypes = [vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]
+        L.apus_submit_device_packed.argtypes = [vp, u32, vp, vp, vp, vp, vp, u64, vp, C.POINTER(u64)]
+        L.apus_consume_device_packed.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp, u64, vp, vp]
     _lib = L
     return L
 
@@ -277,6 +279,43 @@ class Replica:
             "apus_submit_device")
         return int(t.value)
 
+    def submit_device_packed(self, types, conns, req_ids, offsets, values, stream=None):
+        """n requests in the packed (jagged) layout, packed into the HBM submission ring in `stream` order
+        (apus_submit_device_packed): request k's cmd is values[offsets[k]:offsets[k+1]].  types uint8 [n], conns
+        int16/uint16 [n], req_ids int64 [n] (as uint64), offsets int64 [n+1] (offsets[0] may be > 0), values a 1-D uint8
+        tensor; all contiguous CUDA tensors on the leader's device.  The payload-ring reservation is bounded by
+        values.numel() (min(n * 65552, round16(values.numel() + 17 n)) bytes), so pass only the slice of values the batch
+        uses.  Returns the first ticket.  A type that is not CSM/CONNECT/SEND/CLOSE or a cmd above 65535 B becomes a
+        NOOP entry; offsets that decrease or end past values.numel() turn the whole batch into NOOPs (see
+        device_submit_status())."""
+        import torch
+        dev = torch.device("cuda", self.device)
+        if not isinstance(types, torch.Tensor) or types.dim() != 1:
+            raise ApusError("submit_device_packed: types must be a 1-D uint8 CUDA tensor [n]")
+        n = types.shape[0]
+        spec = (("types", types, (torch.uint8,), (n,)), ("conns", conns, (torch.int16, torch.uint16), (n,)),
+                ("req_ids", req_ids, (torch.int64,), (n,)), ("offsets", offsets, (torch.int64,), (n + 1,)),
+                ("values", values, (torch.uint8,), None))
+        for name, t, dtypes, shape in spec:
+            if not isinstance(t, torch.Tensor):
+                raise ApusError(f"submit_device_packed: {name} must be a torch tensor")
+            if t.device != dev:
+                raise ApusError(f"submit_device_packed: {name} is on {t.device}, the leader is on {dev}")
+            if t.dtype not in dtypes:
+                raise ApusError(f"submit_device_packed: {name} has dtype {t.dtype}, expected one of {dtypes}")
+            if (tuple(t.shape) != shape) if shape else t.dim() != 1:
+                raise ApusError(f"submit_device_packed: {name} has shape {tuple(t.shape)}, expected "
+                                f"{list(shape) if shape else '1-D'}")
+            if not t.is_contiguous():
+                raise ApusError(f"submit_device_packed: {name} is not contiguous")
+        s = self._stream(stream)
+        nv = values.numel()
+        t = u64()
+        _ck(lib().apus_submit_device_packed(self.h, n, types.data_ptr(), conns.data_ptr(), req_ids.data_ptr(),
+                                            offsets.data_ptr(), values.data_ptr() if nv else None, nv, s.cuda_stream,
+                                            C.byref(t)), "apus_submit_device_packed")
+        return int(t.value)
+
     def device_submit_status(self):
         """(requests of device batches written as NOOPs, ticket of the first of them or 0)"""
         rej, first = u64(), u64()
@@ -321,6 +360,47 @@ class Replica:
         _ck(lib().apus_consume_device(self.h, max_n, idx.data_ptr(), types.data_ptr(), conns.data_ptr(),
                                       req_ids.data_ptr(), lens.data_ptr(), payloads.data_ptr() if stride else None,
                                       stride, count.data_ptr(), s.cuda_stream), "apus_consume_device")
+        return out
+
+    def consume_device_packed(self, max_n, values_cap, out=None, stream=None):
+        """consume_device with packed output (apus_consume_device_packed).  Returns (idx int64 [max_n], types uint8
+        [max_n], conns int16 [max_n], req_ids int64 [max_n], offsets int64 [max_n+1], values uint8 [values_cap], count
+        int32 [1]): row r's cmd is values[offsets[r]:offsets[r+1]], offsets[0] = 0, for the count rows written.  The
+        call stops before the first cmd that would end past values_cap; when that is the first row, consume_status()
+        .need_stride is the capacity it needs.  `out`: those seven tensors to fill (allocated when None); int16 or
+        uint16 for conns, int32 or uint32 for count."""
+        import torch
+        dev = torch.device("cuda", self.device)
+        s = self._stream(stream)
+        if out is None:
+            with torch.cuda.stream(s):
+                out = (torch.empty(max_n, dtype=torch.int64, device=dev), torch.empty(max_n, dtype=torch.uint8, device=dev),
+                       torch.empty(max_n, dtype=torch.int16, device=dev), torch.empty(max_n, dtype=torch.int64, device=dev),
+                       torch.empty(max_n + 1, dtype=torch.int64, device=dev),
+                       torch.empty(values_cap, dtype=torch.uint8, device=dev),
+                       torch.empty(1, dtype=torch.int32, device=dev))
+        if len(out) != 7:
+            raise ApusError("consume_device_packed: out must be (idx, types, conns, req_ids, offsets, values, count)")
+        spec = (("idx", (torch.int64,), (max_n,)), ("types", (torch.uint8,), (max_n,)),
+                ("conns", (torch.int16, torch.uint16), (max_n,)), ("req_ids", (torch.int64,), (max_n,)),
+                ("offsets", (torch.int64,), (max_n + 1,)), ("values", (torch.uint8,), (values_cap,)),
+                ("count", (torch.int32, torch.uint32), (1,)))
+        for (name, dtypes, shape), t in zip(spec, out):
+            if not isinstance(t, torch.Tensor):
+                raise ApusError(f"consume_device_packed: {name} must be a torch tensor")
+            if t.device != dev:
+                raise ApusError(f"consume_device_packed: {name} is on {t.device}, the replica is on {dev}")
+            if t.dtype not in dtypes:
+                raise ApusError(f"consume_device_packed: {name} has dtype {t.dtype}, expected one of {dtypes}")
+            if tuple(t.shape) != shape:
+                raise ApusError(f"consume_device_packed: {name} has shape {tuple(t.shape)}, expected {shape}")
+            if not t.is_contiguous():
+                raise ApusError(f"consume_device_packed: {name} is not contiguous")
+        idx, types, conns, req_ids, offsets, values, count = out
+        _ck(lib().apus_consume_device_packed(self.h, max_n, idx.data_ptr(), types.data_ptr(), conns.data_ptr(),
+                                             req_ids.data_ptr(), offsets.data_ptr(),
+                                             values.data_ptr() if values_cap else None, values_cap, count.data_ptr(),
+                                             s.cuda_stream), "apus_consume_device_packed")
         return out
 
     def consume_status(self):
@@ -557,6 +637,14 @@ class Group:
         """Replica.submit_device on the leader; keeps `tickets` up to date so that run() covers the batch."""
         n = payloads.shape[0]
         t0 = self.leader.submit_device(types, conns, req_ids, lens, payloads, stream)
+        if n:
+            self.tickets = t0 + n - 1
+        return t0
+
+    def submit_device_packed(self, types, conns, req_ids, offsets, values, stream=None):
+        """Replica.submit_device_packed on the leader; keeps `tickets` up to date so that run() covers the batch."""
+        n = types.shape[0]
+        t0 = self.leader.submit_device_packed(types, conns, req_ids, offsets, values, stream)
         if n:
             self.tickets = t0 + n - 1
         return t0

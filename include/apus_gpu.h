@@ -216,6 +216,21 @@ uint8_t apus_synth_byte(uint32_t seed, uint64_t req_id, uint32_t k);
 int  apus_submit_device(apus_replica_t *leader, uint32_t n, const uint8_t *types, const uint16_t *connection_ids,
                         const uint64_t *req_ids, const uint16_t *lens, const void *payloads, size_t stride,
                         void *stream, uint64_t *first_ticket);
+/* Requests in device memory in the packed (jagged) layout: request k's cmd is values[offsets[k], offsets[k + 1]),
+ * as in torch's jagged layout (values + offsets[n + 1]); offsets[0] need not be 0, so a slice of a larger buffer may be
+ * passed.  The arrays are device memory on the leader's GPU; offsets and req_ids must be 8 B aligned, connection_ids
+ * 2 B, values may have any alignment (and be NULL when values_bytes is 0).  Stream order, tickets, the doorbell, the
+ * rejection of a type that is not CSM, CONNECT, SEND or CLOSE, APUS_RETRY and APUS_ERROR: as apus_submit_device, except:
+ *   - the payload ring reserves min(n * round16(2 + 65535), round16(values_bytes + 17 n)) bytes (slot_packed_reserve),
+ *     decided from n and values_bytes alone: pass only the slice of values the batch uses;
+ *   - a cmd longer than 65535 B is written as a NOOP and counted;
+ *   - if any offsets[k] > offsets[k + 1], or offsets[n] > values_bytes, EVERY request of the batch is written as a NOOP
+ *     and counted: nothing is read outside values[0, values_bytes) and nothing written outside the reservation.
+ * The packing reads offsets in more than one pass: they, like the other arrays, must not change until `stream` has
+ * passed the call (a caller that rewrites them outside stream order races with the packing). */
+int  apus_submit_device_packed(apus_replica_t *leader, uint32_t n, const uint8_t *types,
+                               const uint16_t *connection_ids, const uint64_t *req_ids, const uint64_t *offsets,
+                               const void *values, uint64_t values_bytes, void *stream, uint64_t *first_ticket);
 /* requests of device batches rejected so far (written as NOOPs) and the ticket of the first of them (0 = none); a
  * batch is counted once its packing has run (e.g. after synchronising the stream it was submitted on) */
 int  apus_device_submit_status(apus_replica_t *leader, uint64_t *rejected, uint64_t *first_rejected_ticket);
@@ -286,6 +301,17 @@ int  apus_log_read_range(apus_replica_t *r, uint64_t from, uint64_t to, void *ds
 int  apus_consume_device(apus_replica_t *follower, uint32_t max_n, uint64_t *idx, uint8_t *types,
                          uint16_t *connection_ids, uint64_t *req_ids, uint16_t *lens, void *payloads, size_t stride,
                          uint32_t *count, void *stream);
+/* apus_consume_device with packed output: row r's cmd goes to values + offsets[r], contiguous and unpadded, with
+ * offsets[0] = 0 and offsets[r + 1] = offsets[r] + its length for the *count rows written (offsets has max_n + 1
+ * words; neither offsets past *count nor bytes of values past offsets[*count] are written).  Everything else as
+ * apus_consume_device, except the stop: the examination stops just before the first CSM-like entry whose cmd would end
+ * past values_cap.  When that entry would be the call's first row, apus_consume_status's need_stride reports its length
+ * (a buffer of at least that many bytes delivers it); a stop after rows were delivered is not an error, the next call
+ * continues there.  idx, req_ids and offsets must be 8 B aligned, count 4 B, connection_ids 2 B; values may have any
+ * alignment (and be NULL when values_cap is 0). */
+int  apus_consume_device_packed(apus_replica_t *follower, uint32_t max_n, uint64_t *idx, uint8_t *types,
+                                uint16_t *connection_ids, uint64_t *req_ids, uint64_t *offsets, void *values,
+                                uint64_t values_cap, uint32_t *count, void *stream);
 #define APUS_CONSUME_BAD_IDX 1   /* an entry at an index word does not carry the expected idx */
 /* the pinned words the consume work writes: the cursor and the idx of the next entry after the latest call that ran,
  * the stride the entry that stopped it needs (0 = it did not stop on a long entry), APUS_CONSUME_* (0 = none) */
