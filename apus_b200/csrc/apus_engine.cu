@@ -1955,6 +1955,23 @@ extern "C" int apus_replica_set_role(apus_replica_t *r, uint8_t leader_idx, uint
     apus_loghdr_t h; apus_ctrl_t c;
     if (own_read(r, APUS_HDR_OFF, &h, sizeof h) != APUS_OK || own_read(r, 0, &c, sizeof c) != APUS_OK) return APUS_ERROR;
     const uint64_t L = r->log_len, last = c.acked;
+    /* adopt the largest commit offset my voters granted me (poll_vote_count, dare_server.c:1356-1362): the old leader's
+     * commit pushes reach its followers at different times, so a voter may know of more committed entries than I do.
+     * Every follower is then told this commit, so none of them runs ahead of mine.  Only offsets in (commit, end] by
+     * ring order from my head are taken: `log_len` means "no vote", and a word left from an earlier election that lies
+     * outside what I hold cannot be a commit of this log. */
+    if (h.end != L) {
+        uint64_t va[16];
+        if (own_read(r, APUS_CTL_OFF + offsetof(apus_ctlwords_t, vote_ack), va, sizeof va) != APUS_OK) return APUS_ERROR;
+        const uint64_t pe = (h.end + L - h.head) % L;
+        uint64_t pc = (h.commit + L - h.head) % L;
+        for (int i = 0; i < 16; i++) {
+            if (i == r->cfg.server_idx || va[i] >= L) continue;
+            const uint64_t pv = (va[i] + L - h.head) % L;
+            if (pv > pc && pv <= pe) { pc = pv; h.commit = va[i]; }
+        }
+        r->hw->commit_off = h.commit;    /* what the host sees as committed until my kernel's first commit store */
+    }
     /* entries between my commit offset and my end are published but not committed: count them by walking the offset
      * index backwards until an entry starts at or before the commit offset */
     uint64_t unc = 0, tail = L;

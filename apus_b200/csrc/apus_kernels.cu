@@ -523,6 +523,15 @@ __device__ __noinline__ void t1_scan(LeaderShared *S, int tid)
     bar_sync(1, NT);
 }
 
+// the apply offset of replica i that the pruning rule reads: mine from my header, a follower's as it reported it, and
+// for a replica I am not connected to (removed, or the leader I took over from) my own: the reference sets the apply
+// offset of a server that is off to the leader's (log_pruning, dare_server.c:2028-2031), so it never holds the head back
+__device__ __forceinline__ uint64_t ld_apply(const apus_devctx_t *__restrict__ cx, const apus_ctrl_t *ctrl,
+                                             const apus_loghdr_t *hdr, int i)
+{
+    return (i == cx->idx || !cx->peer[i]) ? ld_relaxed_sys(&hdr->apply) : ld_relaxed_sys(&ctrl->apply_off[i]);
+}
+
 // T2b (inside the place turn): place the next sub-tile of the fetched batch (entries kbase..nf) --
 // log_append_entry's offset rules, free-space rule E2 and the pruning rule, on the placement
 // state this CTA holds.  Kept short: everything state independent was done by t1_scan.
@@ -1441,7 +1450,6 @@ __device__ __forceinline__ void t1_fetch(const apus_devctx_t *__restrict__ cx, L
 // (S->fast); else leave the state in S->st for leader_place.
 __device__ __forceinline__ void place_fast(const apus_devctx_t *__restrict__ cx, LeaderShared *S, LeaderProf &P)
 {
-    const int me = cx->idx;
     apus_ctrl_t *ctrl = reinterpret_cast<apus_ctrl_t *>(cx->region);
     apus_seq_t *seq = reinterpret_cast<apus_seq_t *>(cx->region + APUS_SEQ_OFF);
     apus_loghdr_t *hdr = reinterpret_cast<apus_loghdr_t *>(cx->region + APUS_HDR_OFF);
@@ -1463,8 +1471,7 @@ __device__ __forceinline__ void place_fast(const apus_devctx_t *__restrict__ cx,
     bool prune_due = false;
     if (autoprune && r.end != L && used >= (L >> 2) && !r.prev_head && L - pos0 >= APUS_HDR_BYTES) {
         if (!S->ap_valid) {
-            for (int i = 0; i < cx->group_size; i++)
-                S->ap[i] = (i == me) ? ld_relaxed_sys(&hdr->apply) : ld_relaxed_sys(&ctrl->apply_off[i]);
+            for (int i = 0; i < cx->group_size; i++) S->ap[i] = ld_apply(cx, ctrl, hdr, i);
             S->ap_valid = 1;
         }
         uint64_t d = 0;
@@ -1519,7 +1526,7 @@ __device__ __forceinline__ void place_fast(const apus_devctx_t *__restrict__ cx,
 __device__ __forceinline__ void t2_place(const apus_devctx_t *__restrict__ cx, LeaderShared *S, bool have_place_turn,
                                          LeaderProf &P, int lane)
 {
-    const int N = cx->group_size, me = cx->idx;
+    const int N = cx->group_size;
     apus_ctrl_t *ctrl = reinterpret_cast<apus_ctrl_t *>(cx->region);
     apus_seq_t *seq = reinterpret_cast<apus_seq_t *>(cx->region + APUS_SEQ_OFF);
     apus_loghdr_t *hdr = reinterpret_cast<apus_loghdr_t *>(cx->region + APUS_HDR_OFF);
@@ -1529,7 +1536,7 @@ __device__ __forceinline__ void t2_place(const apus_devctx_t *__restrict__ cx, L
         if (S->fast) return;
     }
     if (!S->ap_valid) {
-        if (lane < N) S->ap[lane] = (lane == me) ? ld_relaxed_sys(&hdr->apply) : ld_relaxed_sys(&ctrl->apply_off[lane]);
+        if (lane < N) S->ap[lane] = ld_apply(cx, ctrl, hdr, lane);
         __syncwarp();
         if (lane == 0) S->ap_valid = 1;
         __syncwarp();
@@ -1846,7 +1853,7 @@ __device__ void leader_main(const apus_devctx_t *__restrict__ cx, const uint32_t
                         st_relaxed_sys(&seq->abort_flag, 1); S->finish = 1;
                     }
                 }
-                if (tid < N) S->ap[tid] = (tid == me) ? ld_relaxed_sys(&hdr->apply) : ld_relaxed_sys(&ctrl->apply_off[tid]);
+                if (tid < N) S->ap[tid] = ld_apply(cx, ctrl, hdr, tid);
                 bar_sync(1, NT);
                 if (S->finish) { aborted = true; break; }
                 continue;

@@ -54,5 +54,9 @@ uint32_t orc_sizeof_entry(void) { return ORC_HDR; }
 #define L_GET_TAIL(l) orc_get_tail(l)
 #define L_PREV_HEAD(l) ((l)->prev_head)
 #define L_NORM(l, off) (((l)->rules == ORC_RULES_ENGINE && (off) == (l)->len) ? 0 : (off))
+static orc_nc_buf_t g_nc[ORC_MAX_SERVER_COUNT];   /* the leader's nc_buf[i] (dare_log.h:99) */
+#define L_NC_MAX ORC_NC_MAX
+#define L_NC_BUILD(l, f, i) (orc_entries_to_nc_buf((f), &g_nc[i]), g_nc[i].len)
+#define L_FIND_REMOTE_END(l, i) orc_find_remote_end_offset((l), &g_nc[i])
 #include "cluster_sim.inc"
 #include "cpu_bench.inc"

@@ -7,7 +7,8 @@
  * links or falls back to this code.
  *
  * What it restates (reference = /root/reference, hku-systems/apus):
- *   src/include/dare/dare_log.h   the circular log: layout, append, walkers
+ *   src/include/dare/dare_log.h   the circular log: layout, append, walkers, and the
+ *                                 not-committed-entry list of log adjustment
  * Every function cites the reference lines it follows.  The restatement is an
  * independent re-write working on explicit byte offsets (no struct overlay), so
  * it also documents the byte layout the CUDA engine must reproduce:
@@ -251,6 +252,46 @@ static uint64_t orc_append(orc_log_t *l, uint64_t term, uint64_t req_id, uint16_
     l->end += orc_entry_len(e);                                   /* :549 */
     if (l->rules == ORC_RULES_ENGINE && l->end == l->len) l->end = 0;   /* E1 */
     return idx;
+}
+
+/* dare_log.h:50-65: {idx, term, offset} of every entry that is not committed */
+#define ORC_NC_MAX 1024                         /* MAX_NC_ENTRIES */
+typedef struct orc_nc_buf {
+    uint64_t len;
+    struct { uint64_t idx, term, offset; } e[ORC_NC_MAX];
+} orc_nc_buf_t;
+
+/* dare_log.h:340-359 log_entries_to_nc_buf: walk from the commit offset to the end;
+ * the offset recorded is where the walk found the header (a ghost's, for an entry
+ * that continues at 0) */
+static void orc_entries_to_nc_buf(orc_log_t *l, orc_nc_buf_t *nc)
+{
+    uint64_t off = l->commit, n = 0;
+    uint8_t *e;
+    while ((e = orc_get_entry(l, &off)) != NULL) {
+        nc->e[n].idx = orc_ld64(e + ORC_OFF_IDX);
+        nc->e[n].term = orc_ld64(e + ORC_OFF_TERM);
+        nc->e[n].offset = off;
+        n++;
+        orc_walk_next(l, &off, e);
+    }
+    nc->len = n;
+}
+
+/* dare_log.h:368-394 log_find_remote_end_offset: the offset of the first listed
+ * entry that this log does not hold at the same offset with the same {idx, term},
+ * or the offset behind the last one */
+static uint64_t orc_find_remote_end_offset(orc_log_t *l, const orc_nc_buf_t *nc)
+{
+    uint64_t off = 0;
+    for (uint64_t i = 0; i < nc->len; i++) {
+        off = nc->e[i].offset;
+        uint8_t *e = orc_get_entry(l, &off);
+        if (!e) return off;
+        if (orc_ld64(e + ORC_OFF_IDX) != nc->e[i].idx || orc_ld64(e + ORC_OFF_TERM) != nc->e[i].term) return off;
+        orc_walk_next(l, &off, e);
+    }
+    return off;
 }
 
 /* FNV-1a 64 over a byte range; the checksum quoted in SURVEY.md s8c */

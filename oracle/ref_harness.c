@@ -10,7 +10,8 @@
  * replicate/ack/commit/apply steps come from cluster_sim.inc (the files holding
  * them in the reference need libibverbs/libev and cannot be compiled here) but
  * run on the reference's log_append_entry / log_get_entry / log_fit_entry /
- * log_entry_len / log_offset_end_distance / log_is_offset_larger / log_get_tail.
+ * log_entry_len / log_offset_end_distance / log_is_offset_larger / log_get_tail, and log adjustment on its
+ * log_entries_to_nc_buf / log_find_remote_end_offset.
  *
  * Built only where /root/reference exists (oracle/Makefile target `ref`); the
  * resulting .so travels to the GPU box, the reference tree does not.
@@ -95,5 +96,10 @@ uint64_t ref_log_size(void) { return (uint64_t)(LOG_SIZE); }
 #define L_GET_TAIL(l) log_get_tail(l)
 #define L_PREV_HEAD(l) prev_log_entry_head
 #define L_NORM(l, off) (off)
+/* log adjustment: the follower builds the list in its own log (server_to_follower); the leader reads it into its
+ * nc_buf[i] (LR_GET_NCE) -- here built straight into the leader's slot, which holds the same bytes */
+#define L_NC_MAX MAX_NC_ENTRIES
+#define L_NC_BUILD(l, f, i) (log_entries_to_nc_buf((f), &(l)->nc_buf[i]), (l)->nc_buf[i].len)
+#define L_FIND_REMOTE_END(l, i) log_find_remote_end_offset((l), &(l)->nc_buf[i])
 #include "cluster_sim.inc"
 #include "cpu_bench.inc"

@@ -176,21 +176,25 @@ class Replay:
         self.c.close()
 
     def end(self):
-        return self.c.offsets(0)["end"]
+        return self.c.offsets(self.c.leader)["end"]
 
-    def launch(self, lc, requests, replica=0, on_head=None):
+    def launch(self, lc, requests, replica=None, on_head=None, live=None):
         """Append what one launch appended (`lc`, read back from replica `replica`; `requests` the submitted stream, a
         CONFIG request standing for the prologue), run two quiescent rounds and poll_head on every follower, then
         compare the oracle's bytes of that replica in the launch's range with the ones read back: every entry the
         launch wrote, before a later lap overwrites it.  A follower's reply bytes are masked: nothing orders its own
         reply-byte stores before a host read of a committed range.  `on_head(entry, abs_start, prev_abs_start)`, called
-        for every HEAD entry once appended, returns None or why that HEAD could not have been taken when it was."""
+        for every HEAD entry once appended, returns None or why that HEAD could not have been taken when it was.
+        `replica` defaults to the leader; `live` (follower indices, default all) are the followers that ran: only they
+        receive, ack and poll heads in the oracle's rounds."""
         c, L = self.c, self.L
+        lead = c.leader
+        replica = lead if replica is None else replica
         src = "" if replica == c.leader else f"follower {replica}'s read: "
         for e in lc.entries:
-            before = c.offsets(0)
+            before = c.offsets(lead)
             if e.typ == O.HEAD:
-                b = live_boundaries(oracle_view(c, 0), before["head"], before["end"], L)
+                b = live_boundaries(oracle_view(c, lead), before["head"], before["end"], L)
                 nxt = request_stride(requests[self.pos]) if self.pos < len(requests) else None
                 why = head_violation(L, before["head"], before["end"], e.value, b, self.prev_head, nxt)
                 assert why is None, f"{src}HEAD idx {e.idx} at {e.off}: {why}"
@@ -206,7 +210,7 @@ class Replay:
                 assert got == want, f"entry idx {e.idx} at {e.off}: engine {got}, request {self.pos - 1} is {want}"
                 idx = c.prologue() if typ == O.CONFIG else c.submit(typ, clt, rid, O.cmd_image(payload))
                 self.prev_head = False
-            after = c.offsets(0)
+            after = c.offsets(lead)
             assert idx == e.idx, f"engine idx {e.idx} at {e.off}, oracle appended idx {idx}"
             assert after["tail"] == e.off, f"idx {e.idx}: engine wrote it at {e.off}, the oracle at {after['tail']}"
             start = 0 if before["end"] == L else before["end"]
@@ -220,13 +224,13 @@ class Replay:
                     assert why is None, f"{src}HEAD idx {e.idx} at {e.off}: {why}"
                 # commit it and let the followers poll it now: poll_head keeps the head closer to `end`, and a follower
                 # head left stale while the launch laps most of the ring would look closer than the new one
-                c.round()
-                c.round()
-                poll_heads(c, self.cid)
-        assert c.offsets(0)["end"] == lc.end, f"engine end {lc.end}, oracle end {c.offsets(0)['end']}"
-        c.round()
-        c.round()
-        poll_heads(c, self.cid)
+                c.round(live=live)
+                c.round(live=live)
+                poll_heads(c, self.cid, live)
+        assert c.offsets(lead)["end"] == lc.end, f"engine end {lc.end}, oracle end {c.offsets(lead)['end']}"
+        c.round(live=live)
+        c.round(live=live)
+        poll_heads(c, self.cid, live)
         if len(lc.buf):
             pos = (lc.start + np.arange(len(lc.buf))) % L
             mine, want = lc.buf, oracle_view(c, replica)[pos]
@@ -248,10 +252,11 @@ class Replay:
         return self.heads[-1].value if self.heads else 0
 
 
-def poll_heads(c, cid):
-    """SIM(poll_head) on every follower of the oracle cluster `c`; `cid`: each replica's scan position, carried over"""
+def poll_heads(c, cid, live=None):
+    """SIM(poll_head) on every follower of the oracle cluster `c` (on those in `live`, when given); `cid`: each replica's
+    scan position, carried over"""
     for i in range(c.n):
-        if i != c.leader:
+        if i != c.leader and (live is None or i in live):
             cur = C.c_uint64(cid[i])
             c.poll_head(i, C.byref(cur))
             cid[i] = int(cur.value)

@@ -89,6 +89,8 @@ class Oracle:
         # newer than the rest of the API: a library built by an older recipe (a prebuilt oracle/_ref kept where the
         # reference tree is absent) lacks it, and everything else in it still works
         f("prune_to", u64, [vp, u64], optional=True)
+        f("take_over", None, [vp, C.c_int, u64, C.POINTER(u64)], optional=True)
+        f("adjust", u64, [vp, C.c_int], optional=True)
         f("round", None, [vp])
         f("cluster_offsets", None, [vp, C.c_int, C.POINTER(u64)])
         f("cluster_entries", C.POINTER(u8), [vp, C.c_int])
@@ -188,6 +190,19 @@ class Cluster:
         """SIM(prune_to): head := `head` and append <HEAD, head>, without the pruning rule's checks (the replay of a
         run whose HEAD entries the engine decided, tests/autoprune_replay.py).  Returns the HEAD idx, 0 when full."""
         return self.o.prune_to(self.h, head)
+
+    def take_over(self, winner, term, vote_commits):
+        """SIM(take_over): `winner` leads in `term`, adopting the largest commit offset among `vote_commits`
+        ({voter: commit offset}).  Call prologue() next, then adjust() for each voter."""
+        arr = (u64 * self.n)(*[vote_commits.get(i, self.len) for i in range(self.n)])
+        self.o.take_over(self.h, winner, term, arr)
+        self.leader = winner
+
+    def adjust(self, i):
+        """SIM(adjust): log adjustment of voter i; returns the shared end (remote_end[i], now follower i's end)."""
+        re = int(self.o.adjust(self.h, i))
+        assert re <= self.len, f"follower {i} holds more not-committed entries than the reference's list takes"
+        return re
 
     def round(self, live=None):
         """One round of SIM(round) (oracle/cluster_sim.inc).  With `live` (follower indices), only those followers
