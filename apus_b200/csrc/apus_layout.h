@@ -1,6 +1,7 @@
 /*
  * apus_layout.h -- HBM layout of one replica and the structures shared between
- * the host engine (apus_engine.cu) and the kernels (apus_kernels.cu).
+ * the host engine (apus_engine.cu) and the kernels (the replica kernel of
+ * apus_kernels.cu, the batch kernels of apus_batch.cu).
  *
  * One cudaMalloc'd REGION per replica (one IPC handle maps all of it in a peer):
  *
@@ -340,6 +341,30 @@ typedef struct apus_consume_args {
     uint64_t *offsets;                        /* packed: max_n + 1 words */
     uint64_t  values_cap;
 } apus_consume_args_t;
+
+/* Device batches (apus_submit_device, apus_submit_device_packed): one batch as the packing kernels see it, in either
+ * layout.  A packing block has as many threads as a consume block (the two share one block scan). */
+#define APUS_PACK_THREADS 256u     /* requests per packing block */
+/* words per packing block: external bytes (-> their exclusive scan), rejected, first rejected, and the packed layout's
+ * verdict: the block saw offsets that decrease or end past values_bytes (-> the whole batch's verdict) */
+#define APUS_PACK_BLK_WORDS 4u
+static inline uint32_t apus_pack_blocks(uint64_t n) { return (uint32_t)((n + APUS_PACK_THREADS - 1) / APUS_PACK_THREADS); }
+typedef struct apus_pack_args {
+    apus_slot_t *ring;
+    uint8_t *pay;
+    uint64_t *blk;                /* APUS_PACK_BLK_WORDS per block, see above */
+    const uint8_t *types;
+    const uint16_t *conns;
+    const uint64_t *req_ids;
+    const uint16_t *lens;         /* strided layout (apus_submit_device): cmd k is payloads[k * stride, + lens[k]) */
+    const uint64_t *offsets;      /* packed layout (apus_submit_device_packed, lens NULL): cmd k is
+                                     payloads[offsets[k], offsets[k + 1]), inside [0, values_bytes) */
+    const uint8_t *payloads;
+    uint64_t stride, values_bytes;
+    uint64_t first_slot;          /* submitted count before the batch: request k gets ticket first_slot + k + 1 */
+    uint64_t res_pos;             /* ring position of the batch's payload reservation */
+    uint32_t n, mask;
+} apus_pack_args_t;
 
 #define APUS_KERNEL_THREADS    512
 #define APUS_MAX_TILE_ENTRIES  512u             /* slots fetched per tile (48 KiB of shared memory) */

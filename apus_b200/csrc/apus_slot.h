@@ -1,8 +1,9 @@
 /*
  * apus_slot.h -- the submission-slot format (DESIGN.md section 2), written by the host submit paths
- * (apus_engine.cu: ring_put, apus_submit_uniform), by the device fill kernels (apus_synth_kernel and the
- * packing kernel of apus_submit_device) and checked on the CPU by tests/hostlogic/slot_props.c, which is why it
- * compiles as plain C as well.
+ * (apus_engine.cu: ring_put, apus_submit_uniform), by the device fill kernels (apus_batch.cu: apus_synth_kernel and
+ * the packing kernels of apus_submit_device) and checked on the CPU by tests/hostlogic/slot_props.c, which is why it
+ * compiles as plain C as well.  The payload bytes of synthetic requests (synth_word) are defined here too, for the
+ * fill kernel and the host alike.
  *
  * A request's data image (sm_cmd_t {u16 len; cmd[]}, the 16 B dare_cid_t of CONFIG, the 8 B offset of HEAD) travels
  * inline in its 128 B slot when it has at most APUS_SLOT_INLINE bytes, else in the payload byte ring at a 16 B aligned
@@ -126,5 +127,18 @@ APUS_HD void slot_finish(apus_slot_t *d, uint64_t ticket, uint32_t type_off, uin
     __atomic_store_n(&d->stamp1, ticket, __ATOMIC_RELEASE);
     __atomic_store_n(&d->stamp0, ticket, __ATOMIC_RELEASE);
 #endif
+}
+
+/* payload byte k of the synthetic request `req_id` (apus_submit_synth): the fill kernel writes it, the host's
+ * apus_synth_byte reads it back */
+APUS_HD uint32_t synth_word(uint32_t seed, uint64_t req_id, uint32_t w)
+{
+    uint32_t x = seed ^ ((uint32_t)req_id * 0x9E3779B1u) ^ ((uint32_t)(req_id >> 32) * 0x7F4A7C15u) ^ (w * 0x85EBCA77u);
+    x ^= x >> 16; x *= 0x7feb352du; x ^= x >> 15; x *= 0x846ca68bu; x ^= x >> 16;
+    return x;
+}
+APUS_HD uint8_t synth_byte(uint32_t seed, uint64_t req_id, uint32_t k)
+{
+    return (uint8_t)(synth_word(seed, req_id, k >> 2) >> (8u * (k & 3u)));
 }
 #endif /* APUS_SLOT_H */

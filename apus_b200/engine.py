@@ -498,7 +498,7 @@ class Replica:
 
 def synth_payload(seed: int, req_id: int, length: int) -> bytes:
     """Payload of the device-generated request `req_id` (apus_submit_synth), computed on the host with numpy --
-    the same integer mix the fill kernel runs (apus_engine.cu: synth_word)."""
+    the same integer mix the fill kernel runs (apus_slot.h: synth_word)."""
     if length == 0:
         return b""
     w = np.arange((length + 3) // 4, dtype=np.uint64)

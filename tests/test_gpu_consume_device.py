@@ -20,6 +20,7 @@ from test_gpu_prune_in_launch import _submit_all
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(600)]
 
 FOREVER = EU.FOREVER
+SENTINEL = 0xA5
 
 
 @pytest.fixture(scope="module")
@@ -76,20 +77,40 @@ def close_all(eng, reps):
             r.close()
 
 
-class Consumer:
-    """One follower's device consumer: consume_device into reused tensors on its own stream, rows copied to the host
-    only to be checked"""
+class _ConsumerBase:
+    """What a follower's device consumer keeps in either layout: its own stream, the rows received, the calls made and
+    the cursors reported"""
 
-    def __init__(self, rep, stride, cap):
+    def __init__(self, rep):
         import torch
-        self.rep, self.stride, self.cap = rep, stride, cap
+        self.rep = rep
         self.stream = torch.cuda.Stream(device=rep.device)
-        self.out = None
         self.rows = []            # (idx, type, conn, req_id, cmd bytes)
         self.calls = 0
         # cursors as absolute positions (ring bytes consumed), each with the time its call was made: the cursor did
         # not exist before that, so a HEAD read earlier cannot legitimately carry it
         self.cur, self.at, self.reports = 0, 0, []
+
+    def _status(self, t_call):
+        """after a call made at t_call: its status, which must carry no error, and the cursor it reported"""
+        self.calls += 1
+        st = self.rep.consume_status()
+        assert st.error == 0, st
+        adv = (st.cursor - self.cur) % self.rep.log_len
+        if adv:
+            self.cur, self.at = st.cursor, self.at + adv
+            self.reports.append((self.at, t_call))
+        return st
+
+
+class Consumer(_ConsumerBase):
+    """One follower's device consumer: consume_device into reused tensors on its own stream, rows copied to the host
+    only to be checked"""
+
+    def __init__(self, rep, stride, cap):
+        super().__init__(rep)
+        self.stride, self.cap = stride, cap
+        self.out = None
 
     def step(self, max_n, stride=None):
         stride = self.stride if stride is None else stride
@@ -102,13 +123,76 @@ class Consumer:
         idx, ty, co, rq, ln, pl = (t[:k].cpu().numpy() for t in self.out[:6])
         for q in range(k):
             self.rows.append((int(idx[q]), int(ty[q]), int(co[q]) & 0xFFFF, int(rq[q]), pl[q, :int(ln[q]) & 0xFFFF].tobytes()))
-        self.calls += 1
-        st = self.rep.consume_status()
-        assert st.error == 0, st
-        adv = (st.cursor - self.cur) % self.rep.log_len
-        if adv:
-            self.cur, self.at = st.cursor, self.at + adv
-            self.reports.append((self.at, t_call))
+        return k, self._status(t_call)
+
+
+class PackedConsumer(_ConsumerBase):
+    """One follower's packed device consumer: consume_device_packed into slices of reused buffers on its own stream,
+    with a sentinel in the output before every call.  values_cap is chosen from the lengths of the rows still to come
+    (`lens`): on a cumulative boundary, one byte short of it or one byte past it; after a stop on the first row, the
+    capacity need_stride asks for.  Rows are copied to the host only to be checked."""
+
+    def __init__(self, rep, lens, max_n_cap=4096, cap_max=1 << 22, seed=0):
+        import torch
+        super().__init__(rep)
+        self.lens = np.asarray(lens, dtype=np.int64)
+        dev = torch.device("cuda", rep.device)
+        with torch.cuda.stream(self.stream):
+            self.buf = (torch.empty(max_n_cap, dtype=torch.int64, device=dev),
+                        torch.empty(max_n_cap, dtype=torch.uint8, device=dev),
+                        torch.empty(max_n_cap, dtype=torch.int16, device=dev),
+                        torch.empty(max_n_cap, dtype=torch.int64, device=dev),
+                        torch.empty(max_n_cap + 1, dtype=torch.int64, device=dev),
+                        torch.empty(cap_max, dtype=torch.uint8, device=dev),
+                        torch.empty(1, dtype=torch.int32, device=dev))
+        self.cap_max = cap_max
+        self.rng = np.random.default_rng(seed)
+        self.need = 0
+        self.exact = None            # set: every row still to come is committed, and no NOOP / CONFIG / HEAD is ahead
+
+    def pick_cap(self, max_n):
+        nxt = self.lens[len(self.rows):len(self.rows) + max_n]
+        if self.need:
+            return self.need
+        if len(nxt) == 0:
+            return int(self.rng.integers(0, 70000))
+        cum = np.cumsum(nxt)
+        r = int(self.rng.integers(0, len(cum)))
+        return int(min(self.cap_max, max(0, cum[r] + int(self.rng.integers(-1, 2)))))
+
+    def step(self, max_n, cap=None):
+        import torch
+        cap = self.pick_cap(max_n) if cap is None else cap
+        idx, ty, co, rq, of, va, cn = self.buf
+        out = (idx[:max_n], ty[:max_n], co[:max_n], rq[:max_n], of[:max_n + 1], va[:cap], cn)
+        with_exact = self.exact is not None and self.exact()
+        with torch.cuda.stream(self.stream):
+            of.fill_(-7)
+            va[:min(cap + 1, self.cap_max)].fill_(SENTINEL)
+        t_call = time.perf_counter()
+        self.rep.consume_device_packed(max_n, cap, out=out, stream=self.stream)
+        self.stream.synchronize()
+        k = int(cn.cpu()[0])
+        offs = of[:max_n + 1].cpu().numpy()
+        vals = va[:min(cap + 1, self.cap_max)].cpu().numpy()
+        assert offs[0] == 0 and np.all(np.diff(offs[:k + 1]) >= 0), offs[:k + 1]
+        assert np.all(offs[k + 1:] == -7), "offsets past count were written"
+        assert offs[k] <= cap
+        assert np.all(vals[offs[k]:] == SENTINEL), "bytes past offsets[count] were written"
+        ii, tt, cc, rr = (x[:k].cpu().numpy() for x in (idx, ty, co, rq))
+        for q in range(k):
+            self.rows.append((int(ii[q]), int(tt[q]), int(cc[q]) & 0xFFFF, int(rr[q]), vals[offs[q]:offs[q + 1]].tobytes()))
+        st = self._status(t_call)
+        nxt = self.lens[len(self.rows) - k:len(self.rows) - k + max_n]
+        if with_exact and len(nxt):
+            cum = np.cumsum(nxt)
+            want = int(np.searchsorted(cum, cap, side="right"))
+            assert k == min(max_n, len(nxt), want), (k, max_n, len(nxt), want, cap)
+            if want == 0:
+                assert st.need_stride == nxt[0], (st.need_stride, nxt[0])
+        if k:
+            assert st.need_stride == 0, st
+        self.need = st.need_stride
         return k, st
 
 
@@ -278,14 +362,16 @@ def heads_against_reports(L, segs, reports, lagging, hits):
     return on_head
 
 
+@pytest.mark.parametrize("layout", ["strided", "packed"])
 @pytest.mark.parametrize("kind,L,ctas", [("ragged1500", 1 << 18, 2), ("sized3k9k", 1 << 15, 4)])
-def test_pruning_in_one_launch_replayed(eng, orc, kind, L, ctas):
+def test_pruning_in_one_launch_replayed(eng, orc, kind, L, ctas, layout):
     """One launch laps a small ring more than six times with APUS_F_AUTOPRUNE.  Followers 2 and 3 consume on the
-    device from host threads, 3 lagging with small max_n and pauses; follower 1's host applies through a recorder
-    (APUS_F_HOST_APPLY), which gives the replay the leader's append sequence byte for byte.  Every HEAD entry must carry
-    a head no further than any follower's report made before the HEAD was first read -- the lagging consumer's cursor
-    among them -- and be one of those reports; the HEADs are replayed into the oracle, every recorded read is compared
-    with it, and at the end every byte and offset of every replica.  Every row of every consumer equals the stream."""
+    device, strided or packed, from host threads, 3 lagging with small max_n and pauses; follower 1's host applies
+    through a recorder (APUS_F_HOST_APPLY), which gives the replay the leader's append sequence byte for byte.  Every
+    HEAD entry must carry a head no further than any follower's report made before the HEAD was first read -- the
+    lagging consumer's cursor among them -- and be one of those reports; the HEADs are replayed into the oracle, every
+    recorded read is compared with it, and at the end every byte and offset of every replica.  Every row of every
+    consumer equals the stream."""
     from apus_b200 import engine as E
     n = 4
     stream, stride = _lap_case(kind, L)
@@ -295,7 +381,11 @@ def test_pruning_in_one_launch_replayed(eng, orc, kind, L, ctas):
     rec = AR.Recorder(reps[1], 1, L)
     rp = AR.Replay(orc, n, L)
     try:
-        cons = [Consumer(r, stride, 256) for r in reps[2:]]
+        if layout == "strided":
+            cons = [Consumer(r, stride, 256) for r in reps[2:]]
+        else:
+            cons = [PackedConsumer(r, [len(p) for *_, p in stream], max_n_cap=256, cap_max=1 << 20, seed=90 + k)
+                    for k, r in enumerate(reps[2:])]
         errs, total = [], {}
 
         def run(cn, lag, seed):

@@ -3,19 +3,17 @@ ragged byte data.  apus_submit_device_packed batches are checked byte for byte a
 strided device batches and host batches; apus_consume_device_packed rows are checked against the request stream and,
 where the log does not lap, the oracle's log, with the capacity stop exercised on, one byte short of and one byte past
 the cumulative boundaries of the rows.  Marked gpu."""
-import threading
 import time
 import types as T
 
 import numpy as np
 import pytest
 
-import autoprune_replay as AR
 import engine_util as EU
 import orc as O
 import streams as S
-from test_gpu_consume_device import (_lap_case, check_rows, close_all, consumer_group, drain, heads_against_reports,
-                                     oracle_rows, wait_forwarded)
+from test_gpu_consume_device import (PackedConsumer, check_rows, close_all, consumer_group, drain, oracle_rows,
+                                     wait_forwarded)
 from test_gpu_device_submit import submit_host, tensors
 from test_gpu_parity import MODES, devices_for, prune_both, wrap_stream
 from test_gpu_prune_in_launch import _submit_all
@@ -23,7 +21,6 @@ from test_gpu_prune_in_launch import _submit_all
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(600)]
 
 FOREVER = EU.FOREVER
-SENTINEL = 0xA5
 
 
 @pytest.fixture(scope="module")
@@ -301,83 +298,6 @@ def test_batch_verdict_reaches_every_block(eng, orc, bad):
         c.close()
 
 
-class PackedConsumer:
-    """One follower's packed device consumer: consume_device_packed into slices of reused buffers on its own stream,
-    with a sentinel in the output before every call.  values_cap is chosen from the lengths of the rows still to come
-    (`lens`): on a cumulative boundary, one byte short of it or one byte past it; after a stop on the first row, the
-    capacity need_stride asks for.  Rows are copied to the host only to be checked."""
-
-    def __init__(self, rep, lens, max_n_cap=4096, cap_max=1 << 22, seed=0):
-        import torch
-        self.rep, self.lens = rep, np.asarray(lens, dtype=np.int64)
-        self.stream = torch.cuda.Stream(device=rep.device)
-        dev = torch.device("cuda", rep.device)
-        with torch.cuda.stream(self.stream):
-            self.buf = (torch.empty(max_n_cap, dtype=torch.int64, device=dev),
-                        torch.empty(max_n_cap, dtype=torch.uint8, device=dev),
-                        torch.empty(max_n_cap, dtype=torch.int16, device=dev),
-                        torch.empty(max_n_cap, dtype=torch.int64, device=dev),
-                        torch.empty(max_n_cap + 1, dtype=torch.int64, device=dev),
-                        torch.empty(cap_max, dtype=torch.uint8, device=dev),
-                        torch.empty(1, dtype=torch.int32, device=dev))
-        self.cap_max = cap_max
-        self.rng = np.random.default_rng(seed)
-        self.rows, self.calls, self.need = [], 0, 0
-        self.cur, self.at, self.reports = 0, 0, []
-        self.exact = None            # set: every row still to come is committed, and no NOOP / CONFIG / HEAD is ahead
-
-    def pick_cap(self, max_n):
-        nxt = self.lens[len(self.rows):len(self.rows) + max_n]
-        if self.need:
-            return self.need
-        if len(nxt) == 0:
-            return int(self.rng.integers(0, 70000))
-        cum = np.cumsum(nxt)
-        r = int(self.rng.integers(0, len(cum)))
-        return int(min(self.cap_max, max(0, cum[r] + int(self.rng.integers(-1, 2)))))
-
-    def step(self, max_n, cap=None):
-        import torch
-        cap = self.pick_cap(max_n) if cap is None else cap
-        idx, ty, co, rq, of, va, cn = self.buf
-        out = (idx[:max_n], ty[:max_n], co[:max_n], rq[:max_n], of[:max_n + 1], va[:cap], cn)
-        with_exact = self.exact is not None and self.exact()
-        with torch.cuda.stream(self.stream):
-            of.fill_(-7)
-            va[:min(cap + 1, self.cap_max)].fill_(SENTINEL)
-        t_call = time.perf_counter()
-        self.rep.consume_device_packed(max_n, cap, out=out, stream=self.stream)
-        self.stream.synchronize()
-        k = int(cn.cpu()[0])
-        offs = of[:max_n + 1].cpu().numpy()
-        vals = va[:min(cap + 1, self.cap_max)].cpu().numpy()
-        assert offs[0] == 0 and np.all(np.diff(offs[:k + 1]) >= 0), offs[:k + 1]
-        assert np.all(offs[k + 1:] == -7), "offsets past count were written"
-        assert offs[k] <= cap
-        assert np.all(vals[offs[k]:] == SENTINEL), "bytes past offsets[count] were written"
-        ii, tt, cc, rr = (x[:k].cpu().numpy() for x in (idx, ty, co, rq))
-        for q in range(k):
-            self.rows.append((int(ii[q]), int(tt[q]), int(cc[q]) & 0xFFFF, int(rr[q]), vals[offs[q]:offs[q + 1]].tobytes()))
-        self.calls += 1
-        st = self.rep.consume_status()
-        assert st.error == 0, st
-        nxt = self.lens[len(self.rows) - k:len(self.rows) - k + max_n]
-        if with_exact and len(nxt):
-            cum = np.cumsum(nxt)
-            want = int(np.searchsorted(cum, cap, side="right"))
-            assert k == min(max_n, len(nxt), want), (k, max_n, len(nxt), want, cap)
-            if want == 0:
-                assert st.need_stride == nxt[0], (st.need_stride, nxt[0])
-        if k:
-            assert st.need_stride == 0, st
-        self.need = st.need_stride
-        adv = (st.cursor - self.cur) % self.rep.log_len
-        if adv:
-            self.cur, self.at = st.cursor, self.at + adv
-            self.reports.append((self.at, t_call))
-        return k, st
-
-
 @pytest.mark.parametrize("kind", ["ragged", "heavy"])
 @pytest.mark.parametrize("mode", sorted(MODES))
 def test_packed_consumption_matches_oracle(eng, orc, mode, kind):
@@ -451,93 +371,6 @@ def test_capacity_stop(eng):
             assert k6 == 0 and st6.need_stride == 0
     finally:
         close_all(eng, reps)
-
-
-@pytest.mark.parametrize("kind,L,ctas", [("ragged1500", 1 << 18, 2), ("sized3k9k", 1 << 15, 4)])
-def test_packed_pruning_in_one_launch_replayed(eng, orc, kind, L, ctas):
-    """One launch laps a small ring more than six times with APUS_F_AUTOPRUNE.  Followers 2 and 3 consume packed on the
-    device, 3 lagging with small max_n and pauses; follower 1's host applies through a recorder.  Every HEAD entry must
-    carry a head no further than any follower's report made before the HEAD was first read, the lagging consumer's
-    cursor among them; the HEADs are replayed into the oracle and every replica is compared byte for byte."""
-    from apus_b200 import engine as E
-    n = 4
-    stream, _ = _lap_case(kind, L)
-    requests = [(O.CONFIG, 0, 0, b"")] + stream
-    reps = consumer_group(eng, n, L, leader_flags=E.F_AUTOPRUNE, ring_slots=1 << 14, ring_bytes=1 << 17, ctas=ctas,
-                          follower_flags=[E.F_HOST_APPLY, E.F_DEVICE_APPLY, E.F_DEVICE_APPLY])
-    rec = AR.Recorder(reps[1], 1, L)
-    rp = AR.Replay(orc, n, L)
-    try:
-        lens = [len(p) for *_, p in stream]
-        cons = [PackedConsumer(r, lens, max_n_cap=256, cap_max=1 << 20, seed=90 + k) for k, r in enumerate(reps[2:])]
-        errs, total = [], {}
-
-        def run(cn, lag, seed):
-            rng = np.random.default_rng(seed)
-            try:
-                drain(cn, lambda st: "t" in total and st.next_idx > total["t"] + total["heads"](),
-                      [1, 2, 3] if lag else [16, 256], rng, pause=0.002 if lag else 0.0)
-            except Exception as e:        # noqa: BLE001 - reported below
-                errs.append(e)
-        total["heads"] = lambda: reps[0].stats()["auto_heads"]
-        th = [threading.Thread(target=run, args=(cn, k == len(cons) - 1, 90 + k)) for k, cn in enumerate(cons)]
-        rec.start()
-        for x in th:
-            x.start()
-        EU.launch_each(eng, reps, FOREVER)
-        lead = reps[0]
-        lead.submit(O.CONFIG, 0, 0, O.cid_image(n))
-        t = _submit_all(lead, stream)
-        deadline = time.time() + 300
-        while lead.committed() < t:
-            rec.check()
-            assert not errs, errs
-            assert time.time() < deadline, f"committed {lead.committed()} of {t}; leader {lead.offsets()}"
-            time.sleep(0.005)
-        total["t"] = t
-        final = lead.offsets()["end"]
-        rec.finish(final)
-        for x in th:
-            x.join(300)
-            assert not x.is_alive()
-        assert not errs, errs
-        wait_forwarded(reps)
-        EU.stop_each(eng, reps)
-
-        pieces, flat, src, gaps = AR.recording_pieces([rec.rec], L)
-        assert gaps[1] is None, gaps
-        hits = []
-        on_head = heads_against_reports(L, rec.rec.segs, {1: rec.rec.reports, 2: cons[0].reports, 3: cons[1].reports},
-                                        3, hits)
-        for c0, lc in pieces:
-            rp.launch(lc, requests, replica=src, on_head=on_head)
-            for s, b, _ in rec.rec.segs:
-                if s + len(b) == c0 + len(lc.buf):
-                    AR.compare_read(rp, 1, s, b, flat)
-        assert rp.pos == len(requests)
-        assert rp.written >= 6 * L, rp.written / L
-        assert hits, "no HEAD carried the lagging consumer's cursor: the test never gated the pruning rule"
-        for cn in cons:
-            assert cn.at == rp.written
-        for i, r in enumerate(reps):
-            eo, oo = r.offsets(), rp.c.offsets(i)
-            for key in ("end", "commit", "head"):
-                assert eo[key] == oo[key], (i, key, eo, oo)
-            assert eo["apply"] == (oo["apply"] if i == 0 else final), (i, eo)
-            ei, oi = r.image(), rp.c.image(i)
-            d = np.nonzero(ei != oi)[0]
-            assert len(d) == 0, f"replica {i}: {len(d)} bytes differ, first at {int(d[0])}"
-        st = lead.stats()
-        assert st["auto_heads"] == len(rp.heads) >= int(rp.written / L), (st["auto_heads"], len(rp.heads))
-        for cn in cons:
-            check_rows(cn.rows, stream, first_idx=2)
-            assert cn.rep.consume_status().next_idx == t + st["auto_heads"] + 1
-        print(f"{rp.written / L:.2f} laps, {len(rp.heads)} HEAD entries replayed, {len(hits)} carried the lagging "
-              f"consumer's cursor, {cons[1].calls} calls of the lagging consumer")
-    finally:
-        rec.stop.set()
-        close_all(eng, reps)
-        rp.close()
 
 
 def test_jagged_round_trip(eng):
