@@ -119,6 +119,14 @@ __device__ __forceinline__ uint64_t ld_relaxed_sys_u64_any(const uint8_t *entrie
 // scope is .sys, not .gpu, so that the chain stays at the scope it started at (the writes came from a peer GPU); it
 // costs one store per commit advance.  Reader: the consume work's first kernel on the same GPU, with ld.acquire.sys;
 // the kernels that read the entries run after it in stream order.
+// On a leader (APUS_F_APPLY_ANY_ROLE) the writer is the commit warp's lane 0, once per commit advance, and every write
+// the record covers was made on the leader's own GPU: the entry bytes and index words by its worker CTAs, each tile's
+// behind a fence in the lane that stores its publish record's PR_END pair (t6_publish after its CTA barrier, the
+// express path after a __syncwarp), so that pair is a release of the tile's stores.  The commit warp finds records with
+// relaxed loads in several lanes, so before the record lane 0 re-reads the PR_END pair of EVERY record the advance
+// commits with ld.acquire.gpu: each read synchronises with its own writer's fence, whatever order the workers took
+// their turns in.  Then it stores the record with st.release.gpu (cons_publish_gpu), cumulative over all of them.  GPU
+// scope is enough, since the writers, the bytes and the consume kernels are all on this GPU.
 // ---------------------------------------------------------------------------------
 static_assert(offsetof(apus_ctrl_t, cons_rec) == 896 && sizeof(apus_ctrl_t) == APUS_CTL_OFF,
               "the consumer words use the spare line after turn_ns and end where the control-plane words start");
@@ -127,6 +135,11 @@ static_assert(offsetof(apus_ctrl_t, cons_rec) % 16 == 0 && offsetof(apus_ctrl_t,
 __device__ __forceinline__ void cons_publish(apus_ctrl_t *ctrl, uint64_t held_off, uint64_t held_entries)
 {
     asm volatile("st.release.sys.global.v2.u64 [%0], {%1,%2};" ::"l"(ctrl->cons_rec), "l"(held_off), "l"(held_entries)
+                 : "memory");
+}
+__device__ __forceinline__ void cons_publish_gpu(apus_ctrl_t *ctrl, uint64_t held_off, uint64_t held_entries)
+{
+    asm volatile("st.release.gpu.global.v2.u64 [%0], {%1,%2};" ::"l"(ctrl->cons_rec), "l"(held_off), "l"(held_entries)
                  : "memory");
 }
 __device__ __forceinline__ void cons_read(const apus_ctrl_t *ctrl, uint64_t &held_off, uint64_t &held_entries)

@@ -273,7 +273,7 @@ static int replica_init(apus_replica *r, const apus_config_t *cfg, uint64_t log_
     if (r->cfg.flags & APUS_F_DEVICE_APPLY) {
         /* the consumers start at offset 0 with idx 1, where the first entry goes; nothing is committed yet */
         c.cons_cur[1] = 1;
-        c.cons_on = 1;
+        c.cons_on = (r->cfg.flags & APUS_F_APPLY_ANY_ROLE) ? 2 : 1;    /* what a leader adjusting this replica looks at */
         pthread_mutex_init(&r->cons_mu, NULL);
         CK(cudaStreamCreateWithFlags(&r->cons_stream, cudaStreamNonBlocking));
         for (cudaEvent_t &e : r->ev_cons) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
@@ -331,7 +331,9 @@ extern "C" int apus_replica_create(const apus_config_t *cfg, apus_replica_t **ou
     uint32_t bytes = cfg->ring_bytes ? cfg->ring_bytes : (16u << 20);
     if ((cfg->flags & APUS_F_DEVICE_APPLY) && (cfg->flags & APUS_F_HOST_APPLY))
         return fail("APUS_F_DEVICE_APPLY and APUS_F_HOST_APPLY exclude each other: one consumer reports the apply offset");
-    if ((cfg->flags & APUS_F_DEVICE_APPLY) && cfg->server_idx == cfg->leader_idx)
+    if ((cfg->flags & APUS_F_APPLY_ANY_ROLE) && !(cfg->flags & APUS_F_DEVICE_APPLY))
+        return fail("APUS_F_APPLY_ANY_ROLE needs APUS_F_DEVICE_APPLY: it lets the device consumers work in every role");
+    if ((cfg->flags & APUS_F_DEVICE_APPLY) && !(cfg->flags & APUS_F_APPLY_ANY_ROLE) && cfg->server_idx == cfg->leader_idx)
         return fail("APUS_F_DEVICE_APPLY is for followers");
     if (slots & (slots - 1)) return fail("ring_slots must be a power of two");
     if (bytes % 4096 || bytes < (1u << 17)) return fail("ring_bytes must be a multiple of 4096, >= 128 KiB");
@@ -1241,7 +1243,8 @@ extern "C" int apus_consume_device(apus_replica_t *r, uint32_t max_n, uint64_t *
                                    size_t stride, uint32_t *count, void *stream)
 {
     if (!r) return fail("null argument");
-    if (is_leader(r)) return fail("apus_consume_device: consumption is a follower's (the leader's log is its own)");
+    if (is_leader(r) && !(r->cfg.flags & APUS_F_APPLY_ANY_ROLE))
+        return fail("apus_consume_device: consumption is a follower's (the leader's log is its own)");
     if (!(r->cfg.flags & APUS_F_DEVICE_APPLY)) return fail("apus_consume_device needs a replica created with APUS_F_DEVICE_APPLY");
     if (max_n == 0) return fail("apus_consume_device: max_n is 0");
     if (!idx || !types || !connection_ids || !req_ids || !lens || !count || (!payloads && stride)) return fail("null argument");
@@ -1261,7 +1264,8 @@ extern "C" int apus_consume_device_packed(apus_replica_t *r, uint32_t max_n, uin
                                           uint64_t values_cap, uint32_t *count, void *stream)
 {
     if (!r) return fail("null argument");
-    if (is_leader(r)) return fail("apus_consume_device_packed: consumption is a follower's (the leader's log is its own)");
+    if (is_leader(r) && !(r->cfg.flags & APUS_F_APPLY_ANY_ROLE))
+        return fail("apus_consume_device_packed: consumption is a follower's (the leader's log is its own)");
     if (!(r->cfg.flags & APUS_F_DEVICE_APPLY))
         return fail("apus_consume_device_packed needs a replica created with APUS_F_DEVICE_APPLY");
     if (max_n == 0) return fail("apus_consume_device_packed: max_n is 0");
@@ -1566,6 +1570,9 @@ extern "C" int apus_ctl_last_entry(apus_replica_t *r, uint64_t *idx, uint64_t *t
     return APUS_OK;
 }
 
+/* bytes from log offset `from` forward to `to` on a ring of L bytes */
+static inline uint64_t ring_dist_h(uint64_t from, uint64_t to, uint64_t L) { return to >= from ? to - from : L - (from - to); }
+
 static int copy_to_peer(apus_replica *r, uint8_t peer, size_t off, size_t len)
 {
     if (!len) return APUS_OK;
@@ -1584,7 +1591,7 @@ extern "C" int apus_ctl_adjust_follower(apus_replica_t *r, uint8_t peer, uint64_
     apus_loghdr_t mh, fh; apus_ctrl_t mc, fc;
     if (own_read(r, APUS_HDR_OFF, &mh, sizeof mh) != APUS_OK || own_read(r, 0, &mc, sizeof mc) != APUS_OK) return APUS_ERROR;
     if (peer_read(r, peer, APUS_HDR_OFF, &fh, sizeof fh) != APUS_OK || peer_read(r, peer, 0, &fc, sizeof fc) != APUS_OK) return APUS_ERROR;
-    if (fc.cons_on) return fail("peer %u consumes on the device (APUS_F_DEVICE_APPLY): no log adjustment", (unsigned)peer);
+    if (fc.cons_on == 1) return fail("peer %u consumes on the device (APUS_F_DEVICE_APPLY): no log adjustment", (unsigned)peer);
     const uint64_t mine = mc.published, theirs = fc.acked;      /* idx of the last entry each of us holds */
     /* last entry we share: walk down from min(mine, theirs) comparing {offset, idx, term} (the leader's log is the
      * truth, log_find_remote_end_offset, dare_log.h:362-394).  Entries up to the follower's commit are shared by
@@ -1599,6 +1606,42 @@ extern "C" int apus_ctl_adjust_follower(apus_replica_t *r, uint8_t peer, uint64_
         j--;
     }
     if (!found) { j = 0; keep_end = 0; }
+    /* a peer whose device consumers run in any role (cons_on == 2): nothing they have read, or may read on their
+     * current record, is rewritten -- checked before anything is written */
+    uint64_t rec[2] = { fc.cons_rec[0], fc.cons_rec[1] };
+    bool rewrite_rec = false;
+    if (fc.cons_on) {
+        const uint64_t cur = fc.cons_cur[0], nidx = fc.cons_cur[1];
+        if (j > 0) {
+            if (nidx - 1 > j || ring_dist_h(cur, rec[0], L) > ring_dist_h(cur, keep_end, L))
+                return fail("peer %u: its device consumers have read, or may read, past the last entry it shares with me "
+                            "(idx %llu, next idx %llu): no log adjustment", (unsigned)peer, (unsigned long long)j,
+                            (unsigned long long)nidx);
+            /* entries past what it holds after the resend have stale index words: the record may not name them */
+            if (rec[1] > mine) { rec[1] = mine; rewrite_rec = true; }
+        } else {
+            /* it shares nothing with me: its consumers can go on only from my head (joining a device consumer needs a
+             * snapshot of its device state) */
+            uint64_t hidx = 0;
+            if (mh.end == L || mh.head == mh.end) hidx = mine + 1;
+            else {
+                uint8_t eh[8];
+                uint64_t o, i2, t2; uint32_t s2;
+                if (own_read(r, r->entries_off + mh.head + E_IDX, eh, 8) != APUS_OK) return APUS_ERROR;
+                memcpy(&hidx, eh, 8);
+                if (hidx == 0 || hidx > mine || entry_at(r, -1, hidx, &o, &i2, &t2, &s2) != APUS_OK || o != mh.head || i2 != hidx)
+                    hidx = 0;                                                     /* no entry of mine starts at my head */
+            }
+            if (cur != mh.head || nidx != hidx)
+                return fail("peer %u shares no entry with me and its device consumers stand at offset %llu, next idx %llu, "
+                            "not at my head (offset %llu, idx %llu): no log adjustment", (unsigned)peer,
+                            (unsigned long long)cur, (unsigned long long)nidx, (unsigned long long)mh.head,
+                            (unsigned long long)hidx);
+            rec[0] = cur; rec[1] = nidx - 1; rewrite_rec = true;                /* nothing of its old log */
+        }
+    }
+    /* the record first, so that no consume call that runs during the resend trusts the old one (one 16 B copy) */
+    if (rewrite_rec && peer_write(r, peer, offsetof(apus_ctrl_t, cons_rec), rec, 16) != APUS_OK) return APUS_ERROR;
     uint64_t bytes = 0;
     if (mine > j && mh.end != L) {
         /* everything behind the shared prefix: entry bytes [keep_end, my end) -- a wrapped range is two copies, a wrap
@@ -1667,7 +1710,8 @@ extern "C" int apus_replica_disconnect(apus_replica_t *r, uint8_t peer_idx)
 extern "C" int apus_replica_set_role(apus_replica_t *r, uint8_t leader_idx, uint64_t term)
 {
     if (!r || leader_idx >= r->cfg.group_size) return fail("bad argument");
-    if (r->cfg.flags & APUS_F_DEVICE_APPLY) return fail("a replica with device consumers (APUS_F_DEVICE_APPLY) keeps its role");
+    if ((r->cfg.flags & APUS_F_DEVICE_APPLY) && !(r->cfg.flags & APUS_F_APPLY_ANY_ROLE))
+        return fail("a replica with device consumers (APUS_F_DEVICE_APPLY) keeps its role");
     if (r->in_flight) return fail("stop the kernel first");
     DeviceGuard g(r->cfg.device);
     const bool was_leader = is_leader(r);
@@ -1730,6 +1774,17 @@ extern "C" int apus_replica_set_role(apus_replica_t *r, uint8_t leader_idx, uint
     for (int i = 0; i < 16; i++) { c.ack[i] = 0; c.apply_off[i] = h.head; c.fbeat[i] = 0; }   /* dare_server.c:1507-1510 */
     h.tail = tail; h.old_end = h.end;
     if (own_write(r, 0, &c, offsetof(apus_ctrl_t, fin_entries)) != APUS_OK) return APUS_ERROR;
+    if (r->cfg.flags & APUS_F_APPLY_ANY_ROLE) {
+        /* my device consumers go on as a leader's: the record names what I now know committed -- the adopted commit
+         * and the entries before it -- and my apply offset is their cursor (the commit warp keeps it so).  The consume
+         * work enqueued so far runs to its end first, so that none of it sees the record change under it, and none
+         * is enqueued meanwhile */
+        StageLock cl(&r->cons_mu);
+        CK(cudaStreamSynchronize(r->cons_stream));
+        const uint64_t rec[2] = { h.commit, last - unc };
+        if (own_read(r, offsetof(apus_ctrl_t, cons_cur), &h.apply, 8) != APUS_OK) return APUS_ERROR;
+        if (own_write(r, offsetof(apus_ctrl_t, cons_rec), rec, 16) != APUS_OK) return APUS_ERROR;
+    }
     if (own_write(r, APUS_HDR_OFF, &h, sizeof h) != APUS_OK) return APUS_ERROR;
     return APUS_OK;
 }

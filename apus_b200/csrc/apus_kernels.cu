@@ -891,6 +891,12 @@ __device__ __noinline__ int leader_express(const apus_devctx_t *__restrict__ cx,
     const uint64_t t_turn = xprof ? globaltimer_ns() : 0;
     const uint64_t cumt = term_word(cum, cx->term);
     const bool cert = caught && !(cx->flags & APUS_FLAG_NO_EXPRESS);
+    if (cx->flags & APUS_FLAG_APPLY_ANY_ROLE) {
+        // my own consumers read this entry once the commit warp has acquired the record's PR_END pair (apus_dev.h):
+        // the warp's local entry and index stores go before that pair
+        __syncwarp();
+        if (lane == 16 + PR_END) asm volatile("fence.acq_rel.gpu;" ::: "memory");
+    }
     if (isf) {
         apus_ctrl_t *pc = reinterpret_cast<apus_ctrl_t *>(cx->peer[lane]);
         if (cert) {
@@ -1070,8 +1076,9 @@ __device__ __forceinline__ bool cw_walk(const apus_devctx_t *__restrict__ cx, Co
 }
 
 // commit stores: {commit offset, term} into every follower (dare_ibv_rc.c:1810), {commit offset, tickets} to the host,
-// and the leader's bookkeeping, in publish order (single writer)
-__device__ __forceinline__ void cw_commit(const apus_devctx_t *__restrict__ cx, CommitWarp &C, const PubRec &r, int lane)
+// and the leader's bookkeeping, in publish order (single writer).  Records [t0, C.tail) are the ones this advance commits.
+__device__ __forceinline__ void cw_commit(const apus_devctx_t *__restrict__ cx, CommitWarp &C, const PubRec &r, int lane,
+                                          uint64_t t0)
 {
     apus_ctrl_t *ctrl = C.ctrl;
     apus_loghdr_t *hdr = C.hdr;
@@ -1083,9 +1090,18 @@ __device__ __forceinline__ void cw_commit(const apus_devctx_t *__restrict__ cx, 
         st_relaxed_sys_2x64(&C.hw->commit_off, off, tickets);
         st_relaxed_sys(&C.hw->consumed, tickets);                 // submission-ring space
         st_relaxed_sys(&C.hw->last_commit_ns, globaltimer_ns());
+        if (cx->flags & APUS_FLAG_APPLY_ANY_ROLE) {
+            // my own device consumers: acquire the PR_END pair of every record this advance commits (each stored
+            // behind its own writer's fence), then release the consumer record over them (apus_dev.h).  Before
+            // pub_tail: none of the records is reused meanwhile
+            uint64_t st_, end_;
+            for (uint64_t h = t0; h != C.tail; h++) ld_acquire_gpu_2x64(&C.ring[h & PUBMASK].w[2 * PR_END], st_, end_);
+            cons_publish_gpu(ctrl, off, C.committed);
+        }
         st_relaxed_sys(&C.seq->pub_tail, C.tail);                 // publish-ring space
         hdr->commit = off;
-        st_relaxed_sys(&hdr->apply, off);                       // leader applies = update_state
+        // leader applies = update_state; with device consumers my apply offset is their cursor (cw_forward_apply)
+        if (!(cx->flags & APUS_FLAG_APPLY_ANY_ROLE)) st_relaxed_sys(&hdr->apply, off);
         hdr->end = off; hdr->tail = r.tail; hdr->old_end = off;
         ctrl->committed = C.committed; ctrl->committed_tickets = tickets; ctrl->lat_count = C.lat_count;
         ctrl->published = C.committed; ctrl->consumed = tickets; ctrl->next_idx = r.next_idx; ctrl->hwm = r.hwm;
@@ -1107,6 +1123,15 @@ __device__ __forceinline__ void cw_heartbeat(const apus_devctx_t *__restrict__ c
             if (C.peer) st_relaxed_sys(&C.peer->hb, term_word(C.hb_beat, cx->term));
         }
     }
+}
+
+// APUS_F_APPLY_ANY_ROLE, lane 0, every 64th pass (C.spins counts them in cw_exit) and on the way out: my device
+// consumers' cursor becomes my apply offset, the one ld_apply gives the pruning rule for me -- what f_housekeeping
+// forwards on a follower
+__device__ __forceinline__ void cw_forward_apply(const apus_devctx_t *__restrict__ cx, const CommitWarp &C, int lane, bool last)
+{
+    if ((cx->flags & APUS_FLAG_APPLY_ANY_ROLE) && lane == 0 && (last || (C.spins & 0x3fu) == 0))
+        st_relaxed_sys(&C.hdr->apply, ld_relaxed_sys(&C.ctrl->cons_cur[0]));
 }
 
 // exit decision: 1 every worker finished and nothing is in flight, 2 abort (or the watchdog), 0 go on
@@ -1154,10 +1179,12 @@ __device__ void leader_commit_warp(const apus_devctx_t *__restrict__ cx)
         const uint64_t Q = cw_quorum(C, lane);
         if (Q > C.committed && C.tail != C.seen) {
             PubRec r;
-            if (cw_walk(cx, C, Q, rv, nvalid, lane, r)) cw_commit(cx, C, r, lane);
+            const uint64_t t0 = C.tail;
+            if (cw_walk(cx, C, Q, rv, nvalid, lane, r)) cw_commit(cx, C, r, lane, t0);
         }
         cw_heartbeat(cx, C, lane);
         const int ex = cw_exit(cx, C, nvalid != 0, lane);
+        cw_forward_apply(cx, C, lane, ex != 0);
         if (ex) {
             if (ex == 1 && cx->target != ~0ull && C.peer) fin_publish(C.peer, C.committed, cx->target);
             break;
@@ -1639,8 +1666,10 @@ __device__ __forceinline__ void t6_publish(const apus_devctx_t *__restrict__ cx,
     const bool pubs = lane < N && lane != me && cx->peer[lane];
     // data before tail (invariant I1): all data stores of the tile -> bar.sync (before this phase) -> one system
     // fence per publishing lane (cumulative over the barrier) -> the tail.  A system fence costs microseconds;
-    // fencing in every warp serializes 15 of them.
-    if (pubs) __threadfence_system();
+    // fencing in every warp serializes 15 of them.  With device consumers on this leader (APUS_F_APPLY_ANY_ROLE) the
+    // lane that stores the record's PR_END pair fences too, in the same instruction: the commit warp acquires that pair
+    // before it publishes the consumer record (apus_dev.h).
+    if (pubs || ((cx->flags & APUS_FLAG_APPLY_ANY_ROLE) && lane == 16 + PR_END)) __threadfence_system();
     // the publish turn: {slot number, record number} in one 16 B word.  Held for the N-1 tail stores
     // and the eight 16 B stores of the publish record -- no fence inside the turn
     if (lane == 0) {

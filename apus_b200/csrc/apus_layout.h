@@ -123,7 +123,8 @@ typedef struct apus_ctrl {
                                     release store per commit advance (cons_publish / cons_read) */
     uint64_t cons_cur[2];        /* consume work -> follower kernel: {cursor offset, idx of the next entry}; the cursor is
                                     the apply offset the follower reports to the leader's pruning rule */
-    uint64_t cons_on;            /* 1: this replica was created with APUS_F_DEVICE_APPLY (the control plane refuses it) */
+    uint64_t cons_on;            /* 1: this replica was created with APUS_F_DEVICE_APPLY (the control plane refuses it);
+                                    2: ... with APUS_F_APPLY_ANY_ROLE too (log adjustment guards its consumers) */
     uint64_t pad4[11];
 } apus_ctrl_t;
 
@@ -264,6 +265,8 @@ typedef struct apus_hostwords {
                                        lengthen the path: kept out of measured runs) */
 
 #define APUS_FLAG_DEVICE_APPLY 0x200u /* follower: the apply offset it reports is the device consumers' cursor */
+#define APUS_FLAG_APPLY_ANY_ROLE 0x400u /* with DEVICE_APPLY, on a leader: the commit warp publishes the consumer record,
+                                           and the consumers' cursor is the leader's apply offset */
 
 #define APUS_PUB_CERT      (1ull << 63)         /* pub_end: this publish is self-certifying (no writer fence) */
 #define APUS_PUB_TERM_SHIFT 48                   /* pub_cum / hb: term in the top 16 bits */

@@ -20,6 +20,7 @@ MAX_SERVERS = 13
 F_FENCED_ACK, F_DEVICE_STATS, F_AUTOPRUNE, F_FOLLOWER_WALK, F_EXPLICIT = 0x1, 0x2, 0x4, 0x8, 0x80000000
 F_HOST_APPLY, F_NO_EXPRESS, F_PROFILE, F_FABRIC = 0x10, 0x20, 0x40, 0x100
 F_DEVICE_APPLY = 0x200
+F_APPLY_ANY_ROLE = 0x400   # with F_DEVICE_APPLY: the device consumers work on a leader too, and through a take-over
 CONSUME_BAD_IDX = 1
 UINT64_MAX = (1 << 64) - 1
 
@@ -323,8 +324,10 @@ class Replica:
         return int(rej.value), int(first.value)
 
     def consume_device(self, max_n, stride, out=None, stream=None):
-        """Follower created with F_DEVICE_APPLY: the next committed entries, at most max_n of them, into CUDA tensors
-        on this replica's device, in `stream` order (apus_consume_device).  Returns (idx int64 [max_n], types uint8
+        """Follower created with F_DEVICE_APPLY, or any replica created with F_DEVICE_APPLY | F_APPLY_ANY_ROLE: the next
+        committed entries, at most max_n of them, into CUDA tensors on this replica's device, in `stream` order
+        (apus_consume_device).  On a leader they are every committed entry of its log, its own tickets and the entries
+        of earlier terms alike: every replica applies the same rows in the same order.  Returns (idx int64 [max_n], types uint8
         [max_n], conns int16 [max_n], req_ids int64 [max_n], lens int16 [max_n], payloads uint8 [max_n, stride],
         count int32 [1]): rows 0 .. count-1 are the CSM-like entries examined; NOOP / CONFIG / HEAD entries are
         skipped, idx shows them.  Read count after synchronising with `stream`.  `out`: those seven tensors to
@@ -363,7 +366,7 @@ class Replica:
         return out
 
     def consume_device_packed(self, max_n, values_cap, out=None, stream=None):
-        """consume_device with packed output (apus_consume_device_packed).  Returns (idx int64 [max_n], types uint8
+        """consume_device with packed output (apus_consume_device_packed), in the same roles.  Returns (idx int64 [max_n], types uint8
         [max_n], conns int16 [max_n], req_ids int64 [max_n], offsets int64 [max_n+1], values uint8 [values_cap], count
         int32 [1]): row r's cmd is values[offsets[r]:offsets[r+1]], offsets[0] = 0, for the count rows written.  The
         call stops before the first cmd that would end past values_cap; when that is the first row, consume_status()

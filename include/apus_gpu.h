@@ -84,7 +84,16 @@ extern "C" {
 #define APUS_F_PROFILE      0x40u /* fine-grained device timestamps in the latency path (diagnostic runs only: each is a %globaltimer read) */
 #define APUS_F_DEVICE_APPLY 0x200u /* follower: the apply offset reported to the leader's pruning rule is the cursor of
                                      the device consumers (apus_consume_device), the device counterpart of
-                                     APUS_F_HOST_APPLY.  Refused together with APUS_F_HOST_APPLY and on a leader */
+                                     APUS_F_HOST_APPLY.  Refused together with APUS_F_HOST_APPLY and on a leader
+                                     (unless APUS_F_APPLY_ANY_ROLE is set too) */
+#define APUS_F_APPLY_ANY_ROLE 0x400u /* with APUS_F_DEVICE_APPLY (refused without it): the device consumers work in
+                                     every role, so that a group that applies in GPU memory keeps its failover.  On a
+                                     leader they deliver every committed entry of its log, its own tickets included --
+                                     every replica applies the same rows in the same order -- and their cursor is the
+                                     leader's own apply offset in the pruning rule (a slow consumer holds the leader
+                                     back instead of being overwritten).  apus_replica_set_role changes such a
+                                     replica's role in both directions, and apus_ctl_adjust_follower adjusts it as long
+                                     as nothing its consumers have read is rewritten */
 #define APUS_F_EXPLICIT     0x80000000u /* flags are exactly as given (no defaults OR-ed in) */
 
 typedef struct apus_replica apus_replica_t;
@@ -280,8 +289,9 @@ int  apus_set_applied(apus_replica_t *r, uint64_t offset);
 /* copy the committed-and-held range [from, to) of the circular log (it may wrap) into dst (capacity cap);
  * *got = bytes copied.  One or two device->host copies through a pinned buffer. */
 int  apus_log_read_range(apus_replica_t *r, uint64_t from, uint64_t to, void *dst, uint64_t cap, uint64_t *got);
-/* Follower, APUS_F_DEVICE_APPLY: deliver committed entries straight into device memory, in stream order.  The arrays
- * are device memory on the follower's GPU, element types as apus_submit_device's plus idx; row k's cmd goes to
+/* Follower, APUS_F_DEVICE_APPLY (any role with APUS_F_APPLY_ANY_ROLE): deliver committed entries straight into device
+ * memory, in stream order.  The arrays are device memory on the replica's GPU, element types as apus_submit_device's
+ * plus idx; row k's cmd goes to
  * payloads + k*stride (payloads may be NULL when stride is 0).  `stream` is a cudaStream_t (NULL = the legacy default
  * stream).  Returns once the work is enqueued, without synchronising the host:
  *   - the work runs after everything enqueued on `stream` before the call, and `stream` waits for it; every call on
@@ -294,9 +304,13 @@ int  apus_log_read_range(apus_replica_t *r, uint64_t from, uint64_t to, void *ds
  *     stride it needs: nothing is truncated or lost) and before an entry that does not carry the idx its index word
  *     promises (APUS_CONSUME_BAD_IDX, sticky: nothing more is delivered);
  *   - the cursor moves past every examined entry only after every read of their bytes has completed: the leader may
- *     prune, then overwrite, everything behind it (the follower's kernel reports it on its idle passes).
+ *     prune, then overwrite, everything behind it (the follower's kernel reports it on its idle passes; a leader's
+ *     commit warp takes it as its own apply offset on its idle passes);
+ *   - on a leader (APUS_F_APPLY_ANY_ROLE) the rows are every committed entry of its log, its own tickets and the
+ *     entries of earlier terms it took over alike: the same rows, in the same order, as every follower's.
  * It never waits for commits: it delivers what is committed when it runs, which may be nothing.  APUS_ERROR on a
- * leader, on a replica without APUS_F_DEVICE_APPLY, for a null array, for an array not aligned to its element size
+ * leader without APUS_F_APPLY_ANY_ROLE, on a replica without APUS_F_DEVICE_APPLY, for a null array, for an array not
+ * aligned to its element size
  * (idx and req_ids 8 B, count 4 B, connection_ids and lens 2 B; payloads may have any alignment), or for max_n == 0. */
 int  apus_consume_device(apus_replica_t *follower, uint32_t max_n, uint64_t *idx, uint8_t *types,
                          uint16_t *connection_ids, uint64_t *req_ids, uint16_t *lens, void *payloads, size_t stride,
@@ -351,10 +365,16 @@ int  apus_ctl_heartbeat(apus_replica_t *r, uint64_t *word);
 int  apus_ctl_last_entry(apus_replica_t *r, uint64_t *idx, uint64_t *term, uint64_t *commit, uint64_t *end);
 /* elected leader, kernels stopped: bring follower `peer_idx` to my log -- find the last entry we share from its
  * commit offset on (log_find_remote_end_offset, dare_log.h:362-394), copy everything behind it (entry bytes and
- * offset index) peer to peer, and tell it to follow `sid` from there.  *resent = bytes copied. */
+ * offset index) peer to peer, and tell it to follow `sid` from there.  *resent = bytes copied.  A peer whose device
+ * consumers run in any role (APUS_F_APPLY_ANY_ROLE) is refused, with nothing written, when its consumers have read
+ * past the last entry it shares with me, or when it shares nothing with me and its consumers do not stand exactly at
+ * my head; its consumer record is left naming no entry beyond what its offset index holds after the resend. */
 int  apus_ctl_adjust_follower(apus_replica_t *leader, uint8_t peer_idx, uint64_t sid, uint64_t *resent);
 /* role and term for the next launch.  Becoming leader takes over the log as this replica holds it (entry counters,
- * tail, submission ring); becoming follower adopts what the new leader's adjustment left (apus_ctl_view.adj_*). */
+ * tail, submission ring); becoming follower adopts what the new leader's adjustment left (apus_ctl_view.adj_*).  With
+ * APUS_F_APPLY_ANY_ROLE a new leader's device consumers go on from their cursor: the consume work enqueued before the
+ * call runs first, then they may read up to the commit offset the leader adopted (the entries of earlier terms
+ * committed with it). */
 int  apus_replica_set_role(apus_replica_t *r, uint8_t leader_idx, uint64_t term);
 /* leader: liveness counters of the followers (their kernels bump them while polling); a counter that stands still
  * is a follower that is gone (HB replies, dare_ibv_rc.c:912-958 -> fail_count -> check_failure_count) */

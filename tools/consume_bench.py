@@ -14,6 +14,15 @@ the launch), and for `device` the entries/s and GB/s per follower from the event
 shapes: the 64 B header and the cmd read, the row written); the card's name and power limit read in the same run.
 
   python tools/consume_bench.py [--steps 3] [--warmup 1] [--out FILE]
+
+--leg any_role: what APUS_F_APPLY_ANY_ROLE costs the latency path.  Two groups of five replicas on GPU 0, device
+consumers on every follower; the leader of one is created with APUS_F_DEVICE_APPLY | APUS_F_APPLY_ANY_ROLE (the express
+path's fence before its publish record, the commit warp's acquire and consumer record), the other's without.  Each
+round resident-launches one group, runs apus_closed_loop (one 64 B request in flight: the express path), stops it; the
+groups alternate.  Prints per group the host-clock p50 / p99 of the closed loop and the device-clock commit latency
+(APUS_F_DEVICE_STATS samples), and checks afterwards that the flagged leader's own consumer delivers every request.
+
+  python tools/consume_bench.py --leg any_role [--steps 5] [--warmup 1] [--out FILE]
 """
 import argparse
 import json
@@ -27,6 +36,10 @@ import time
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+
+if any("any_role" in a for a in sys.argv[1:]):
+    # two groups' streams beside resident launches (the default consume leg keeps the default 8 queues it was measured with)
+    os.environ.setdefault("CUDA_DEVICE_MAX_CONNECTIONS", "32")
 
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
@@ -168,14 +181,92 @@ def run_step(way, reps, req, seed):
     return t, lead.last_launch_ms(), counts, times
 
 
+LOOP_N = 20000        # closed-loop requests per round (--leg any_role)
+
+
+def any_role_group(flagged):
+    ff = E.F_DEVICE_STATS | E.F_DEVICE_APPLY | (E.F_APPLY_ANY_ROLE if flagged else 0)
+    reps = [E.Replica(0, i, REPLICAS, 0, 1, A.LOG_SIZE, E.RING_HOST_MAPPED, 0, 0,
+                      ff if (i != 0 or flagged) else E.F_DEVICE_STATS, 0) for i in range(REPLICAS)]
+    blobs = [r.export() for r in reps]
+    for r in reps:
+        for j, b in enumerate(blobs):
+            if j != r.idx:
+                r.connect(j, b)
+    return reps
+
+
+def any_role_leg(args):
+    lines = [json.dumps({"leg": "any_role", "card": card(), "torch": torch.__version__, "replicas": REPLICAS,
+                         "requests_per_round": LOOP_N, "payload": PAYLOAD})]
+    print(lines[0], flush=True)
+    groups = {w: any_role_group(w == "any_role") for w in ("plain", "any_role")}
+    res = {w: {"host_ns": [], "dev_ns": []} for w in groups}
+    rid = {w: 1 for w in groups}
+    for w, reps in groups.items():
+        reps[0].submit(E.CONFIG, 0, 0, E.cid_image(REPLICAS))
+    for s in range(args.warmup + args.steps):
+        for w in ("plain", "any_role"):                           # alternating
+            reps = groups[w]
+            arr = (E.C.c_void_p * REPLICAS)(*[r.h for r in reps])
+            E._ck(E.lib().apus_replicas_launch(arr, REPLICAS, E.UINT64_MAX), "apus_replicas_launch")
+            n0 = reps[0].stats()["lat_samples"]
+            lat = reps[0].closed_loop(LOOP_N, PAYLOAD, 7, rid[w])
+            rid[w] += LOOP_N
+            dev = reps[0].latency_ns(LOOP_N)
+            E._ck(E.lib().apus_replicas_stop(arr, REPLICAS), "apus_replicas_stop")
+            for r in reps:
+                r.wait(60_000)
+            got = reps[0].stats()["lat_samples"] - n0
+            print(f"[{w}] round {s}: host p50 {np.percentile(lat, 50) / 1e3:.2f} us, device samples {got}",
+                  file=sys.stderr, flush=True)
+            if s >= args.warmup:
+                res[w]["host_ns"].extend(int(x) for x in lat)
+                res[w]["dev_ns"].extend(int(x) for x in dev[-min(got, LOOP_N):])
+    # the flagged leader's own consumer: every request it committed, in order
+    lead = groups["any_role"][0]
+    rows, out = 0, None
+    while True:
+        out = lead.consume_device(MAX_N, PAYLOAD, out=out)
+        torch.cuda.synchronize(0)
+        k = int(out[6].cpu()[0])
+        rows += k
+        if k == 0:
+            break
+    st = lead.consume_status()
+    assert st.error == 0 and rows == rid["any_role"] - 1, (rows, rid["any_role"] - 1, st)
+    for w in ("plain", "any_role"):
+        h, d = np.asarray(res[w]["host_ns"]), np.asarray(res[w]["dev_ns"])
+        lines.append(json.dumps({"group": w, "rounds": args.steps, "requests": int(len(h)),
+                                 "host_p50_us": float(np.percentile(h, 50)) / 1e3,
+                                 "host_p99_us": float(np.percentile(h, 99)) / 1e3,
+                                 "device_p50_us": float(np.percentile(d, 50)) / 1e3 if len(d) else None,
+                                 "device_p99_us": float(np.percentile(d, 99)) / 1e3 if len(d) else None,
+                                 "leader_rows_consumed": rows if w == "any_role" else None}))
+        print(lines[-1], flush=True)
+    for reps in groups.values():
+        for r in reps:
+            r.close()
+    return lines
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=3)
     ap.add_argument("--warmup", type=int, default=1)
     ap.add_argument("--out", default=None)
+    ap.add_argument("--leg", choices=["consume", "any_role"], default="consume")
     args = ap.parse_args()
     if not torch.cuda.is_available() or A.lib().apus_device_count() < 1:
         raise SystemExit("consume_bench.py: no CUDA device; the engine has no CPU fallback")
+    if args.leg == "any_role":
+        torch.zeros(1, device="cuda:0").clone()
+        torch.cuda.synchronize()
+        lines = any_role_leg(args)
+        if args.out:
+            with open(args.out, "w") as f:
+                f.write("\n".join(lines) + "\n")
+        return
     global WALK
     WALK = load_walk()
     torch.zeros(1, device="cuda:0").clone()
