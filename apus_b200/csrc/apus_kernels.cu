@@ -155,7 +155,7 @@ struct LeaderShared {
     uint64_t st_hwm;
     // current sub-tile
     uint32_t kbase, m, gap, ghost, fresh, auto_head, ext_bytes, last, blocked, hbytes;
-    uint32_t base_es, base_xb, fast, pad1;
+    uint32_t base_es, base_xb, fast, after_gap;   // after_gap: the last placement was a wrap gap (leader_place)
     uint64_t ext_base, auto_head_val, a, b, idx0, cum_after, new_end, tail_after, hwm_after;
     uint8_t  *peer_entries[APUS_MAX_SERVERS];
     uint32_t *peer_index[APUS_MAX_SERVERS];
@@ -468,8 +468,14 @@ __device__ __noinline__ void leader_place(const apus_devctx_t *__restrict__ cx, 
     uint64_t new_head = 0;
     // "never two HEAD entries in a row" (prev_log_entry_head, dare_server.c:2042) keeps an idle log from filling with HEAD
     // entries; a placement that is BLOCKED on space right behind a HEAD entry must still be able to prune again once the
-    // followers' applications have caught up -- else a slow follower host deadlocks the leader (back-pressure, rule E2)
-    if (autoprune && end != L && used >= (L >> 2) && (!S->st.prev_head || S->was_blocked) && L - pos0 >= APUS_HDR_BYTES) {
+    // followers' applications have caught up -- else a slow follower host deadlocks the leader (back-pressure, rule E2).
+    // Never right after a gap: the gap and the entry at 0 are one append of the reference (log_append_entry), and
+    // log_pruning saw the end before the gap, where this rule was already evaluated.  Here `used` would count the
+    // skipped stretch [old end, L) and could put a HEAD between the ghost and its entry.  That placement cannot block:
+    // the gap was taken only because the entry fits at 0.  A gap placement is never a tile's last (S->last stays 0),
+    // so its state never reaches the next claim's place_fast: the placement after it is always this CTA's leader_place.
+    if (autoprune && !S->after_gap && end != L && used >= (L >> 2) && (!S->st.prev_head || S->was_blocked) &&
+        L - pos0 >= APUS_HDR_BYTES) {
         uint64_t d = 0;                                   // distance apply -> end, per replica
         if (lane < N) {
             d = ring_dist(S->ap[lane], end, L);
@@ -543,6 +549,7 @@ __device__ __noinline__ void leader_place(const apus_devctx_t *__restrict__ cx, 
         if (S->blocked) S->was_blocked = 1;
         if (!S->blocked) {
             S->was_blocked = 0;
+            S->after_gap = S->gap;
             // commit the placement to the state this CTA carries
             if (autoh) st_relaxed_sys(&hdr->head, new_head);
             if (autoh) S->st.head = new_head;
@@ -1724,7 +1731,7 @@ __device__ void leader_main(const apus_devctx_t *__restrict__ cx, const uint32_t
         } else {
             while (ld_acquire_gpu(&seq->ready_epoch) != cx->epoch) { }
         }
-        S->finish = 0; S->abort = 0; S->was_blocked = 0; S->pub_tail_seen = 0; S->ap_valid = 0;
+        S->finish = 0; S->abort = 0; S->was_blocked = 0; S->after_gap = 0; S->pub_tail_seen = 0; S->ap_valid = 0;
         S->idx_base = ctrl->next_idx - 1 - ctrl->published;
         for (int i = 0; i < APUS_MAX_SERVERS; i++) {
             S->peer_entries[i] = (i < N && i != me && cx->peer[i]) ? cx->peer[i] + cx->entries_off : nullptr;

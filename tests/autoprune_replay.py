@@ -112,13 +112,21 @@ def placement_refusal(L, head, end, stride):
     return None
 
 
-def head_violation(L, head_old, end, v, boundaries, prev_was_head, next_stride=None):
+def head_violation(L, head_old, end, v, boundaries, prev_was_head, next_stride=None, at=None):
     """The engine's pruning rule (leader_place) as a predicate over one HEAD entry appended at `end` while the head was
     `head_old`: None when a HEAD carrying `v` is legal there, else the reason.  `boundaries`: the starts and ends of
     the entries of [head_old, end).  `prev_was_head`: the entry just before is a HEAD.  The leader appends a second
     HEAD right behind one only when its placement blocked on space there: `next_stride`, the stride of the next
     non-HEAD entry of the sequence (None: there is none), must then not be placeable at the head and end the first
-    HEAD left, which are `head_old` and `end`."""
+    HEAD left, which are `head_old` and `end`.  `at`: where the engine wrote the HEAD.  A HEAD is never placed
+    anywhere but at `end`: the rule is not evaluated between a wrapping entry's ghost (or skipped stretch) and the
+    entry, which the reference appends as one, nor where less than a header is left before len."""
+    pos0 = 0 if end == L else end
+    if at is not None and at != pos0:
+        return (f"HEAD between a wrapping entry's ghost/skip and the entry: HEAD at {at}, the end was {end} "
+                f"({L - pos0} bytes skipped)")
+    if L - pos0 < O.HDR:
+        return f"the HEAD's header does not fit at {end}: {L - pos0} bytes before len (the rule is not evaluated there)"
     used = 0 if end == L else dist(head_old, end, L)
     if used < L // 4:
         return f"ring used {used} < L/4 = {L // 4}"
@@ -196,7 +204,7 @@ class Replay:
             if e.typ == O.HEAD:
                 b = live_boundaries(oracle_view(c, lead), before["head"], before["end"], L)
                 nxt = request_stride(requests[self.pos]) if self.pos < len(requests) else None
-                why = head_violation(L, before["head"], before["end"], e.value, b, self.prev_head, nxt)
+                why = head_violation(L, before["head"], before["end"], e.value, b, self.prev_head, nxt, at=e.off)
                 assert why is None, f"{src}HEAD idx {e.idx} at {e.off}: {why}"
                 idx = c.prune_to(e.value)
                 self.pairs += self.prev_head

@@ -170,6 +170,27 @@ def test_head_violation_rules(head, end, v, prev, nxt, expect):
         assert why is not None and expect in why, why
 
 
+# A HEAD is appended at the end or nowhere: never at 0 behind a wrapping entry's ghost header (128 B left before the
+# ring's end) or behind the stretch skipped when even the header does not fit (32 B left).  Counting that stretch can
+# put the ring over a quarter used where the end alone does not.
+@pytest.mark.parametrize("head,end,v,at,expect", [
+    (640, 896, 768, 896, None),                                      # legal at the end (256 used)
+    (640, 896, 768, 0, "ghost/skip"),                                # the same HEAD behind the ghost
+    (704, 896, 832, 896, "L/4"),                                     # 192 used: not due at the end ...
+    (704, 896, 832, 0, "ghost/skip"),                                # ... named as such at 0, not as a used count
+    (704, 960, 832, 960, None),                                      # 256 used, exactly one header left
+    (704, 992, 832, 992, "does not fit"),                            # 288 used, but the header would cross len
+    (704, 992, 832, 0, "ghost/skip"),
+    (640, 0, 768, 0, None),                                          # end 0 after an exact fit (E1): 0 is the end
+])
+def test_head_between_a_wrap_and_its_entry(head, end, v, at, expect):
+    why = R.head_violation(L1K, head, end, v, _b(head, end), False, None, at=at)
+    if expect is None:
+        assert why is None, why
+    else:
+        assert why is not None and expect in why, why
+
+
 # ---- recordings of host-applying followers (replay_recordings), produced by the oracle alone -------------------------
 def recorded_run(orc, n, L, stream, seed, step):
     """The oracle standing in for a launch that laps the ring with host-applying followers: requests appended in
