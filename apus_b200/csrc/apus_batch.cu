@@ -5,6 +5,7 @@
  *   synth    apus_submit_synth: device-generated requests written into the HBM submission ring
  *   pack     apus_submit_device / apus_submit_device_packed: sizes, scan and pack passes, then the doorbell (bell)
  *   consume  apus_consume_device / apus_consume_device_packed: head, count, scan, copy and tail
+ *   wait     apus_consume_wait: one warp between consume calls, until enough entries are committed past the cursor
  *
  * apus_engine.cu checks the arguments, accounts ring space, and brackets each enqueue below in the caller's stream
  * order.  The batch layouts are apus_layout.h; the slot format is apus_slot.h; the device helpers shared with the
@@ -321,7 +322,7 @@ __global__ void apus_consume_head_kernel(apus_consume_args_t a)
     uint64_t committed, held;
     cons_read(ctrl, committed, held);
     const uint64_t cursor = ld_relaxed_sys(&ctrl->cons_cur[0]), nidx = ld_relaxed_sys(&ctrl->cons_cur[1]);
-    const uint64_t avail = (held + 1 > nidx) ? held + 1 - nidx : 0;
+    const uint64_t avail = cons_avail(held, nidx);
     s->cursor = cursor; s->next_idx = nidx; s->committed = committed;
     s->m = s->error ? 0 : (avail < a.max_n ? avail : a.max_n);
 }
@@ -535,6 +536,51 @@ __global__ void apus_consume_tail_kernel(apus_consume_args_t a)
 }
 
 // ---------------------------------------------------------------------------------
+// CONSUME WAITS (apus_consume_wait): one warp on the consume stream, between consume calls, until at least min_entries
+// committed entries lie past the cursor.  The cursor moves only inside the consume calls on this same stream, so the
+// host cannot name the absolute count to wait for when it enqueues the wait (a cuStreamWaitValue64 would need it).
+// Lane 0 polls the consumer record (the head kernel's acquire) and the cursor, backing off with __nanosleep so that a
+// waiting consumer does not load L2 beside the resident replica kernels, and reads the host's release word over PCIe
+// only every APUS_WAIT_RELEASE_POLL_NS.  It writes nothing the replica kernels read.
+// ---------------------------------------------------------------------------------
+#define APUS_WAIT_SLEEP_MIN_NS     32u
+#define APUS_WAIT_SLEEP_MAX_NS     1024u      // bounds the delay a wait adds to commit-to-applied latency
+#define APUS_WAIT_RELEASE_POLL_NS  20000ull
+
+__device__ __forceinline__ uint64_t globaltimer_ns()
+{
+    uint64_t t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+
+__global__ void apus_consume_wait_kernel(const apus_ctrl_t *ctrl, apus_hostwords_t *hw, uint64_t epoch,
+                                         uint32_t min_entries, uint64_t timeout_ns, uint32_t *outcome)
+{
+    if (threadIdx.x != 0) return;
+    const uint64_t t0 = globaltimer_ns();
+    uint64_t t_rel = t0, avail;
+    uint32_t why, sleep = APUS_WAIT_SLEEP_MIN_NS;
+    for (;;) {
+        uint64_t committed, held;
+        cons_read(ctrl, committed, held);
+        avail = cons_avail(held, ld_relaxed_sys(&ctrl->cons_cur[1]));
+        if (avail >= min_entries) { why = APUS_WAIT_READY; break; }
+        const uint64_t now = globaltimer_ns();
+        if (now - t_rel >= APUS_WAIT_RELEASE_POLL_NS) {
+            t_rel = now;
+            if (ld_relaxed_sys(&hw->cons_wait_epoch) != epoch) { why = APUS_WAIT_RELEASED; break; }
+        }
+        if (now - t0 >= timeout_ns) { why = APUS_WAIT_TIMED_OUT; break; }
+        __nanosleep(sleep);
+        if (sleep < APUS_WAIT_SLEEP_MAX_NS) sleep <<= 1;
+    }
+    if (outcome) *(volatile uint32_t *)outcome = why;
+    st_relaxed_sys(&hw->cons_wait_outcome, why);
+    st_relaxed_sys(&hw->cons_wait_avail, avail);
+}
+
+// ---------------------------------------------------------------------------------
 // host side: loading and enqueueing (apus_engine.cu brackets each enqueue in the caller's stream order)
 // ---------------------------------------------------------------------------------
 // These kernels run while the replica kernels are resident.  Under lazy module loading (CUDA_MODULE_LOADING=LAZY, the
@@ -554,6 +600,7 @@ extern "C" cudaError_t apus_batch_load(void)
     if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, apus_consume_scan_kernel);
     if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, apus_consume_copy_kernel);
     if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, apus_consume_tail_kernel);
+    if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, apus_consume_wait_kernel);
     return e;
 }
 
@@ -594,5 +641,14 @@ extern "C" cudaError_t apus_consume_enqueue(const apus_consume_args_t *a, cudaSt
     apus_consume_scan_kernel<<<1, APUS_CONS_THREADS, 0, stream>>>(*a);
     apus_consume_copy_kernel<<<a->nblk, APUS_CONS_THREADS, 0, stream>>>(*a);
     apus_consume_tail_kernel<<<1, 1, 0, stream>>>(*a);
+    return cudaGetLastError();
+}
+
+extern "C" cudaError_t apus_consume_wait_enqueue(const uint8_t *region, apus_hostwords_t *hw, uint64_t epoch,
+                                                 uint32_t min_entries, uint64_t timeout_ns, uint32_t *outcome,
+                                                 cudaStream_t stream)
+{
+    apus_consume_wait_kernel<<<1, 32, 0, stream>>>(reinterpret_cast<const apus_ctrl_t *>(region), hw, epoch, min_entries,
+                                                   timeout_ns, outcome);
     return cudaGetLastError();
 }

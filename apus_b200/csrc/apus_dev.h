@@ -146,5 +146,12 @@ __device__ __forceinline__ void cons_read(const apus_ctrl_t *ctrl, uint64_t &hel
 {
     ld_acquire_sys_2x64(ctrl->cons_rec, held_off, held_entries);
 }
+// committed entries past the consumers' cursor: the record holds entries 1 .. held_entries, the cursor stands at idx
+// next_idx.  What a consume call may examine (apus_consume_head_kernel) and what a consume wait waits for
+// (apus_consume_wait_kernel): one definition, so that a ready wait and the consume after it agree.
+__device__ __forceinline__ uint64_t cons_avail(uint64_t held_entries, uint64_t next_idx)
+{
+    return held_entries + 1 > next_idx ? held_entries + 1 - next_idx : 0;
+}
 
 #endif /* APUS_DEV_H */

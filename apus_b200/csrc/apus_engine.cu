@@ -37,6 +37,9 @@ extern "C" cudaError_t apus_synth_enqueue(apus_slot_t *ring, uint32_t mask, uint
 extern "C" cudaError_t apus_pack_enqueue(const apus_pack_args_t *a, apus_hostwords_t *hw, uint64_t *bell, uint64_t upto,
                                          cudaStream_t stream);
 extern "C" cudaError_t apus_consume_enqueue(const apus_consume_args_t *a, cudaStream_t stream);
+extern "C" cudaError_t apus_consume_wait_enqueue(const uint8_t *region, apus_hostwords_t *hw, uint64_t epoch,
+                                                 uint32_t min_entries, uint64_t timeout_ns, uint32_t *outcome,
+                                                 cudaStream_t stream);
 
 #define MAX_ROLES 160          /* CTAs of one fused launch: leader workers + local followers */
 static __thread char g_err[512];
@@ -215,6 +218,12 @@ extern "C" int apus_device_numa_node(int device)
 
 static inline int is_leader(const apus_replica *r) { return r->cfg.server_idx == r->cfg.leader_idx; }
 
+/* end every consume wait enqueued so far (apus_consume_wait): each carries the epoch it was enqueued under */
+static inline void consume_wait_release(apus_replica *r)
+{
+    if (r->hw) __atomic_fetch_add(&r->hw->cons_wait_epoch, 1ull, __ATOMIC_SEQ_CST);
+}
+
 static int ensure_host_ring(apus_replica *r)
 {
     /* device ring: the pinned staging copy of the ring is only needed when the HOST submits (lazily allocated:
@@ -286,6 +295,7 @@ static int replica_init(apus_replica *r, const apus_config_t *cfg, uint64_t log_
 
     CK(cudaHostAlloc(&r->hw, sizeof(apus_hostwords_t), cudaHostAllocMapped | cudaHostAllocPortable));
     memset((void *)r->hw, 0, sizeof(apus_hostwords_t));
+    r->hw->cons_wait_outcome = ~0ull;                                  /* no consume wait has run */
     CK(cudaHostGetDevicePointer(&r->hw_dev, r->hw, 0));
     pthread_mutex_init(&r->stage_mu, NULL);
     r->stage_bytes = 1u << 20;
@@ -378,6 +388,8 @@ extern "C" void apus_replica_destroy(apus_replica_t *r)
     }
     free(r->waits);
     if (r->copy_stream) cudaStreamSynchronize(r->copy_stream);      /* device batches still packing into the rings */
+    /* consume waits poll the hostwords page freed below: end them rather than wait for their timeouts */
+    if (r->cons_stream) consume_wait_release(r);
     if (r->cons_stream) cudaStreamSynchronize(r->cons_stream);      /* consume work still reading the region */
     for (int i = 0; i < APUS_MAX_SERVER_COUNT; i++)
         if (r->peer_is_ipc[i] && r->peer_ptr[i]) cudaIpcCloseMemHandle(r->peer_ptr[i]);
@@ -568,6 +580,8 @@ extern "C" int apus_replicas_stop(apus_replica_t **rs, int n)
 {
     if (!rs) return fail("null argument");
     for (int i = 0; i < n; i++) rs[i]->hw->stop = 1;
+    /* nothing commits on a stopped replica: its pending consume waits end now instead of at their timeouts */
+    for (int i = 0; i < n; i++) consume_wait_release(rs[i]);
     __sync_synchronize();
     int rc = APUS_OK;
     for (int i = 0; i < n; i++) {
@@ -1294,6 +1308,49 @@ extern "C" int apus_consume_status(apus_replica_t *r, uint64_t *cursor_offset, u
     return APUS_OK;
 }
 
+#define APUS_WAIT_MAX_US 60000000u     /* every consume wait ends by itself, after at most a minute */
+
+extern "C" int apus_consume_wait(apus_replica_t *r, uint32_t min_entries, uint32_t timeout_us, uint32_t *outcome,
+                                 void *stream)
+{
+    if (!r) return fail("null argument");
+    if (is_leader(r) && !(r->cfg.flags & APUS_F_APPLY_ANY_ROLE))
+        return fail("apus_consume_wait: consumption is a follower's (the leader's log is its own)");
+    if (!(r->cfg.flags & APUS_F_DEVICE_APPLY)) return fail("apus_consume_wait needs a replica created with APUS_F_DEVICE_APPLY");
+    if (min_entries == 0 || min_entries > r->idx_cap)
+        return fail("apus_consume_wait: min_entries %u outside [1, %u] (the index ring's capacity)", min_entries, r->idx_cap);
+    if (timeout_us == 0 || timeout_us > APUS_WAIT_MAX_US)
+        return fail("apus_consume_wait: timeout_us %u outside [1, %u]", timeout_us, APUS_WAIT_MAX_US);
+    if ((uintptr_t)outcome & 3u) return fail("apus_consume_wait: misaligned outcome (4 B)");
+    DeviceGuard g(r->cfg.device);
+    StageLock sl(&r->cons_mu);
+    /* the epoch is read under cons_mu, in the order of the enqueues: a release after this call ends this wait */
+    const uint64_t epoch = r->hw->cons_wait_epoch;
+    return side_stream_run((cudaStream_t)stream, r->cons_stream, r->ev_cons, "apus_consume_wait_enqueue", [&] {
+        return apus_consume_wait_enqueue(r->region, r->hw_dev, epoch, min_entries, 1000ull * timeout_us, outcome,
+                                         r->cons_stream);
+    });
+}
+
+extern "C" int apus_consume_wait_release(apus_replica_t *r)
+{
+    if (!r) return fail("null argument");
+    if (!(r->cfg.flags & APUS_F_DEVICE_APPLY))
+        return fail("apus_consume_wait_release needs a replica created with APUS_F_DEVICE_APPLY");
+    consume_wait_release(r);
+    return APUS_OK;
+}
+
+extern "C" int apus_consume_wait_status(apus_replica_t *r, uint64_t *outcome, uint64_t *available)
+{
+    if (!r) return fail("null argument");
+    if (!(r->cfg.flags & APUS_F_DEVICE_APPLY))
+        return fail("apus_consume_wait_status needs a replica created with APUS_F_DEVICE_APPLY");
+    if (outcome) *outcome = r->hw->cons_wait_outcome;
+    if (available) *available = r->hw->cons_wait_avail;
+    return APUS_OK;
+}
+
 extern "C" uint64_t apus_leader_suspect(apus_replica_t *r) { return r ? r->hw->leader_suspect : 0; }
 extern "C" uint64_t apus_last_commit_ns(apus_replica_t *r) { return r ? r->hw->last_commit_ns : 0; }
 
@@ -1779,6 +1836,7 @@ extern "C" int apus_replica_set_role(apus_replica_t *r, uint8_t leader_idx, uint
          * and the entries before it -- and my apply offset is their cursor (the commit warp keeps it so).  The consume
          * work enqueued so far runs to its end first, so that none of it sees the record change under it, and none
          * is enqueued meanwhile */
+        consume_wait_release(r);                 /* a pending wait would hold the drain for its whole timeout */
         StageLock cl(&r->cons_mu);
         CK(cudaStreamSynchronize(r->cons_stream));
         const uint64_t rec[2] = { h.commit, last - unc };

@@ -243,7 +243,12 @@ typedef struct apus_hostwords {
     volatile uint64_t cons_next_idx;     /* ... the idx of the next entry, */
     volatile uint64_t cons_need_stride;  /* ... the stride the entry that stopped it needs (0 = none), */
     volatile uint64_t cons_error;        /* ... and APUS_CONSUME_BAD_IDX (apus_gpu.h; 0 = none; sticky) */
-    uint64_t pad1[6];
+    volatile uint64_t cons_wait_epoch;   /* host -> consume waits: apus_consume_wait_release bumps it; a wait enqueued
+                                            under an older value ends as APUS_WAIT_RELEASED */
+    volatile uint64_t cons_wait_outcome; /* consume wait -> host: APUS_WAIT_* of the latest wait that ran (UINT64_MAX:
+                                            none has run yet) ... */
+    volatile uint64_t cons_wait_avail;   /* ... and the committed entries past the cursor when it ended */
+    uint64_t pad1[3];
     volatile uint32_t stop;              /* host -> kernel */
     uint32_t pad2[31];
     volatile uint64_t host_apply;        /* host -> follower kernel (APUS_FLAG_HOST_APPLY): offset up to which the

@@ -22,6 +22,7 @@ F_HOST_APPLY, F_NO_EXPRESS, F_PROFILE, F_FABRIC = 0x10, 0x20, 0x40, 0x100
 F_DEVICE_APPLY = 0x200
 F_APPLY_ANY_ROLE = 0x400   # with F_DEVICE_APPLY: the device consumers work on a leader too, and through a take-over
 CONSUME_BAD_IDX = 1
+WAIT_READY, WAIT_TIMED_OUT, WAIT_RELEASED = 0, 1, 2      # outcomes of Replica.consume_wait (APUS_WAIT_*)
 UINT64_MAX = (1 << 64) - 1
 
 u64, u32, u16, u8, i64, i32 = C.c_uint64, C.c_uint32, C.c_uint16, C.c_uint8, C.c_int64, C.c_int32
@@ -53,6 +54,7 @@ class Stats(C.Structure):
 
 
 ConsumeStatus = namedtuple("ConsumeStatus", "cursor next_idx need_stride error")
+WaitStatus = namedtuple("WaitStatus", "outcome available")
 
 _lib = None
 
@@ -70,6 +72,7 @@ EXPORTS = [
     "apus_replica_disconnect", "apus_follower_beats", "apus_device_numa_node", "apus_group_multicast", "apus_ctl_heartbeat",
     "apus_submit_device", "apus_device_submit_status", "apus_stream_wait_committed", "apus_committed_word",
     "apus_consume_device", "apus_consume_status", "apus_submit_device_packed", "apus_consume_device_packed",
+    "apus_consume_wait", "apus_consume_wait_release", "apus_consume_wait_status",
 ]
 
 
@@ -131,6 +134,9 @@ def load_library(path=LIB_PATH):
         L.apus_consume_status.argtypes = [vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]
         L.apus_submit_device_packed.argtypes = [vp, u32, vp, vp, vp, vp, vp, u64, vp, C.POINTER(u64)]
         L.apus_consume_device_packed.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp, u64, vp, vp]
+        L.apus_consume_wait.argtypes = [vp, u32, u32, vp, vp]
+        L.apus_consume_wait_release.argtypes = [vp]
+        L.apus_consume_wait_status.argtypes = [vp, C.POINTER(u64), C.POINTER(u64)]
     _lib = L
     return L
 
@@ -413,6 +419,42 @@ class Replica:
         _ck(lib().apus_consume_status(self.h, C.byref(cur), C.byref(nidx), C.byref(need), C.byref(err)),
             "apus_consume_status")
         return ConsumeStatus(int(cur.value), int(nidx.value), int(need.value), int(err.value))
+
+    def consume_wait(self, min_entries, timeout_us, outcome=None, stream=None):
+        """Make the consumers wait in `stream` order, without the host, until at least min_entries committed entries
+        (NOOP / CONFIG / HEAD included) lie past the cursor, or a release, or timeout_us from when the wait starts to
+        run (apus_consume_wait), in the roles consume_device accepts.  A consume call made after it sees at least the
+        entries it waited for.  `outcome`: an int32 or uint32 CUDA tensor [1] on this replica's device that receives
+        WAIT_READY, WAIT_TIMED_OUT or WAIT_RELEASED, for device code downstream; returned (None when not given)."""
+        import torch
+        dev = torch.device("cuda", self.device)
+        s = self._stream(stream)
+        if outcome is not None:
+            if not isinstance(outcome, torch.Tensor):
+                raise ApusError("consume_wait: outcome must be a torch tensor")
+            if outcome.device != dev:
+                raise ApusError(f"consume_wait: outcome is on {outcome.device}, the replica is on {dev}")
+            if outcome.dtype not in (torch.int32, torch.uint32):
+                raise ApusError(f"consume_wait: outcome has dtype {outcome.dtype}, expected one of "
+                                f"{(torch.int32, torch.uint32)}")
+            if tuple(outcome.shape) != (1,):
+                raise ApusError(f"consume_wait: outcome has shape {tuple(outcome.shape)}, expected (1,)")
+            if not outcome.is_contiguous():
+                raise ApusError("consume_wait: outcome is not contiguous")
+        _ck(lib().apus_consume_wait(self.h, min_entries, timeout_us, None if outcome is None else outcome.data_ptr(),
+                                    s.cuda_stream), "apus_consume_wait")
+        return outcome
+
+    def consume_wait_release(self):
+        """end every consume wait enqueued so far (they report WAIT_RELEASED); later waits are not affected"""
+        _ck(lib().apus_consume_wait_release(self.h), "apus_consume_wait_release")
+
+    def consume_wait_status(self):
+        """(WAIT_* outcome of the latest consume wait that ran, or UINT64_MAX before any; committed entries past the
+        cursor when it ended)"""
+        o, a = u64(), u64()
+        _ck(lib().apus_consume_wait_status(self.h, C.byref(o), C.byref(a)), "apus_consume_wait_status")
+        return WaitStatus(int(o.value), int(a.value))
 
     def wait_committed_on_stream(self, ticket, stream=None):
         """make `stream` (default: the current stream of the leader's device) wait until `ticket` is committed"""

@@ -308,7 +308,8 @@ int  apus_log_read_range(apus_replica_t *r, uint64_t from, uint64_t to, void *ds
  *     commit warp takes it as its own apply offset on its idle passes);
  *   - on a leader (APUS_F_APPLY_ANY_ROLE) the rows are every committed entry of its log, its own tickets and the
  *     entries of earlier terms it took over alike: the same rows, in the same order, as every follower's.
- * It never waits for commits: it delivers what is committed when it runs, which may be nothing.  APUS_ERROR on a
+ * It never waits for commits: it delivers what is committed when it runs, which may be nothing (apus_consume_wait,
+ * enqueued before it, waits in stream order until enough is committed).  APUS_ERROR on a
  * leader without APUS_F_APPLY_ANY_ROLE, on a replica without APUS_F_DEVICE_APPLY, for a null array, for an array not
  * aligned to its element size
  * (idx and req_ids 8 B, count 4 B, connection_ids and lens 2 B; payloads may have any alignment), or for max_n == 0. */
@@ -331,6 +332,37 @@ int  apus_consume_device_packed(apus_replica_t *follower, uint32_t max_n, uint64
  * the stride the entry that stopped it needs (0 = it did not stop on a long entry), APUS_CONSUME_* (0 = none) */
 int  apus_consume_status(apus_replica_t *follower, uint64_t *cursor_offset, uint64_t *next_idx, uint64_t *need_stride,
                          uint64_t *error);
+/* outcomes of apus_consume_wait */
+#define APUS_WAIT_READY      0u  /* at least min_entries committed entries lie past the consumer's cursor */
+#define APUS_WAIT_TIMED_OUT  1u
+#define APUS_WAIT_RELEASED   2u  /* ended by apus_consume_wait_release, apus_replicas_stop, apus_replica_set_role or destroy */
+/* Make the consumers wait, in stream order and without the host, until at least min_entries committed entries lie past
+ * the consumer's cursor (entries, not rows: NOOP, CONFIG and HEAD entries count), so that an application can enqueue
+ * wait -> consume -> its own apply kernel many times ahead and synchronise only when it wants to.  Accepted in the roles
+ * the consume calls accept.  `stream` is a cudaStream_t (NULL = the legacy default stream):
+ *   - the wait runs on the engine-owned consume stream, in call order with every consume call on this replica; it runs
+ *     after everything enqueued on `stream` before the call, and `stream` waits for it.  So a consume call of
+ *     max_n >= min_entries made after a READY wait examines at least min_entries entries, unless it stops on a long cmd
+ *     or on capacity as it always does;
+ *   - the wait ends on whichever comes first: ready; a release (apus_consume_wait_release, apus_replicas_stop,
+ *     apus_replica_set_role when a follower takes over, apus_replica_destroy: each ends every wait enqueued before it,
+ *     none enqueued after it); or timeout_us, counted from when the wait begins to run on the stream;
+ *   - it then writes its APUS_WAIT_* outcome to `outcome` (optional: a 4 B-aligned device word on the replica's GPU, for
+ *     device code downstream to branch on) and to the status words (apus_consume_wait_status);
+ *   - a consumer stopped for good by APUS_CONSUME_BAD_IDX gets no outcome of its own: its wait ends as the counts say,
+ *     and the consume after it delivers nothing and reports the error.
+ * A pending wait occupies the hardware queue of the consume stream until it ends: work of other streams that shares
+ * that queue (CUDA_DEVICE_MAX_CONNECTIONS) waits behind it, and if that work is what commits the entries (a leader's
+ * device batches on the same GPU), the wait runs to its timeout.  APUS_ERROR, with nothing enqueued, where the consume
+ * calls refuse the replica, for min_entries 0 or above the index ring's capacity, for timeout_us 0 or above 60 s, and
+ * for an `outcome` not aligned to 4 B. */
+int  apus_consume_wait(apus_replica_t *r, uint32_t min_entries, uint32_t timeout_us, uint32_t *outcome, void *stream);
+/* end every consume wait enqueued on this replica before the call (they report APUS_WAIT_RELEASED); later waits are
+ * not affected.  Returns without waiting for them to end. */
+int  apus_consume_wait_release(apus_replica_t *r);
+/* the pinned words the latest consume wait that ran wrote: its APUS_WAIT_* outcome (UINT64_MAX before any wait has
+ * run) and the committed entries past the cursor when it ended */
+int  apus_consume_wait_status(apus_replica_t *r, uint64_t *outcome, uint64_t *available);
 /* failure detector: 0 while the leader's heartbeats arrive, else 1 + the term whose leader fell silent */
 uint64_t apus_leader_suspect(apus_replica_t *follower);
 /* %globaltimer (ns) of the leader kernel's latest commit (device clock; step timing of resident kernels) */
