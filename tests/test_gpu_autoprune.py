@@ -13,42 +13,13 @@ import autoprune_replay as AR
 import engine_util as EU
 import orc as O
 import streams as S
-from test_gpu_parity import MODES, devices_for, submit_part, wrap_stream
+from apus_b200 import engine as E
+from engine_util import MODES, devices_for, eng, pin_and_wait, settle, submit_part, wrap_stream  # noqa: F401
+from shadow import check_heads
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(240)]
 
 FOREVER = EU.FOREVER
-F_AUTOPRUNE, F_STATS = 0x4, 0x2
-
-
-@pytest.fixture(scope="module")
-def eng():
-    import __graft_entry__ as g
-    g.build()
-    import apus_b200
-    if apus_b200.lib().apus_device_count() < 1:
-        pytest.fail("no CUDA device visible on a gpu-marked test")
-    return apus_b200
-
-
-def settle(g, t, timeout=5.0):
-    """resident kernels: wait until every follower has acked `t` entries and holds the leader's commit offset"""
-    t0 = time.time()
-    lo = g.leader.offsets()
-    while time.time() - t0 < timeout:
-        if all(r.stats()["entries_acked"] >= t and r.offsets()["commit"] == lo["commit"]
-               for i, r in enumerate(g.replicas) if i != g.leader_idx):
-            return
-        time.sleep(0.002)
-    raise AssertionError(f"followers did not settle on {t} entries / commit {lo['commit']}")
-
-
-def check_heads(reps, rp, what):
-    """every follower adopted the head of the last committed HEAD entry (poll_config_entries); the leader holds it"""
-    want = rp.last_committed_head()
-    for i, r in enumerate(reps):
-        got = r.offsets()["head"]
-        assert got == want == rp.c.offsets(i)["head"], f"{what}: replica {i} head {got}, last HEAD carries {want}"
 
 
 def check_final(g, rp):
@@ -63,7 +34,6 @@ def check_final(g, rp):
 
 
 def synth_stream(nreq, length, seed):
-    from apus_b200 import engine as E
     return [(S.CONNECT, 0, 1, b"")] + [(S.SEND, 0, 2 + i, E.synth_payload(seed, 2 + i, length)) for i in range(nreq)]
 
 
@@ -99,7 +69,7 @@ def test_autoprune_laps_replayed(eng, orc, n, L, kind, seed, mode, ctas, ring):
     rp = AR.Replay(orc, n, L)
     t_start = time.time()
     try:
-        with eng.Group(n, devices=devices_for(eng, n), log_size=L, flags=MODES[mode] | F_AUTOPRUNE, leader_ctas=ctas,
+        with eng.Group(n, devices=devices_for(eng, n), log_size=L, flags=MODES[mode] | E.F_AUTOPRUNE, leader_ctas=ctas,
                        **dev) as g:
             g.prologue()
             prev = 0
@@ -133,27 +103,11 @@ def test_autoprune_laps_replayed(eng, orc, n, L, kind, seed, mode, ctas, ring):
         rp.close()
 
 
-def _pin_and_wait(lead, reps, pins, timeout=5.0):
-    """report `pins[i]` as follower i's applied offset (APUS_F_HOST_APPLY) and wait until the leader's pruning rule
-    sees them"""
-    for i, r in enumerate(reps):
-        if i:
-            r.set_applied(pins[i])
-    t0 = time.time()
-    while True:
-        seen = lead.remote_apply_offsets()
-        if all(seen[i] == pins[i] for i in range(1, len(reps))):
-            return
-        assert time.time() - t0 < timeout, f"the leader sees apply offsets {seen[:len(reps)]}, pinned {pins}"
-        time.sleep(0.001)
-
-
 def test_autoprune_head_is_the_lagging_application(eng, orc):
     """Followers whose host replays the log (APUS_F_HOST_APPLY) report pinned apply offsets: follower 1 the end of
     launch k-2, the others the end of launch k-1.  Every auto HEAD must carry exactly follower 1's offset.  Then a
     launch that needs more room than follower 1 leaves: the leader holds (rule E2) without touching what follower 1
     has not applied, and once the offsets are raised it prunes to the released value and completes."""
-    from apus_b200 import engine as E
     n, L = 3, 1 << 18
     stream = wrap_stream("u200", 98, L)
     requests = [(O.CONFIG, 0, 0, b"")] + stream
@@ -172,7 +126,7 @@ def test_autoprune_head_is_the_lagging_application(eng, orc):
         pos = 0
         for k in range(12):
             pins = [0, ends[-2]] + [ends[-1]] * (n - 2)
-            _pin_and_wait(lead, reps, pins)
+            pin_and_wait(lead, reps, pins)
             part = requests[pos:pos + step]
             pos += len(part)
             lead.defer(True)
@@ -193,7 +147,7 @@ def test_autoprune_head_is_the_lagging_application(eng, orc):
 
         # ---- a launch that needs more room than follower 1 allows: back-pressure, then release
         pins = [0, ends[-2]] + [ends[-1]] * (n - 2)
-        _pin_and_wait(lead, reps, pins)
+        pin_and_wait(lead, reps, pins)
         kept = [r.read_range(pins[1], ends[-1], cap=L) for r in reps]     # follower 1 has not applied these
         part = requests[pos:pos + int(0.85 * L / 264)]
         pos += len(part)
@@ -216,7 +170,7 @@ def test_autoprune_head_is_the_lagging_application(eng, orc):
             assert np.array_equal(r.read_range(pins[1], ends[-1], cap=L), kept[i]), \
                 f"replica {i}: bytes follower 1 had not applied were overwritten while blocked"
         release = ends[-1]
-        _pin_and_wait(lead, reps, [0] + [release] * (n - 1))
+        pin_and_wait(lead, reps, [0] + [release] * (n - 1))
         lead.wait_committed(t, 10_000_000)
         settle(G, t)
         end = lead.offsets()["end"]
@@ -253,7 +207,7 @@ def test_express_closed_loop_with_autoprune(eng, orc):
     requests = [(O.CONFIG, 0, 0, b"")] + stream
     rp = AR.Replay(orc, n, L)
     try:
-        with eng.Group(n, devices=devices_for(eng, n), log_size=L, flags=F_STATS | F_AUTOPRUNE) as g:
+        with eng.Group(n, devices=devices_for(eng, n), log_size=L, flags=E.F_DEVICE_STATS | E.F_AUTOPRUNE) as g:
             g.launch(target=FOREVER)
             t = g.prologue()
             g.leader.wait_committed(t)

@@ -8,9 +8,7 @@ Every replica here holds a resident launch plus a copy and a consume stream, and
 their own: more than the 8 hardware queues a process gets by default, and consume work whose stream lands on a resident
 launch's queue never runs (DESIGN.md s2, "Device paths beside resident kernels").  So each case runs in a worker
 process of this file that sets CUDA_DEVICE_MAX_CONNECTIONS=32 before CUDA starts.  Marked gpu."""
-import json
 import os
-import subprocess
 import sys
 import threading
 import time
@@ -32,39 +30,18 @@ import autoprune_replay as AR  # noqa: E402
 import engine_util as EU  # noqa: E402
 import orc as O  # noqa: E402
 import streams as S  # noqa: E402
-from test_gpu_consume_device import (Consumer, PackedConsumer, check_rows, close_all, consumer_group,  # noqa: E402
-                                     drain, heads_against_reports, oracle_rows)
-from test_gpu_device_submit import tensors  # noqa: E402
-from test_gpu_parity import MODES, devices_for  # noqa: E402
-from test_gpu_prune_in_launch import _submit_all  # noqa: E402
-from test_gpu_quorum import QUIET_S, wait_for  # noqa: E402
-from test_gpu_takeover import Takeover, check_heads, ctl, elect, lap_stream, sid, watch_commits  # noqa: E402
+from apus_b200 import engine as E  # noqa: E402
+from consumers import (ANY, Consumer, PackedConsumer, catch_up, check_rows, close_all, consumer_group,  # noqa: E402
+                       drain, heads_against_reports, idx_cap, oracle_rows, wait_forwarded_all)
+from engine_util import MODES, QUIET_S, devices_for, eng, run_case, submit_all, tensors, wait_for  # noqa: E402,F401
+from shadow import Takeover, check_heads, ctl, elect, lap_stream, sid, watch_commits  # noqa: E402
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(900)]
 
 FOREVER = EU.FOREVER
-F_DEVICE_APPLY, F_APPLY_ANY_ROLE, F_NO_EXPRESS, F_AUTOPRUNE, F_HOST_APPLY = 0x200, 0x400, 0x20, 0x4, 0x10
-ANY = F_DEVICE_APPLY | F_APPLY_ANY_ROLE
 
 
-# ---- the pytest side: build once, then one worker process per case ----------------------------------------------
-@pytest.fixture(scope="module")
-def built():
-    import __graft_entry__ as g
-    g.build()
-    import apus_b200
-    if apus_b200.lib().apus_device_count() < 1:
-        pytest.fail("no CUDA device visible on a gpu-marked test")
-
-
-def run_case(name, **params):
-    cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + [os.path.abspath(__file__), name,
-                                                                         json.dumps(params)]
-    p = subprocess.run(cmd, capture_output=True, text=True, timeout=840)
-    print(p.stdout[-4000:])
-    assert p.returncode == 0, f"{name} {params}: exit {p.returncode}\n{p.stdout[-3000:]}\n{p.stderr[-6000:]}"
-
-
+# ---- the pytest side: one worker process per case ------------------------------------------------------------------
 # N, follower mode, express path, consumer layout, requests from device tensors: every mode, both N, both layouts,
 # both batch kinds and the express path on and off each appear with the others
 LEADER_CASES = [(3, "index_earlyack", True, "strided", False), (3, "walk_fenced", False, "packed", True),
@@ -76,19 +53,19 @@ LEADER_CASES = [(3, "index_earlyack", True, "strided", False), (3, "walk_fenced"
 @pytest.mark.parametrize("n,mode,express,layout,device_batch", LEADER_CASES,
                          ids=[f"n{n}-{m}-{'express' if x else 'fenced'}-{lay}-{'device' if d else 'host'}"
                               for n, m, x, lay, d in LEADER_CASES])
-def test_leader_consumes(built, n, mode, express, layout, device_batch):
+def test_leader_consumes(eng, n, mode, express, layout, device_batch):
     """a ragged 0..1500 B stream (host batches or one device batch) and closed-loop requests: every replica's rows,
     the leader's included, equal the stream and the oracle's log; every final cursor is the commit offset and is
     forwarded as the apply offset; the logs are byte-equal to the oracle's"""
-    run_case("leader_consumes", n=n, mode=mode, express=express, layout=layout, device_batch=device_batch)
+    run_case(__file__, "leader_consumes", n=n, mode=mode, express=express, layout=layout, device_batch=device_batch)
 
 
 @pytest.mark.parametrize("layout", ["strided", "packed"])
-def test_leader_cursor_gates_pruning(built, layout):
+def test_leader_cursor_gates_pruning(eng, layout):
     """one launch laps a 256 KiB ring several times with APUS_F_AUTOPRUNE while the leader's own consumer lags: every
     HEAD is checked against every replica's cursor reports, the leader's among them, and at least one carries the
     leader's lagging cursor"""
-    run_case("leader_gates_pruning", layout=layout)
+    run_case(__file__, "leader_gates_pruning", layout=layout)
 
 
 TAKEOVER_CASES = [("voters_ahead", 5, "index_earlyack", True), ("lagging", 3, "index_earlyack", True),
@@ -98,67 +75,36 @@ TAKEOVER_CASES = [("voters_ahead", 5, "index_earlyack", True), ("lagging", 3, "i
 
 @pytest.mark.parametrize("scenario,n,mode,express", TAKEOVER_CASES,
                          ids=[f"{s}-n{n}-{m}-{'express' if x else 'fenced'}" for s, n, m, x in TAKEOVER_CASES])
-def test_takeover_with_consumers_everywhere(built, scenario, n, mode, express):
+def test_takeover_with_consumers_everywhere(eng, scenario, n, mode, express):
     """the scenarios of test_gpu_takeover.py with device consumers on every replica, called from threads before, during
     (while the replicas are stopped and roles change) and after the take-over: every member's rows are the oracle's
     committed CSM-like entries of the winner's log in idx order, across both terms; the winner delivers the old-term
     entries it never submitted; the rows of the old leader and of replicas left out are a prefix of them; final cursors
     are the commit offsets; Takeover's image and offset checks pass"""
-    run_case("takeover", scenario=scenario, n=n, mode=mode, express=express)
+    run_case(__file__, "takeover", scenario=scenario, n=n, mode=mode, express=express)
 
 
-def test_lapped_resend_with_consumers_everywhere(built):
+def test_lapped_resend_with_consumers_everywhere(eng):
     """test_gpu_takeover.test_lapped_resend_on_a_pruning_ring with a device consumer on every replica: their cursors
     gate the pruning on both sides of the take-over, and the rows of the survivors equal the oracle's replayed log"""
-    run_case("lapped_resend")
+    run_case(__file__, "lapped_resend")
 
 
-def test_argument_checks(built):
+def test_argument_checks(eng):
     """the flag needs APUS_F_DEVICE_APPLY; with it a leader consumes, set_role and adjust_follower accept the replica,
     without it they keep refusing; an adjustment of a peer that shares nothing and whose consumer stands past idx 1,
     with the leader's head pruned past it, is refused and writes nothing"""
-    run_case("argument_checks")
+    run_case(__file__, "argument_checks")
 
 
 # ---- the worker side ---------------------------------------------------------------------------------------------
-def _engine():
-    import apus_b200
-    import torch
-    for d in range(torch.cuda.device_count()):
-        # torch's kernels before the resident ones: a kernel loaded lazily while replica kernels run waits for them to
-        # end.  PackedConsumer fills int64 offsets and uint8 values.
-        for dt in (torch.uint8, torch.int16, torch.int32, torch.int64):
-            x = torch.zeros(16, dtype=dt, device=torch.device("cuda", d))
-            x.fill_(1)
-            x.clone()
-        torch.cuda.synchronize(d)
-    return apus_b200
-
-
-def _oracle():
-    O.build_oracle()
-    return O.Oracle("orc")
-
-
-def wait_forwarded_all(reps, timeout=30):
-    """every replica, the leader included, has forwarded its consumers' cursor: its apply offset is its commit offset"""
-    t = time.time()
-    while True:
-        offs = [r.offsets() for r in reps]
-        if all(o["apply"] == o["commit"] for o in offs):
-            return
-        assert time.time() - t < timeout, offs
-        time.sleep(0.002)
-
-
 def case_leader_consumes(eng, orc, n, mode, express, layout, device_batch):
-    from apus_b200 import engine as E
     L = 1 << 22
     stream = S.ragged_stream(1500, 1500, conns=4, seed=700 + n, close_every=40)
     nlone, ln = 200, 40
     pl = bytes((k * 131 + 7) & 0xFF for k in range(ln))
     lone = [(S.SEND, 9, 1 + i, pl) for i in range(nlone)]
-    base = MODES[mode] | (0 if express else F_NO_EXPRESS)
+    base = MODES[mode] | (0 if express else E.F_NO_EXPRESS)
     reps = consumer_group(eng, n, L, base, leader_flags=ANY, follower_flags=[ANY] * (n - 1),
                           ring_mode=E.RING_DEVICE if device_batch else E.RING_HOST_MAPPED)
     try:
@@ -174,7 +120,7 @@ def case_leader_consumes(eng, orc, n, mode, express, layout, device_batch):
             t0 = lead.submit_device(*tensors(stream, lead.device, 1500))
             t = t0 + len(stream) - 1
         else:
-            t = _submit_all(lead, stream)
+            t = submit_all(lead, stream)
         lead.wait_committed(t, 60_000_000)
         lat = lead.closed_loop(nlone, ln, 9, 1)                # one in flight: the express path when it is on
         assert len(lat) == nlone
@@ -217,8 +163,8 @@ def case_leader_gates_pruning(eng, orc, layout):
     stream = S.ragged_stream(int(6.5 * 1.15 * L / 814) + 1, 1500, conns=3, seed=197, close_every=20)
     stride = 1500
     requests = [(O.CONFIG, 0, 0, b"")] + stream
-    reps = consumer_group(eng, n, L, leader_flags=F_AUTOPRUNE | ANY, ring_slots=1 << 14, ring_bytes=1 << 17, ctas=ctas,
-                          follower_flags=[F_HOST_APPLY, ANY, ANY])
+    reps = consumer_group(eng, n, L, leader_flags=E.F_AUTOPRUNE | ANY, ring_slots=1 << 14, ring_bytes=1 << 17, ctas=ctas,
+                          follower_flags=[E.F_HOST_APPLY, ANY, ANY])
     rec = AR.Recorder(reps[1], 1, L)
     rp = AR.Replay(orc, n, L)
     lagging = 0
@@ -246,7 +192,7 @@ def case_leader_gates_pruning(eng, orc, layout):
         EU.launch_each(eng, reps, FOREVER)
         lead = reps[0]
         lead.submit(O.CONFIG, 0, 0, O.cid_image(n))
-        t = _submit_all(lead, stream)
+        t = submit_all(lead, stream)
         deadline = time.time() + 400
         while lead.committed() < t:
             rec.check()
@@ -306,7 +252,7 @@ def case_leader_gates_pruning(eng, orc, layout):
 
 
 class AnyTakeover(Takeover):
-    """Takeover (test_gpu_takeover.py) with a device consumer on every replica, each called from its own thread with
+    """Takeover (shadow.py) with a device consumer on every replica, each called from its own thread with
     max_n from 1 up, whatever the replicas are doing: running, stopped, changing roles"""
 
     def __init__(self, eng, orc, n, L, flags, seed):
@@ -368,16 +314,6 @@ class AnyTakeover(Takeover):
         super().close()
 
 
-def catch_up(cn, timeout=60):
-    """consume until nothing is left and the cursor is the replica's commit offset"""
-    t_end = time.time() + timeout
-    while True:
-        k, st = cn.step(512)
-        if k == 0 and st.cursor == cn.rep.offsets()["commit"]:
-            return st
-        assert time.time() < t_end, (st, cn.rep.offsets())
-
-
 def check_consumers(c, lead, members, cons, old_lead, want=None):
     """every member's rows are `want` (default: the oracle's CSM-like entries of the winner's log), with strictly
     increasing idx; every other replica's rows are a prefix of them; the winner delivered the old term's rows"""
@@ -401,7 +337,7 @@ def check_consumers(c, lead, members, cons, old_lead, want=None):
 
 
 def case_takeover(eng, orc, scenario, n, mode, express):
-    flags = MODES[mode] | (0 if express else F_NO_EXPRESS)
+    flags = MODES[mode] | (0 if express else E.F_NO_EXPRESS)
     p = AnyTakeover(eng, orc, n, 1 << 20, flags, seed=n + 100)
     try:
         if scenario == "voters_ahead":           # test_voters_commit_ahead_of_the_winners
@@ -480,12 +416,11 @@ def case_lapped_resend(eng, orc):
     third of a lap, a device consumer on every replica from its own thread: follower 2 misses 0.6 to 0.7 of a lap, 1
     takes over with voter 2 (a resend across the ring's wrap and the offset index's), and the new term laps twice.  The consumers
     gate the pruning on both sides; the survivors' rows equal the requests of both terms in order"""
-    from apus_b200 import engine as E
     n, L = 3, 1 << 16
     old, new = lap_stream(20_000, 0, 31), lap_stream(20_000, 1 << 8, 32)
     requests = [(O.CONFIG, 0, 0, b"")]
     rp = AR.Replay(orc, n, L)
-    g = E.Group(n, devices=devices_for(eng, n), log_size=L, flags=MODES["index_earlyack"] | F_AUTOPRUNE | ANY)
+    g = E.Group(n, devices=devices_for(eng, n), log_size=L, flags=MODES["index_earlyack"] | E.F_AUTOPRUNE | ANY)
     cons = [Consumer(r, 1500, 512) for r in g.replicas]
     halt, errs = threading.Event(), []
     state = dict(prev=0, k=0, running=[])
@@ -533,6 +468,15 @@ def case_lapped_resend(eng, orc):
             assert rp.written < 12 * L, "no point to start the lagging range found"
             run(old, 0.04 * L, [1, 2])
         lag_start, w_lag = g.replicas[2].offsets()["end"], rp.written
+        # follower 2 pins the pruning at lag_start, so that the window below never blocks (as in test_gpu_takeover's
+        # case).  A bounded launch ends without waiting for the consumers, and a follower forwards its consumer's cursor
+        # only every few hundred polls, so the cursor the leader holds may lie a launch or more behind: let follower 2
+        # alone run until it has forwarded its consumer's cursor at lag_start
+        state["running"] = [g.replicas[2]]
+        EU.launch_each(eng, state["running"], FOREVER)
+        wait_for(lambda: g.leader.remote_apply_offsets()[2] == lag_start, f"follower 2 to forward its cursor {lag_start}")
+        EU.stop_each(eng, state["running"])
+        state["running"] = []
         while rp.written - w_lag < 0.6 * L or (not [h for h in rp.heads if h.lap_pos >= w_lag] and
                                                 rp.written - w_lag < 0.7 * L):
             run(old, 0.1 * L, [1])
@@ -551,7 +495,8 @@ def case_lapped_resend(eng, orc):
             # (heads are compared at the end, not after each launch: the voter adopts the head of a HEAD entry it was
             # resent only with the next HEAD it acks, and here the consumers' cursors decide when that comes)
             run(new, 0.3 * L, [2])
-        check_heads([g.replicas[1], g.replicas[2]], rp, [1, 2], f"after the new term's last launch, ending at {rp.end()}")
+        check_heads([g.replicas[1], g.replicas[2]], rp, f"after the new term's last launch, ending at {rp.end()}",
+                    [1, 2])
         halt.set()
         for x in th:
             x.join(60)
@@ -589,13 +534,6 @@ def case_lapped_resend(eng, orc):
 INDEX_OFF = 65536 + 320 * 1024          # apus_layout.h APUS_INDEX_OFF: the offset index follows the log header
 
 
-def idx_cap(L):
-    cap = 1024
-    while cap * 64 < L:
-        cap <<= 1
-    return cap
-
-
 def region_bytes(rep, off, n):
     """bytes [off, off + n) of a replica's HBM region (control block, header, offset index), read through the region
     pointer its peer handle carries in this process"""
@@ -612,15 +550,14 @@ def region_bytes(rep, off, n):
 
 
 def case_argument_checks(eng, orc):
-    from apus_b200 import engine as E
     lib = ctl(eng)
     n, L = 3, 1 << 20
     devs = devices_for(eng, n)
     for i in (0, 1):
         with pytest.raises(E.ApusError, match="needs APUS_F_DEVICE_APPLY"):
-            E.Replica(devs[i], i, n, 0, 1, L, flags=F_APPLY_ANY_ROLE)
+            E.Replica(devs[i], i, n, 0, 1, L, flags=E.F_APPLY_ANY_ROLE)
     with pytest.raises(E.ApusError, match="needs APUS_F_DEVICE_APPLY"):
-        E.Replica(devs[1], 1, n, 0, 1, L, flags=F_APPLY_ANY_ROLE | F_HOST_APPLY)
+        E.Replica(devs[1], 1, n, 0, 1, L, flags=E.F_APPLY_ANY_ROLE | E.F_HOST_APPLY)
     plain = consumer_group(eng, n, L)                       # device consumers on the followers only
     a = consumer_group(eng, n, L, leader_flags=ANY, follower_flags=[ANY, ANY])
     b = []
@@ -640,7 +577,7 @@ def case_argument_checks(eng, orc):
         # group a: 40 requests, every consumer reads them all (cursor past idx 1)
         lead = a[0]
         lead.submit(O.CONFIG, 0, 0, O.cid_image(n))
-        t = _submit_all(lead, [(S.CONNECT, 1, 1, b"")] + [(S.SEND, 1, 2 + k, b"a" * (k % 60)) for k in range(40)])
+        t = submit_all(lead, [(S.CONNECT, 1, 1, b"")] + [(S.SEND, 1, 2 + k, b"a" * (k % 60)) for k in range(40)])
         EU.launch_each(eng, a, t)
         for r in a:
             r.wait(60_000)
@@ -655,7 +592,7 @@ def case_argument_checks(eng, orc):
         b[1].connect(0, b[0].export())
         lb = b[0]
         lb.submit(O.CONFIG, 0, 0, O.cid_image(n))
-        tb = _submit_all(lb, [(S.CONNECT, 2, 1, b"")] + [(S.SEND, 2, 2 + k, b"b" * (k % 50)) for k in range(100)])
+        tb = submit_all(lb, [(S.CONNECT, 2, 1, b"")] + [(S.SEND, 2, 2 + k, b"b" * (k % 50)) for k in range(100)])
         EU.launch_each(eng, b, tb)
         for r in b:
             r.wait(60_000)
@@ -694,9 +631,4 @@ def case_argument_checks(eng, orc):
 u64 = C.c_uint64
 
 if __name__ == "__main__":
-    import faulthandler
-    name, params = sys.argv[1], json.loads(sys.argv[2]) if len(sys.argv) > 2 else {}
-    faulthandler.dump_traceback_later(float(os.environ.get("APUS_CASE_TIMEOUT_S", "780")), exit=True)  # where it hung
-    eng_, orc_ = _engine(), _oracle()
-    globals()["case_" + name](eng_, orc_, **params)
-    print(f"{name} {params}: ok")
+    EU.worker_main(globals())

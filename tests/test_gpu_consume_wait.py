@@ -7,9 +7,7 @@ As in test_gpu_consume_any_role.py, every replica holds a resident launch plus a
 consumers bring torch streams of their own; a pending wait also holds its consume stream's hardware queue (DESIGN.md
 s2).  So each case runs in a worker process of this file that sets CUDA_DEVICE_MAX_CONNECTIONS=32 before CUDA starts.
 Marked gpu."""
-import json
 import os
-import subprocess
 import sys
 import time
 
@@ -20,36 +18,23 @@ if __name__ == "__main__":
         if p not in sys.path:
             sys.path.insert(0, p)
 
-import ctypes as C  # noqa: E402
-
 import numpy as np  # noqa: E402
 import pytest  # noqa: E402
 
 import engine_util as EU  # noqa: E402
 import orc as O  # noqa: E402
 import streams as S  # noqa: E402
-from test_gpu_consume_any_role import (ANY, _engine, _oracle, built, catch_up, idx_cap,  # noqa: E402,F401
-                                       wait_forwarded_all)
-from test_gpu_consume_device import Consumer, check_rows, close_all, consumer_group, oracle_rows  # noqa: E402
-from test_gpu_device_submit import tensors  # noqa: E402
-from test_gpu_parity import MODES, devices_for  # noqa: E402
-from test_gpu_prune_in_launch import _submit_all  # noqa: E402
-from test_gpu_takeover import elect  # noqa: E402
+from apus_b200 import engine as E  # noqa: E402
+from consumers import (ANY, Consumer, catch_up, check_rows, close_all, consumer_group, idx_cap,  # noqa: E402
+                       new_stream, oracle_rows, wait_forwarded_all)
+from engine_util import MODES, devices_for, eng, run_case, submit_all, tensors  # noqa: E402,F401
+from shadow import elect  # noqa: E402
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(900)]
 
 FOREVER = EU.FOREVER
-F_DEVICE_APPLY, F_AUTOPRUNE = 0x200, 0x4
 MAX_LEN = 300                  # longest cmd of the streams here: the strided stride, and the packed cap per row
 NEVER = 1 << 12                # far more entries than the release cases commit: a wait for them never becomes ready
-
-
-def run_case(name, **params):
-    cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + [os.path.abspath(__file__), name,
-                                                                         json.dumps(params)]
-    p = subprocess.run(cmd, capture_output=True, text=True, timeout=840)
-    print(p.stdout[-4000:])
-    assert p.returncode == 0, f"{name} {params}: exit {p.returncode}\n{p.stdout[-3000:]}\n{p.stderr[-6000:]}"
 
 
 # N, consumer layout, a small pruning log that laps while waits are pending, consumers on the leader too
@@ -60,81 +45,55 @@ LEADER_CASES = [(3, "strided", False, True), (5, "packed", False, True)]
 
 @pytest.mark.parametrize("n,layout,lapping,leader", AHEAD_CASES,
                          ids=[f"n{n}-{lay}-{'lapping' if lap else 'flat'}" for n, lay, lap, _ in AHEAD_CASES])
-def test_apply_loop_ahead_of_the_host(built, n, layout, lapping, leader):
+def test_apply_loop_ahead_of_the_host(eng, n, layout, lapping, leader):
     """every follower enqueues K rounds of wait(B) -> consume(B) before the leader has a request; the requests then
     come in pieces (host submit_uniform and submit_device) with no host synchronise between rounds: every outcome is
     READY, the rows are the request stream and (where the log does not lap) the oracle's rows, and every cursor ends at
     the commit offset.  The lapping case prunes a 256 KiB log behind the consumers several times while waits are
     pending"""
-    run_case("apply_ahead", n=n, layout=layout, lapping=lapping, leader=leader)
+    run_case(__file__, "apply_ahead", n=n, layout=layout, lapping=lapping, leader=leader)
 
 
 @pytest.mark.parametrize("n,layout,lapping,leader", LEADER_CASES, ids=[f"n{n}-{lay}" for n, lay, _, _ in LEADER_CASES])
-def test_apply_loop_ahead_on_the_leader(built, n, layout, lapping, leader):
+def test_apply_loop_ahead_on_the_leader(eng, n, layout, lapping, leader):
     """the same with APUS_F_DEVICE_APPLY | APUS_F_APPLY_ANY_ROLE on every replica: the leader's own waits are READY and
     its rows are the stream's and the oracle's"""
-    run_case("apply_ahead", n=n, layout=layout, lapping=lapping, leader=leader)
+    run_case(__file__, "apply_ahead", n=n, layout=layout, lapping=lapping, leader=leader)
 
 
-def test_already_ready(built):
+def test_already_ready(eng):
     """a wait for entries that are already committed ends READY at once (host clock far under its timeout), and the
     consume after it delivers them"""
-    run_case("already_ready")
+    run_case(__file__, "already_ready")
 
 
-def test_timeout(built):
+def test_timeout(eng):
     """wait(1, 200 ms) with nothing submitted ends TIMED_OUT after at least 200 ms on the host clock and within a
     generous bound; the consume after it delivers no row and leaves the cursor where it was"""
-    run_case("timeout")
+    run_case(__file__, "timeout")
 
 
-def test_release_points(built):
+def test_release_points(eng):
     """a pending 30 s wait ends RELEASED within 1 s at consume_wait_release (a later wait is not affected), at
     Group.stop() and at close() (destroy)"""
-    run_case("release")
+    run_case(__file__, "release")
 
 
-def test_release_at_takeover(built):
+def test_release_at_takeover(eng):
     """a pending 30 s wait on a follower that takes over ends RELEASED at apus_replica_set_role, which then returns
     within 1 s; a wait enqueued after it sees the old-term entries that commit with the new leader's blank CONFIG, and
     the new leader's rows equal the oracle's"""
-    run_case("release_takeover")
+    run_case(__file__, "release_takeover")
 
 
-def test_refusals(built):
+def test_refusals(eng):
     """min_entries 0 or above idx_cap, timeout_us 0 or above 60 s, a replica without APUS_F_DEVICE_APPLY, a leader
     without APUS_F_APPLY_ANY_ROLE, a misaligned, wrong-device or wrong-dtype outcome: ApusError, nothing enqueued; a
     normal wait and consume work afterwards"""
-    run_case("refusals")
+    run_case(__file__, "refusals")
 
 
 # ---- the worker side ---------------------------------------------------------------------------------------------
-def new_stream(device):
-    """A CUDA stream of its own, created with the runtime rather than taken from torch's pool.  The pool creates dozens
-    of streams at once, and those wrap around the 32 hardware queues onto the replicas' own streams.  A consumer stream
-    that shares a queue with the leader's streams makes them wait behind its pending consume waits (DESIGN.md s2)."""
-    import torch
-    try:
-        rt = C.CDLL("libcudart.so.12")
-    except OSError:
-        import nvidia.cuda_runtime as ncr
-        rt = C.CDLL(os.path.join(list(ncr.__path__)[0], "lib", "libcudart.so.12"))
-    s = C.c_void_p()
-    assert rt.cudaSetDevice(device) == 0
-    assert rt.cudaStreamCreateWithFlags(C.byref(s), 1) == 0                 # cudaStreamNonBlocking
-    return torch.cuda.ExternalStream(s.value, device=torch.device("cuda", device))
-
-
-class StreamConsumer(Consumer):
-    """Consumer (test_gpu_consume_device.py) on a stream from new_stream()"""
-
-    def __init__(self, rep, stride, cap):
-        self.rep, self.stream = rep, new_stream(rep.device)
-        self.rows, self.calls = [], 0
-        self.cur, self.at, self.reports = 0, 0, []
-        self.stride, self.cap, self.out = stride, cap, None
-
-
 class Ahead:
     """K rounds of consume_wait(B) -> consume(B) on one replica's own stream, each round into its own slice of the
     output and its own outcome word; read back once, at the end"""
@@ -231,7 +190,6 @@ def submit_piece(lead, k, part):
 
 
 def case_apply_ahead(eng, orc, n, layout, lapping, leader):
-    from apus_b200 import engine as E
     B = 128
     if lapping:
         L, n_req, B = 1 << 18, 5200, 256  # about 4.3 laps of the log; the HEAD entries the leader adds are not counted
@@ -241,14 +199,14 @@ def case_apply_ahead(eng, orc, n, layout, lapping, leader):
         n_req = K * B - 1                 # the CONFIG and the requests fill the K rounds exactly
     parts = pieces(n_req, seed=300 + n + (7 if lapping else 0) + (11 if leader else 0))
     allreq = [x for p in parts for x in p]
-    ff = [ANY if leader else F_DEVICE_APPLY] * (n - 1)
-    reps = consumer_group(eng, n, L, leader_flags=(ANY if leader else 0) | (F_AUTOPRUNE if lapping else 0),
+    ff = [ANY if leader else E.F_DEVICE_APPLY] * (n - 1)
+    reps = consumer_group(eng, n, L, leader_flags=(ANY if leader else 0) | (E.F_AUTOPRUNE if lapping else 0),
                           follower_flags=ff, ring_mode=E.RING_DEVICE)
     who = list(range(n)) if leader else list(range(1, n))
     try:
         got = {}
         ahead = {i: Ahead(reps[i], layout, K, B) for i in who}
-        cons = {i: StreamConsumer(reps[i], MAX_LEN, 512) for i in who}  # the catch-up after the rounds
+        cons = {i: Consumer(reps[i], MAX_LEN, 512, new_stream(reps[i].device)) for i in who}  # the catch-up after the rounds
         # (the launch first: a launch copies its arguments on a stream that may share a queue with a pending wait)
         EU.launch_each(eng, reps, FOREVER)
         for i in who:                                                    # before the leader has any request
@@ -294,7 +252,6 @@ def case_apply_ahead(eng, orc, n, layout, lapping, leader):
 
 
 def _group(eng, n, L):
-    from apus_b200 import engine as E
     return E.Group(n, devices=devices_for(eng, n), log_size=L, flags=MODES["index_earlyack"] | ANY)
 
 
@@ -304,16 +261,15 @@ def _word(t):
 
 def case_already_ready(eng, orc):
     import torch
-    from apus_b200 import engine as E
     n, L = 3, 1 << 20
     reps = consumer_group(eng, n, L)
     try:
-        cn = StreamConsumer(reps[1], MAX_LEN, 512)
+        cn = Consumer(reps[1], MAX_LEN, 512, new_stream(reps[1].device))
         oc = torch.full((1,), -1, dtype=torch.int32, device=torch.device("cuda", reps[1].device))
         EU.launch_each(eng, reps, FOREVER)
         stream = [(S.SEND, 2, 1 + k, bytes([k & 0xFF]) * (k % 90)) for k in range(100)]
         reps[0].submit(O.CONFIG, 0, 0, O.cid_image(n))
-        reps[0].wait_committed(_submit_all(reps[0], stream))
+        reps[0].wait_committed(submit_all(reps[0], stream))
         commit = reps[0].offsets()["commit"]
         t_end = time.time() + 30
         while reps[1].offsets()["commit"] != commit:
@@ -337,11 +293,10 @@ def case_already_ready(eng, orc):
 
 def case_timeout(eng, orc):
     import torch
-    from apus_b200 import engine as E
     n, L = 3, 1 << 20
     reps = consumer_group(eng, n, L)
     try:
-        cn = StreamConsumer(reps[1], MAX_LEN, 512)
+        cn = Consumer(reps[1], MAX_LEN, 512, new_stream(reps[1].device))
         oc = torch.full((1,), -1, dtype=torch.int32, device=torch.device("cuda", reps[1].device))
         EU.launch_each(eng, reps, FOREVER)
         before = reps[1].consume_status()
@@ -368,7 +323,6 @@ def _pending(rep, oc, stream):
 
 def case_release(eng, orc):
     import torch
-    from apus_b200 import engine as E
     n, L = 3, 1 << 20
     g = _group(eng, n, L)
     try:
@@ -413,17 +367,16 @@ def case_release(eng, orc):
 
 def case_release_takeover(eng, orc):
     import torch
-    from apus_b200 import engine as E
     n, L = 3, 1 << 20
     g = _group(eng, n, L)
-    cons = [StreamConsumer(r, MAX_LEN, 512) for r in g.replicas]
+    cons = [Consumer(r, MAX_LEN, 512, new_stream(r.device)) for r in g.replicas]
     c = None
     try:
         oc = torch.full((2,), -1, dtype=torch.int32, device=torch.device("cuda", g.replicas[1].device))
         EU.launch_each(eng, g.replicas, FOREVER)
         g.prologue()
         stream = S.ragged_stream(300, MAX_LEN, conns=3, seed=77, close_every=40)
-        g.leader.wait_committed(_submit_all(g.leader, stream))
+        g.leader.wait_committed(submit_all(g.leader, stream))
         _, st = cons[1].step(50)                          # the winner's consumer has read only part of the old term
         assert st.next_idx == 51, st
         t_end = time.time() + 30
@@ -468,13 +421,12 @@ def case_release_takeover(eng, orc):
 
 def case_refusals(eng, orc):
     import torch
-    from apus_b200 import engine as E
     n, L = 3, 1 << 20
-    reps = consumer_group(eng, n, L, follower_flags=[F_DEVICE_APPLY, 0])
+    reps = consumer_group(eng, n, L, follower_flags=[E.F_DEVICE_APPLY, 0])
     try:
         r = reps[1]
         dev = torch.device("cuda", r.device)
-        cn = StreamConsumer(r, MAX_LEN, 512)
+        cn = Consumer(r, MAX_LEN, 512, new_stream(r.device))
         buf = torch.zeros(8, dtype=torch.uint8, device=dev)
         cap = idx_cap(L)
         for args, msg in (((0, 1000), "min_entries"), ((cap + 1, 1000), "min_entries"), ((1, 0), "timeout_us"),
@@ -504,7 +456,7 @@ def case_refusals(eng, orc):
         r.consume_wait(11, 10_000_000, outcome=oc, stream=cn.stream)
         reps[0].submit(O.CONFIG, 0, 0, O.cid_image(n))
         stream = [(S.SEND, 4, 1 + k, b"x" * k) for k in range(10)]
-        reps[0].wait_committed(_submit_all(reps[0], stream))
+        reps[0].wait_committed(submit_all(reps[0], stream))
         k, st = cn.step(64)
         assert int(oc.cpu()[0]) == E.WAIT_READY and k == 10 and st.error == 0, (int(oc.cpu()[0]), k, st)
         check_rows(cn.rows, stream, first_idx=2)
@@ -513,9 +465,4 @@ def case_refusals(eng, orc):
 
 
 if __name__ == "__main__":
-    import faulthandler
-    name, params = sys.argv[1], json.loads(sys.argv[2]) if len(sys.argv) > 2 else {}
-    faulthandler.dump_traceback_later(float(os.environ.get("APUS_CASE_TIMEOUT_S", "780")), exit=True)  # where it hung
-    eng_, orc_ = _engine(), _oracle()
-    globals()["case_" + name](eng_, orc_, **params)
-    print(f"{name} {params}: ok")
+    EU.worker_main(globals())

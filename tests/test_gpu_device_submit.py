@@ -9,63 +9,12 @@ import pytest
 import engine_util as EU
 import orc as O
 import streams as S
-from test_gpu_parity import MODES, devices_for, hole_bytes, prune_both, wrap_stream
+from engine_util import (MODES, device_group, devices_for, eng, hole_bytes, prune_both, submit_host,  # noqa: F401
+                         tensors, torch_module, wrap_stream)
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(180)]
 
-FOREVER = (1 << 64) - 1
-
-
-@pytest.fixture(scope="module")
-def eng():
-    import __graft_entry__ as g
-    g.build()
-    import apus_b200
-    if apus_b200.lib().apus_device_count() < 1:
-        pytest.fail("no CUDA device visible on a gpu-marked test")
-    return apus_b200
-
-
-@pytest.fixture(scope="module", autouse=True)
-def release_torch_memory():
-    """hand the memory torch cached for these tests back to the driver before the next module: later tests run
-    several replica processes on the same GPU"""
-    yield
-    import gc
-    import torch
-    gc.collect()
-    if torch.cuda.is_initialized():
-        torch.cuda.synchronize()
-        torch.cuda.empty_cache()
-
-
-def tensors(part, device, stride=None):
-    """the tailq_entry_t fields of `part` as the CUDA tensors submit_device takes"""
-    import torch
-    n = len(part)
-    if stride is None:
-        stride = max([len(p) for *_, p in part] + [1])
-    pl = np.zeros((n, stride), dtype=np.uint8)
-    for k, (_, _, _, p) in enumerate(part):
-        pl[k, :len(p)] = np.frombuffer(p, dtype=np.uint8)
-    dev = torch.device("cuda", device)
-    return (torch.from_numpy(np.array([t for t, *_ in part], dtype=np.uint8)).to(dev),
-            torch.from_numpy(np.array([c for _, c, _, _ in part], dtype=np.uint16).view(np.int16)).to(dev),
-            torch.from_numpy(np.array([r for _, _, r, _ in part], dtype=np.uint64).view(np.int64)).to(dev),
-            torch.from_numpy(np.array([len(p) for *_, p in part], dtype=np.uint16).view(np.int16)).to(dev),
-            torch.from_numpy(pl).to(dev))
-
-
-def submit_host(g, part):
-    """one apus_submit_batch call for `part`"""
-    stride = max([len(p) for *_, p in part] + [1])
-    pl = np.zeros(len(part) * stride, dtype=np.uint8)
-    for k, (_, _, _, p) in enumerate(part):
-        pl[k * stride:k * stride + len(p)] = np.frombuffer(p, dtype=np.uint8)
-    t0 = g.leader.submit_batch([t for t, *_ in part], [c for _, c, _, _ in part], [r for _, _, r, _ in part],
-                               [len(p) for *_, p in part], pl, stride)
-    g.tickets = t0 + len(part) - 1
-    return t0
+FOREVER = EU.FOREVER
 
 
 def submit_mixed(g, part, rng):
@@ -82,10 +31,6 @@ def submit_mixed(g, part, rng):
             t0 = g.submit_device(*tensors(cut, g.leader.device))
         assert t0 == want and g.tickets == want + len(cut) - 1
         k += m
-
-
-def device_group(eng, n, L, **kw):
-    return eng.Group(n, devices=devices_for(eng, n), log_size=L, ring_mode=eng.RING_DEVICE, **kw)
 
 
 @pytest.mark.parametrize("n,seed", [(3, 401), (5, 402)])

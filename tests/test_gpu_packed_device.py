@@ -12,44 +12,13 @@ import pytest
 import engine_util as EU
 import orc as O
 import streams as S
-from test_gpu_consume_device import (PackedConsumer, check_rows, close_all, consumer_group, drain, oracle_rows,
-                                     wait_forwarded)
-from test_gpu_device_submit import submit_host, tensors
-from test_gpu_parity import MODES, devices_for, prune_both, wrap_stream
-from test_gpu_prune_in_launch import _submit_all
+from consumers import PackedConsumer, check_rows, close_all, consumer_group, drain, oracle_rows, wait_forwarded
+from engine_util import (MODES, device_group, devices_for, eng, prune_both, submit_all, submit_host,  # noqa: F401
+                         tensors, torch_module, wrap_stream)
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(600)]
 
 FOREVER = EU.FOREVER
-
-
-@pytest.fixture(scope="module")
-def eng():
-    import __graft_entry__ as g
-    g.build()
-    import apus_b200
-    if apus_b200.lib().apus_device_count() < 1:
-        pytest.fail("no CUDA device visible on a gpu-marked test")
-    import torch
-    for d in range(torch.cuda.device_count()):
-        # load torch's kernels before the replica kernels are resident (a lazy load may wait for running kernels)
-        x = torch.zeros(16, dtype=torch.uint8, device=torch.device("cuda", d))
-        x.fill_(1)
-        x.clone()
-        torch.zeros(4, dtype=torch.int64, device=torch.device("cuda", d)).fill_(-7)
-        torch.cuda.synchronize(d)
-    return apus_b200
-
-
-@pytest.fixture(scope="module", autouse=True)
-def release_torch_memory():
-    yield
-    import gc
-    import torch
-    gc.collect()
-    if torch.cuda.is_initialized():
-        torch.cuda.synchronize()
-        torch.cuda.empty_cache()
 
 
 def heavy_stream(n_req, seed, conns=3, tail_every=40):
@@ -118,10 +87,6 @@ def submit_mixed_packed(g, part, rng, max_cut=300):
             t0 = submit_retry(g, lambda: submit_host(g, cut))
         assert t0 == want and g.tickets == want + len(cut) - 1, (t0, want, g.tickets)
         k += len(cut)
-
-
-def device_group(eng, n, L, **kw):
-    return eng.Group(n, devices=devices_for(eng, n), log_size=L, ring_mode=eng.RING_DEVICE, **kw)
 
 
 def _stream(kind, n):
@@ -314,7 +279,7 @@ def test_packed_consumption_matches_oracle(eng, orc, mode, kind):
         EU.launch_each(eng, reps, FOREVER)
         lead = reps[0]
         lead.submit(O.CONFIG, 0, 0, O.cid_image(n))
-        t = _submit_all(lead, stream)
+        t = submit_all(lead, stream)
         last_idx = len(stream) + 1
         for cn in cons:
             # exact once this follower holds every entry as committed (and the CONFIG at idx 1 is behind the cursor)
@@ -348,7 +313,7 @@ def test_capacity_stop(eng):
     try:
         lead = reps[0]
         lead.submit(O.CONFIG, 0, 0, O.cid_image(n))
-        t = _submit_all(lead, stream)
+        t = submit_all(lead, stream)
         EU.launch_each(eng, reps, t)
         for r in reps:
             r.wait(60_000)
@@ -566,7 +531,7 @@ def test_packed_destroy_right_after_enqueue(eng):
     try:
         lead = reps[0]
         lead.submit(O.CONFIG, 0, 0, O.cid_image(n))
-        t = _submit_all(lead, [(S.CONNECT, 1, 1, b"")] + [(S.SEND, 1, 2 + k, b"x" * k) for k in range(50)])
+        t = submit_all(lead, [(S.CONNECT, 1, 1, b"")] + [(S.SEND, 1, 2 + k, b"x" * k) for k in range(50)])
         EU.launch_each(eng, reps, t)
         for r in reps:
             r.wait(60_000)

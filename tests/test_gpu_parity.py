@@ -10,31 +10,9 @@ import pytest
 import engine_util as EU
 import orc as O
 import streams as S
+from engine_util import MODES, devices_for, eng, prune_both, wrap_case  # noqa: F401
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(180)]
-
-
-@pytest.fixture(scope="module")
-def eng():
-    import __graft_entry__ as g
-    g.build()
-    import apus_b200
-    if apus_b200.lib().apus_device_count() < 1:
-        pytest.fail("no CUDA device visible on a gpu-marked test")
-    return apus_b200
-
-
-def devices_for(eng, n):
-    nd = eng.lib().apus_device_count()
-    return [i % nd for i in range(n)]
-
-
-MODES = {
-    "index_earlyack": 0x2,               # default: offset index, ack on tail observation
-    "walk_fenced": 0x2 | 0x1 | 0x8,      # reference-like follower: parse the bytes, reply bytes before the ack
-    "index_fenced": 0x2 | 0x1,
-    "walk_earlyack": 0x2 | 0x8,
-}
 
 
 def run_and_compare(eng, orc, n, L, stream, ring_mode=0, prologue=True, exact=True, devices=None, chunks=1,
@@ -193,87 +171,27 @@ def test_exact_fit_wrap_rule_E1(eng, orc):
     c.close()
 
 
-def prune_both(g, c):
-    """log_pruning (dare_server.c:1996-2067) on both sides: head := min apply, HEAD entry."""
-    idx = c.prune()
-    if not idx:
-        return False
-    head = c.offsets(0)["head"]
-    g.leader.set_head(head)
-    g.submit(eng_HEAD, 0, 0, head.to_bytes(8, "little"))
-    return True
-
-
-eng_HEAD = 3
-
-
-def wrap_stream(kind, seed, L):
-    """ragged<max>: lengths 0..max (ragged1500 with connection churn); u<len>: uniform, enough for 4.5 laps"""
-    if kind == "ragged180":
-        return S.ragged_stream(max(1500, int(4.5 * L / 150)), 180, conns=3, seed=seed)
-    if kind == "ragged1500":
-        return S.ragged_stream(int(4.5 * L / 814) + 1, 1500, conns=3, seed=seed, close_every=20)
-    size = int(kind[1:])
-    return S.uniform_stream(int(4.5 * L / (64 + size)) + 1, size, conns=1, seed=seed)
-
-
-def submit_part(g, part, uniform):
-    """the requests of one launch: one deferred flush, or (uniform) runs of SENDs through apus_submit_uniform"""
-    if not uniform:
-        g.submit_stream(part)
-        return
-    k = 0
-    while k < len(part):
-        typ, clt, rid, payload = part[k]
-        j = k + 1
-        while (typ == S.SEND and j < len(part) and part[j][0] == S.SEND and part[j][1] == clt and
-               part[j][2] == rid + (j - k) and len(part[j][3]) == len(payload)):
-            j += 1
-        if j - k > 1:
-            pl = np.frombuffer(b"".join(p for _, _, _, p in part[k:j]), dtype=np.uint8)
-            g.tickets = g.leader.submit_uniform(j - k, S.SEND, clt, rid, len(payload), pl) + (j - k) - 1
-        else:
-            g.submit(typ, clt, rid, payload)
-        k = j
-
-
-def hole_bytes(img, ents):
-    """the bytes no append writes: header bytes 41..47 and the slack behind the data image of every entry"""
-    out = []
-    for off, stride in ents:
-        typ = int(img[off + 26])
-        nb = {O.NOOP: 0, O.CONFIG: 16, O.HEAD: 8}.get(typ, 2 + int(img[off + 48]) + 256 * int(img[off + 49]))
-        out.append(img[off + 41:off + 48])
-        out.append(img[off + 48 + nb:off + stride])
-    return np.concatenate(out)
-
-
-def _wrap_case(n, L, kind, seed, mode, step=None, ctas=0, ring="host", id=None):
-    return pytest.param(n, L, kind, seed, mode, step, ctas, ring,
-                        id=id or f"{kind}-n{n}-{L >> 10}K-{mode}-ctas{ctas or 4}" + ("-device" if ring == "device" else ""))
-
-
 WRAP_CASES = [
     # small ragged entries, a dozen per launch: ghost headers, header-does-not-fit jumps, tiny tiles (the original cases,
     # under their original ids)
-    *[_wrap_case(n, L, "ragged180", seed, mode, step=12, id=f"{n}-{L}-{seed}-{mode}")
+    *[wrap_case(n, L, "ragged180", seed, mode, step=12, id=f"{n}-{L}-{seed}-{mode}")
       for mode in ("index_earlyack", "walk_fenced") for n, L, seed in ((3, 16384, 77), (5, 32768, 78), (3, 8192, 79))],
     # below: about a third of the ring per launch, so that a claim holds tens of entries
     # stride 1024: the 16 B register compose path with the holes-only prefill
-    _wrap_case(3, 1 << 16, "u960", 80, "index_earlyack", ctas=1),
-    _wrap_case(5, 1 << 18, "u960", 81, "walk_fenced", ctas=16),
+    wrap_case(3, 1 << 16, "u960", 80, "index_earlyack", ctas=1),
+    wrap_case(5, 1 << 18, "u960", 81, "walk_fenced", ctas=16),
     # stride 1065: byte-granular compose with the holes-only prefill; the slack hole straddles 16 B chunks
-    _wrap_case(3, 1 << 16, "u1001", 82, "walk_fenced", ctas=2),
-    _wrap_case(5, 1 << 18, "u1001", 83, "index_earlyack", ctas=4),
+    wrap_case(3, 1 << 16, "u1001", 82, "walk_fenced", ctas=2),
+    wrap_case(5, 1 << 18, "u1001", 83, "index_earlyack", ctas=4),
     # stride 264: whole-warp compose with the full-sweep prefill
-    _wrap_case(3, 1 << 16, "u200", 84, "index_earlyack", ctas=16),
-    _wrap_case(3, 1 << 18, "u200", 85, "walk_fenced", ctas=96),
+    wrap_case(3, 1 << 16, "u200", 84, "index_earlyack", ctas=16),
+    wrap_case(3, 1 << 18, "u200", 85, "walk_fenced", ctas=96),
     # 0..1500 B with connection churn: ghost headers of large entries, tiles switching between the two prefills
-    _wrap_case(3, 1 << 18, "ragged1500", 86, "index_earlyack", ctas=2),
-    _wrap_case(5, 1 << 16, "ragged1500", 87, "walk_fenced", ctas=16),
-    _wrap_case(3, 1 << 16, "ragged180", 88, "index_earlyack", ctas=1),
+    wrap_case(3, 1 << 18, "ragged1500", 86, "index_earlyack", ctas=2),
+    wrap_case(5, 1 << 16, "ragged1500", 87, "walk_fenced", ctas=16),
+    wrap_case(3, 1 << 16, "ragged180", 88, "index_earlyack", ctas=1),
     # requests in HBM, one bulk call per launch: claims of 256 slots
-    _wrap_case(3, 1 << 18, "u200", 89, "index_earlyack", ctas=1, ring="device"),
+    wrap_case(3, 1 << 18, "u200", 89, "index_earlyack", ctas=1, ring="device"),
 ]
 
 
@@ -283,53 +201,7 @@ def test_wrap_laps_with_pruning(eng, orc, n, L, kind, seed, mode, step, ctas, ri
     stale bytes in entry holes, HEAD entries, for every compose path and prefill of the
     leader and 1..96 leader CTAs.  Pruning happens at quiescent points so that the
     stream of appends is identical on both sides."""
-    stream = wrap_stream(kind, seed, L)
-    if step is None:
-        step = max(1, int(0.3 * L * len(stream) / S.stream_bytes(stream)))
-    assert S.stream_bytes(stream) >= 4 * L                  # laps
-    orc.set_rules(O.RULES_ENGINE)
-    c = O.Cluster(orc, n, leader=0, term=1, length=L)
-    c.prologue()
-    dev = dict(ring_mode=eng.RING_DEVICE, ring_slots=1 << 12, ring_bytes=1 << 20) if ring == "device" else {}
-    with eng.Group(n, devices=devices_for(eng, n), log_size=L, flags=MODES[mode], leader_ctas=ctas, **dev) as g:
-        g.prologue()
-        total = 1
-        marks = []                                          # (log bytes appended so far, leader's end) per launch
-        written, prev = 0, c.offsets(0)["end"]
-        for k in range(0, len(stream), step):
-            part = stream[k:k + step]
-            for typ, clt, rid, payload in part:
-                assert c.submit(typ, clt, rid, O.cmd_image(payload)) != 0
-            c.round(); c.round()
-            submit_part(g, part, ring == "device")
-            total += len(part)
-            g.run()
-            if prune_both(g, c):
-                total += 1
-                c.round(); c.round()
-                g.run()
-            e = c.offsets(0)["end"]
-            written += (e - prev) % L
-            prev = e
-            marks.append((written, e))
-        EU.compare_group_to_oracle(g, c, exact=True)
-        # teeth: the entries of the last lap (all still in the ring) keep bytes of earlier laps in their holes, so a
-        # prefill that stored zeros or loaded the wrong chunk would have shown in the comparison above
-        start = next(e for w, e in marks if written - w < L)
-        img = c.image(0)
-        ents = O.walk_entries(img, start, prev, L)
-        holes = hole_bytes(img, ents)
-        assert len(ents) >= 4 * step // 3 or len(ents) >= 100, len(ents)
-        assert np.count_nonzero(holes) >= 0.5 * len(holes), (np.count_nonzero(holes), len(holes))
-        assert g.leader.committed() == total
-        assert c.offsets(0)["head"] != 0
-        # every follower adopted the head carried by the last committed HEAD entry
-        # (poll_config_entries, dare_server.c:2163-2186)
-        lh = g.leader.offsets()["head"]
-        assert lh == c.offsets(0)["head"]
-        for r in g.replicas[1:]:
-            assert r.offsets()["head"] == lh
-    c.close()
+    EU.wrap_laps_with_pruning(eng, orc, n, L, kind, seed, mode, step, ctas, ring)
 
 
 def test_persistent_service_mode_closed_loop(eng, orc):

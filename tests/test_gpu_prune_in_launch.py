@@ -13,21 +13,11 @@ import autoprune_replay as AR
 import engine_util as EU
 import orc as O
 import streams as S
-from test_gpu_parity import MODES
+from engine_util import MODES, eng, submit_all  # noqa: F401
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(900)]
 
 FOREVER = EU.FOREVER
-
-
-@pytest.fixture(scope="module")
-def eng():
-    import __graft_entry__ as g
-    g.build()
-    import apus_b200
-    if apus_b200.lib().apus_device_count() < 1:
-        pytest.fail("no CUDA device visible on a gpu-marked test")
-    return apus_b200
 
 
 def _case(n, L, kind, mode, ctas, ring, lagging, laps, id):
@@ -62,29 +52,6 @@ def _stream(kind, L, laps):
     return S.sized_stream(int(laps * L / 6200) + 1, 3072, 9216, seed=98)
 
 
-def _submit_all(lead, stream):
-    """the requests (CONNECT first, then runs of SENDs through apus_submit_uniform where they share a shape)"""
-    t, k = 0, 0
-    while k < len(stream):
-        typ, clt, rid, payload = stream[k]
-        j = k + 1
-        while (typ == S.SEND and j < len(stream) and stream[j][0] == S.SEND and stream[j][1] == clt and
-               stream[j][2] == rid + (j - k) and len(stream[j][3]) == len(payload)):
-            j += 1
-        while True:
-            try:
-                if j - k > 1:
-                    pl = np.frombuffer(b"".join(p for _, _, _, p in stream[k:j]), dtype=np.uint8)
-                    t = lead.submit_uniform(j - k, S.SEND, clt, rid, len(payload), pl) + (j - k) - 1
-                else:
-                    t = lead.submit(typ, clt, rid, payload)
-                break
-            except BlockingIOError:                 # a ring smaller than the stream drains while the kernels run
-                time.sleep(0.0005)
-        k = j
-    return t
-
-
 @pytest.mark.parametrize("n,L,kind,mode,ctas,ring,lagging,laps", CASES)
 def test_prune_in_one_launch_replayed(eng, orc, n, L, kind, mode, ctas, ring, lagging, laps):
     from apus_b200 import engine as E
@@ -115,10 +82,10 @@ def test_prune_in_one_launch_replayed(eng, orc, n, L, kind, mode, ctas, ring, la
                 lead.submit(S.CONNECT, 0, 1, b"")
                 t = lead.submit_synth(nreq, S.SEND, 0, 2, 64, seed) + nreq - 1
             else:
-                t = _submit_all(lead, stream)
+                t = submit_all(lead, stream)
         EU.launch_each(eng, reps, FOREVER)
         if fed_later:
-            t = _submit_all(lead, stream)
+            t = submit_all(lead, stream)
         deadline = time.time() + 300
         while lead.committed() < t:
             for r in recs:

@@ -17,189 +17,12 @@ import numpy as np
 import pytest
 
 import engine_util as EU
-import orc as O
 import streams as S
-from test_gpu_parity import MODES, devices_for, eng  # noqa: F401
+from apus_b200 import engine as E
+from engine_util import MODES, devices_for, eng, wait_for  # noqa: F401
+from shadow import Pair
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(300)]
-
-F_PROFILE = 0x40                 # followers count the self-certified publishes they verified (stats phase_ns[0])
-QUIET_S = 0.1                    # how long "nothing commits" is watched
-
-
-def wait_for(cond, what, timeout=10.0):
-    t_end = time.time() + timeout
-    while not cond():
-        assert time.time() < t_end, f"timed out waiting for {what}"
-        time.sleep(0.001)
-
-
-def mask_others(img, ents, me):
-    """zero the reply bytes of every replica but `me`"""
-    img = img.copy()
-    for off, _ in ents:
-        own = img[off + 28 + me]
-        img[off + 28:off + 41] = 0
-        img[off + 28 + me] = own
-    return img
-
-
-class Pair:
-    """One engine group (resident, one launch per replica) and the oracle cluster that shadows it."""
-
-    def __init__(self, eng, orc, n, lead, L, flags, seed):
-        self.eng, self.n, self.lead, self.L = eng, n, lead, L
-        self.quorum = n // 2 + 1
-        self.followers = [i for i in range(n) if i != lead]
-        self.live = set(self.followers)
-        self.rejoined = set()                                # followers that have been down at least once
-        self.rng = np.random.default_rng(seed)
-        self.g = eng.Group(n, devices=devices_for(eng, n), leader=lead, log_size=L, flags=flags)
-        orc.set_rules(O.RULES_ENGINE)
-        self.c = O.Cluster(orc, n, leader=lead, term=1, length=L)
-        self.conn, self.rid = lead << 8, 1
-        EU.launch_each(eng, self.g.replicas)
-        self.g.prologue()
-        self.c.prologue()
-        self.lone(1)                                         # the CONNECT
-        self.rounds()
-        self.settle()
-
-    def close(self):
-        try:
-            # (after a failure) bring the majority back first: a leader stopped with uncommitted entries waits for them
-            for i in self.followers:
-                if i not in self.live:
-                    self.relaunch(i)
-            self.leader.wait_committed(self.g.tickets, 5_000_000)
-        except Exception:                                    # noqa: BLE001 - the test's own failure is the report
-            pass
-        try:
-            self.g.stop()
-        finally:
-            self.g.close()
-            self.c.close()
-
-    @property
-    def leader(self):
-        return self.g.leader
-
-    def rep(self, i):
-        return self.g.replicas[i]
-
-    def has_quorum(self):
-        return 1 + len(self.live) >= self.quorum
-
-    def _next(self, max_len):
-        if self.rid == 1:
-            req = (S.CONNECT, self.conn, 1, b"")
-        else:
-            ln = int(self.rng.integers(0, max_len + 1))
-            req = (S.SEND, self.conn, self.rid, self.rng.integers(0, 256, size=ln, dtype=np.uint8).tobytes())
-        self.rid += 1
-        typ, clt, rid, payload = req
-        assert self.c.submit(typ, clt, rid, O.cmd_image(payload)) != 0
-        return req
-
-    def burst(self, k):
-        """k requests of up to 300 B in one flush: the tile path"""
-        self.g.submit_stream([self._next(300) for _ in range(k)])
-
-    def lone(self, k):
-        """k requests of up to 78 B (an inline image), one at a time: the express path.  Each waits for its commit,
-        or, without a quorum, until it is published"""
-        for _ in range(k):
-            t = self.g.submit(*self._next(78))
-            if self.has_quorum():
-                self.leader.wait_committed(t, 5_000_000)
-            else:
-                self.wait_published(t)
-
-    def wait_published(self, t):
-        wait_for(lambda: self.leader.stats()["entries_published"] >= t, f"entry {t} published")
-
-    def rounds(self):
-        self.c.round(live=self.live)
-        self.c.round(live=self.live)
-
-    def settle(self):
-        """every live follower has acked everything published and followed the leader's commit offset"""
-        t = self.g.tickets
-        self.wait_published(t)
-        lc = self.leader.offsets()["commit"]
-        for i in self.live:
-            r = self.rep(i)
-            wait_for(lambda: r.stats()["entries_acked"] >= t and (not self.has_quorum() or r.offsets()["commit"] == lc),
-                     f"follower {i} acked {t}")
-
-    def stop(self, i):
-        EU.stop_each(self.eng, [self.rep(i)])
-        self.live.discard(i)
-
-    def relaunch(self, i):
-        EU.launch_each(self.eng, [self.rep(i)])
-        self.live.add(i)
-        self.rejoined.add(i)
-
-    def check_images(self):
-        """leader exact over [0, its end); every follower over [0, its end) (the engine's leader also stores beyond a
-        stopped follower's end)"""
-        L, lead = self.L, self.lead
-        lo = self.c.offsets(lead)
-        limg_o = self.c.image(lead)
-        ents = O.walk_entries(limg_o, 0, lo["end"], L)
-        limg_e = self.leader.image()
-        d = np.nonzero(limg_e[:lo["end"]] != limg_o[:lo["end"]])[0]
-        assert len(d) == 0, f"leader: {len(d)} bytes differ, first at {int(d[0])}"
-        for i in self.followers:
-            end = self.c.offsets(i)["end"]
-            ei, oi = self.rep(i).image(0, end), self.c.image(i, 0, end)
-            if i in self.rejoined:
-                fents = [(o, s) for o, s in ents if o + s <= end]
-                ei, oi = mask_others(ei, fents, i), mask_others(oi, fents, i)
-            d = np.nonzero(ei != oi)[0]
-            assert len(d) == 0, f"follower {i} (live {i in self.live}): {len(d)} bytes differ, first at {int(d[0])}"
-
-    def check_offsets(self, keys_leader=("head", "apply", "commit", "end", "tail")):
-        for i in range(self.n):
-            eo, oo = self.rep(i).offsets(), self.c.offsets(i)
-            keys = keys_leader if i == self.lead else ("head", "apply", "commit", "end")
-            assert {k: eo[k] for k in keys} == {k: oo[k] for k in keys}, (i, i in self.live, eo, oo)
-            if i != self.lead:
-                assert eo["commit"] <= eo["end"], f"I4: follower {i} commit {eo['commit']} beyond its end {eo['end']}"
-
-    def check_committed(self):
-        """a quorum is up: everything commits; exact against the oracle"""
-        self.leader.wait_committed(self.g.tickets, 5_000_000)
-        self.rounds()
-        self.settle()
-        assert self.leader.committed() == self.g.tickets
-        self.check_offsets()
-        self.check_images()
-
-    def check_not_committed(self, committed0, progress0, lcommit0):
-        """no quorum: the new entries are published and acked by the live followers, and nothing commits"""
-        self.rounds()
-        self.settle()
-        t_end = time.time() + QUIET_S
-        while time.time() < t_end:
-            assert self.leader.committed() == committed0
-            assert self.leader.progress() == progress0
-            assert self.leader.offsets()["commit"] == lcommit0
-            time.sleep(0.005)
-        assert self.leader.stats()["entries_published"] == self.g.tickets
-        assert self.c.offsets(self.lead)["commit"] == lcommit0
-        self.check_offsets(keys_leader=("head", "apply", "commit"))   # the leader's header `end` follows its commit
-        self.check_images()
-
-    def step(self, k_burst, k_lone):
-        before = (self.leader.committed(), self.leader.progress(), self.leader.offsets()["commit"])
-        self.burst(k_burst)
-        self.lone(k_lone)
-        if self.has_quorum():
-            self.check_committed()
-        else:
-            self.check_not_committed(*before)
 
 
 # Up to 7 replicas: every replica is a launch of its own that stays resident, and a process has 8 hardware work queues
@@ -245,7 +68,8 @@ def test_express_with_a_lagging_follower(eng, orc, n, mode):
     """A stopped follower misses lone requests.  The first one after the stop finds every follower caught up and goes
     out self-certified: the stopped follower verifies it against its own HBM after the relaunch.  With k > 1 it lags,
     the publishes are fenced, and it takes the k entries in one step.  The express path runs in both phases."""
-    p = Pair(eng, orc, n, 0, 1 << 20, MODES[mode] | F_PROFILE, seed=n)
+    # (APUS_F_PROFILE: followers count the self-certified publishes they verified, stats phase_ns[0])
+    p = Pair(eng, orc, n, 0, 1 << 20, MODES[mode] | E.F_PROFILE, seed=n)
     try:
         f = p.followers[-1]
         for k, certs in ((1, 1), (4, 0)):

@@ -25,20 +25,10 @@ import engine_util as EU
 import orc as O
 import ring_edges as RE
 import streams as S
-from test_gpu_autoprune import _pin_and_wait
-from test_gpu_parity import MODES, devices_for, prune_both
+from apus_b200 import engine as E
+from engine_util import MODES, devices_for, eng, pin_and_wait, prune_both  # noqa: F401
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(300)]
-
-
-@pytest.fixture(scope="module")
-def eng():
-    import __graft_entry__ as g
-    g.build()
-    import apus_b200
-    if apus_b200.lib().apus_device_count() < 1:
-        pytest.fail("no CUDA device visible on a gpu-marked test")
-    return apus_b200
 
 
 @pytest.fixture(scope="module")
@@ -117,7 +107,6 @@ class AutoEngine:
     leader's express path on (it places single inline requests itself)."""
 
     def __init__(self, eng, orc, n, L, seed, mode, ctas, express=False):
-        from apus_b200 import engine as E
         self.n, self.L = n, L
         self.express = express
         self.rng = np.random.default_rng(seed)
@@ -162,7 +151,7 @@ class AutoEngine:
 
     def pin(self, v):
         if v != self.pinned:
-            _pin_and_wait(self.lead, self.reps, [0] + [v] * (self.n - 1))
+            pin_and_wait(self.lead, self.reps, [0] + [v] * (self.n - 1))
             self.pinned = v
 
     def _put(self, r, submit):

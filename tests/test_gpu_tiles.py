@@ -4,23 +4,14 @@ through the CTA-wide scan, next to uniform ones), and a check that claims really
 import numpy as np
 import pytest
 
+import engine_util as EU
 import streams as S
-import test_gpu_parity as P
+from engine_util import MODES, devices_for, eng, wrap_case  # noqa: F401
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(180)]
 
 
-@pytest.fixture(scope="module")
-def eng():
-    import __graft_entry__ as g
-    g.build()
-    import apus_b200
-    if apus_b200.lib().apus_device_count() < 1:
-        pytest.fail("no CUDA device visible on a gpu-marked test")
-    return apus_b200
-
-
-def mixed_stream(kind, L, seed):
+def mixed_stream(kind, seed, L):
     """64 B SENDs for 4.5 laps, and in between either a 200 B SEND every 37th request (stride 264: a claim that holds
     one is not uniform and takes the CTA-wide scan) or a CLOSE + CONNECT every 53rd (64 B entries: the 128 B entries
     leave the 128 B grid, so that wraps leave gaps inside a claim)"""
@@ -43,37 +34,32 @@ def mixed_stream(kind, L, seed):
     return out
 
 
-MIXED = ("mix200", "churn")
-
-
-# the u64 and mixed cases run the body of test_gpu_parity.test_wrap_laps_with_pruning -- one lap-and-oracle harness:
+# the u64 and mixed cases run engine_util.wrap_laps_with_pruning, as test_gpu_parity.test_wrap_laps_with_pruning does:
 # about a third of the ring per launch, pruning at quiescent points, every byte against the oracle, and the holes of the
 # last lap non-zero (what catches a prefill that stored zeros or loaded the wrong chunk)
 @pytest.mark.parametrize("n,L,kind,seed,mode,step,ctas,ring", [
-    P._wrap_case(5, 1 << 18, "u64", 90, "index_earlyack", ctas=1, id="5-262144-90-index_earlyack-1-host"),
-    P._wrap_case(5, 1 << 18, "u64", 91, "walk_fenced", ctas=16, id="5-262144-91-walk_fenced-16-host"),
+    wrap_case(5, 1 << 18, "u64", 90, "index_earlyack", ctas=1, id="5-262144-90-index_earlyack-1-host"),
+    wrap_case(5, 1 << 18, "u64", 91, "walk_fenced", ctas=16, id="5-262144-91-walk_fenced-16-host"),
     # requests in HBM, one bulk call per launch: claims of 512 slots
-    P._wrap_case(3, 1 << 18, "u64", 92, "index_earlyack", ctas=1, ring="device", id="3-262144-92-index_earlyack-1-device"),
+    wrap_case(3, 1 << 18, "u64", 92, "index_earlyack", ctas=1, ring="device", id="3-262144-92-index_earlyack-1-device"),
 ])
 def test_u64_laps(eng, orc, n, L, kind, seed, mode, step, ctas, ring):
     """the benchmark's request shape over 4.5 laps of a small ring with pruning"""
-    P.test_wrap_laps_with_pruning(eng, orc, n, L, kind, seed, mode, step, ctas, ring)
+    EU.wrap_laps_with_pruning(eng, orc, n, L, kind, seed, mode, step, ctas, ring)
 
 
 @pytest.mark.parametrize("kind,ctas,ring", [("mix200", 1, "device"), ("mix200", 4, "host"), ("churn", 1, "device"),
                                             ("churn", 16, "host")])
-def test_mixed_shapes_laps(eng, orc, monkeypatch, kind, ctas, ring):
-    base = P.wrap_stream
-    monkeypatch.setattr(P, "wrap_stream", lambda k, seed, L: mixed_stream(k, L, seed) if k in MIXED else base(k, seed, L))
-    P.test_wrap_laps_with_pruning(eng, orc, 3, 1 << 17, kind, 93, "index_earlyack", None, ctas, ring)
+def test_mixed_shapes_laps(eng, orc, kind, ctas, ring):
+    EU.wrap_laps_with_pruning(eng, orc, 3, 1 << 17, kind, 93, "index_earlyack", None, ctas, ring, stream_of=mixed_stream)
 
 
 def test_claims_exceed_256_slots(eng, orc):
     """one bulk launch from a device ring into one worker CTA: the claims hold more than 256 slots on average"""
     n, L, nreq = 3, 1 << 24, 1 << 16
     payloads = np.random.default_rng(94).integers(0, 256, size=nreq * 64, dtype=np.uint8)
-    with eng.Group(n, devices=P.devices_for(eng, n), log_size=L, ring_mode=eng.RING_DEVICE, ring_slots=1 << 17,
-                   ring_bytes=1 << 20, leader_ctas=1, flags=P.MODES["index_earlyack"]) as g:
+    with eng.Group(n, devices=devices_for(eng, n), log_size=L, ring_mode=eng.RING_DEVICE, ring_slots=1 << 17,
+                   ring_bytes=1 << 20, leader_ctas=1, flags=MODES["index_earlyack"]) as g:
         g.prologue()
         g.submit(S.CONNECT, 0, 1, b"")
         g.submit_uniform(nreq, 64, 0, 2, payloads)

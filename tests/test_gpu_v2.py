@@ -13,12 +13,13 @@ import pytest
 import engine_util as EU
 import orc as O
 import streams as S
-from test_gpu_parity import MODES, devices_for, eng, prune_both, check_replica_images_consistent  # noqa: F401
+from apus_b200 import engine as E
+from engine_util import MODES, devices_for, eng, prune_both, settle  # noqa: F401
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(240)]
 
 FOREVER = EU.FOREVER
-F_NO_EXPRESS, F_HOST_APPLY, F_AUTOPRUNE, F_STATS = 0x20, 0x10, 0x4, 0x2
+
 
 def closed_loop(g, stream, timeout_us=5_000_000):
     t = 0
@@ -26,17 +27,6 @@ def closed_loop(g, stream, timeout_us=5_000_000):
         t = g.submit(typ, clt, rid, payload)
         g.leader.wait_committed(t, timeout_us)
     return t
-
-
-def settle(g, t, timeout=5.0):
-    """wait until every follower has acked and applied everything (the commit push is lazy)"""
-    t0 = time.time()
-    lo = g.leader.offsets()
-    while time.time() - t0 < timeout:
-        if all(r.stats()["entries_acked"] >= t and r.offsets()["commit"] == lo["commit"]
-               for i, r in enumerate(g.replicas) if i != g.leader_idx):
-            return
-        time.sleep(0.005)
 
 
 @pytest.mark.parametrize("mode", list(MODES))
@@ -69,7 +59,7 @@ def test_express_off_is_the_same_log(eng, orc):
     n, L = 3, 1 << 20
     stream = S.ragged_stream(300, 78, conns=2, seed=7)
     imgs = []
-    for flags in (F_STATS, F_STATS | F_NO_EXPRESS):
+    for flags in (E.F_DEVICE_STATS, E.F_DEVICE_STATS | E.F_NO_EXPRESS):
         with eng.Group(n, devices=devices_for(eng, n), log_size=L, flags=flags) as g:
             g.launch(target=FOREVER)
             g.leader.wait_committed(g.prologue())
@@ -78,7 +68,7 @@ def test_express_off_is_the_same_log(eng, orc):
             st = g.leader.stats()
             g.stop()
             imgs.append([hashlib.sha256(r.image().tobytes()).hexdigest() for r in g.replicas])
-            if flags & F_NO_EXPRESS:
+            if flags & E.F_NO_EXPRESS:
                 assert st["turn_ns"][5] == 0
     assert imgs[0] == imgs[1]
 
@@ -91,7 +81,7 @@ def test_express_across_wraps_with_pruning(eng, orc):
     orc.set_rules(O.RULES_ENGINE)
     c = O.Cluster(orc, n, leader=0, term=1, length=L)
     c.prologue()
-    with eng.Group(n, devices=devices_for(eng, n), log_size=L, flags=F_STATS) as g:
+    with eng.Group(n, devices=devices_for(eng, n), log_size=L, flags=E.F_DEVICE_STATS) as g:
         g.launch(target=FOREVER)
         total = g.prologue()
         g.leader.wait_committed(total)
@@ -144,7 +134,6 @@ def test_config_shapes_exact(eng, orc, n, payload, nreq):
 def test_device_generated_requests_exact(eng, orc, payload):
     """apus_submit_synth: the fill kernel writes the requests straight into the HBM ring; the log must be what the
     same requests give when the host submits them (payload bytes recomputed on the host with numpy)."""
-    from apus_b200 import engine as E
     n, L, nreq, seed = 5, O.LOG_SIZE, 5000, 0xC0FFEE
     stream = [(S.CONNECT, 0, 1, b"")] + [(S.SEND, 0, 2 + i, E.synth_payload(seed, 2 + i, payload)) for i in range(nreq)]
     with eng.Group(n, devices=devices_for(eng, n), log_size=L, ring_mode=eng.RING_DEVICE, ring_slots=1 << 14,
@@ -222,17 +211,12 @@ def test_slow_follower_host_apply_many_laps(eng):
     one, the leader's pruning rule never lets the ring overwrite entries that were not replayed (it back-pressures
     instead), and after 10+ laps around a 1 MiB ring every follower has replayed exactly the submitted stream."""
     n, L, payload, per, rounds = 3, 1 << 20, 200, 10000, 5
-    flags_l = F_STATS | F_AUTOPRUNE
-    flags_f = F_STATS | F_AUTOPRUNE | F_HOST_APPLY
-    from apus_b200 import engine as E
+    flags_l = E.F_DEVICE_STATS | E.F_AUTOPRUNE
+    flags_f = E.F_DEVICE_STATS | E.F_AUTOPRUNE | E.F_HOST_APPLY
     devs = devices_for(eng, n)
     reps = [E.Replica(devs[i], i, n, 0, 1, L, eng.RING_HOST_MAPPED, 1 << 16, 16 << 20, flags_l if i == 0 else flags_f, 4)
             for i in range(n)]
-    blobs = [r.export() for r in reps]
-    for r in reps:
-        for j, b in enumerate(blobs):
-            if j != r.idx:
-                r.connect(j, b)
+    EU.connected(reps)
     import ctypes as C
     try:
         for dev in sorted(set(devs), key=lambda d: any(r.is_leader and r.device == d for r in reps)):
@@ -293,16 +277,12 @@ def test_stop_while_blocked_on_a_full_log(eng):
     """ADVICE (medium): stop arrives while leader workers wait for free space / for their turns.  Nothing may be
     placed, stored or published with a stale placement: what the replicas hold afterwards is a clean common prefix."""
     n, L, payload = 3, 1 << 18, 200
-    from apus_b200 import engine as E
     # followers never report an applied offset (HOST_APPLY with a host that replays nothing): head cannot move
     devs = devices_for(eng, n)
+    flags = E.F_DEVICE_STATS | E.F_AUTOPRUNE
     reps = [E.Replica(devs[i], i, n, 0, 1, L, eng.RING_HOST_MAPPED, 1 << 14, 4 << 20,
-                      (F_STATS | F_AUTOPRUNE) if i == 0 else (F_STATS | F_AUTOPRUNE | F_HOST_APPLY), 4) for i in range(n)]
-    blobs = [r.export() for r in reps]
-    for r in reps:
-        for j, b in enumerate(blobs):
-            if j != r.idx:
-                r.connect(j, b)
+                      flags if i == 0 else flags | E.F_HOST_APPLY, 4) for i in range(n)]
+    EU.connected(reps)
     import ctypes as C
     try:
         for dev in sorted(set(devs), key=lambda d: any(r.is_leader and r.device == d for r in reps)):
@@ -353,7 +333,8 @@ def test_heartbeats_and_failure_detector(eng):
     """The leader's commit warp beats into every follower (dare_ibv_rc.c:868-958); a follower whose leader kernel
     is gone reports the suspicion within its timeout, not before."""
     n, L = 3, 1 << 20
-    with eng.Group(n, devices=devices_for(eng, n), log_size=L, flags=F_STATS, hb_period_us=100, hb_timeout_us=20_000) as g:
+    with eng.Group(n, devices=devices_for(eng, n), log_size=L, flags=E.F_DEVICE_STATS, hb_period_us=100,
+                   hb_timeout_us=20_000) as g:
         EU.launch_each(eng, g.replicas)
         g.leader.wait_committed(g.prologue())
         time.sleep(0.15)                                    # many timeouts' worth of beats
@@ -374,16 +355,12 @@ def test_heartbeats_and_failure_detector(eng):
 def test_term_fence_ignores_a_deposed_leader(eng, orc):
     """A follower that has moved to term 2 does not look at publishes stamped with term 1 (SURVEY H2, software form):
     it acks nothing and its `end` does not move, while the term-1 majority (leader + the other follower) commits."""
-    from apus_b200 import engine as E
     import ctypes as C
     n, L = 3, 1 << 20
     devs = devices_for(eng, n)
-    reps = [E.Replica(devs[i], i, n, 0, 2 if i == 2 else 1, L, eng.RING_HOST_MAPPED, 0, 0, F_STATS, 2) for i in range(n)]
-    blobs = [r.export() for r in reps]
-    for r in reps:
-        for j, b in enumerate(blobs):
-            if j != r.idx:
-                r.connect(j, b)
+    reps = [E.Replica(devs[i], i, n, 0, 2 if i == 2 else 1, L, eng.RING_HOST_MAPPED, 0, 0, E.F_DEVICE_STATS, 2)
+            for i in range(n)]
+    EU.connected(reps)
     try:
         for dev in sorted(set(devs), key=lambda d: any(r.is_leader and r.device == d for r in reps)):
             rs = [r for r in reps if r.device == dev]
@@ -415,7 +392,6 @@ def test_term_fence_ignores_a_deposed_leader(eng, orc):
 def test_multicast_replication_exact(eng, orc, n, payload):
     """Fabric mode: the replicas' regions are VMM allocations bound to an NVSwitch multicast object; the leader's T5 step
     (and the express push) issue ONE multimem.st per 16 B chunk and the switch fans it out.  Same bytes everywhere."""
-    from apus_b200 import engine as E
     nd = eng.lib().apus_device_count()
     if nd < n:
         pytest.skip(f"needs {n} GPUs (one per replica), {nd} visible")
@@ -426,7 +402,7 @@ def test_multicast_replication_exact(eng, orc, n, payload):
     pb = pl.tobytes()
     stream = [(S.CONNECT, 0, 1, b"")] + [(S.SEND, 0, 2 + i, pb[i * payload:(i + 1) * payload]) for i in range(nreq)]
     with eng.Group(n, devices=list(range(n)), log_size=L, ring_mode=eng.RING_DEVICE, ring_slots=1 << 16,
-                   ring_bytes=64 << 20, flags=F_STATS | E.F_FABRIC) as g:
+                   ring_bytes=64 << 20, flags=E.F_DEVICE_STATS | E.F_FABRIC) as g:
         try:
             g.multicast()
         except E.ApusError as ex:

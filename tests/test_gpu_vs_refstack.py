@@ -9,18 +9,9 @@ import pytest
 
 import orc as O
 import refstack as R
+from engine_util import eng  # noqa: F401
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(300)]
-
-
-@pytest.fixture(scope="module")
-def eng():
-    import __graft_entry__ as g
-    g.build()
-    import apus_b200
-    if apus_b200.lib().apus_device_count() < 1:
-        pytest.fail("no CUDA device visible on a gpu-marked test")
-    return apus_b200
 
 
 @pytest.mark.parametrize("n,nconn,nreq,plen", [(3, 2, 300, 64), (5, 3, 200, 128), (3, 1, 120, -3000), (7, 4, 400, 64)])
