@@ -6,6 +6,7 @@
  *   pack     apus_submit_device / apus_submit_device_packed: sizes, scan and pack passes, then the doorbell (bell)
  *   consume  apus_consume_device / apus_consume_device_packed: head, count, scan, copy and tail
  *   wait     apus_consume_wait: one warp between consume calls, until enough entries are committed past the cursor
+ *   mark     apus_consume_mark: one thread writes the consumer position, for a snapshot of the application's state
  *
  * apus_engine.cu checks the arguments, accounts ring space, and brackets each enqueue below in the caller's stream
  * order.  The batch layouts are apus_layout.h; the slot format is apus_slot.h; the device helpers shared with the
@@ -581,6 +582,18 @@ __global__ void apus_consume_wait_kernel(const apus_ctrl_t *ctrl, apus_hostwords
 }
 
 // ---------------------------------------------------------------------------------
+// CONSUME MARKS (apus_consume_mark): one thread on the consume stream writes the consumer position {cursor offset, idx
+// of the next entry} as the consume calls before it left it, into a 16 B device word of the caller's.  A copy of the
+// application's state enqueued behind the mark in stream order is the state at that position.  A consumer stopped for
+// good (APUS_CONSUME_BAD_IDX) marks next idx 0, which no seed accepts.  It writes nothing the replica kernels read.
+// ---------------------------------------------------------------------------------
+__global__ void apus_consume_mark_kernel(const apus_ctrl_t *ctrl, const apus_cons_state_t *st, uint64_t *mark)
+{
+    const uint64_t cursor = ld_relaxed_sys(&ctrl->cons_cur[0]), nidx = ld_relaxed_sys(&ctrl->cons_cur[1]);
+    *reinterpret_cast<ulonglong2 *>(mark) = make_ulonglong2(cursor, st->error ? 0ull : nidx);
+}
+
+// ---------------------------------------------------------------------------------
 // host side: loading and enqueueing (apus_engine.cu brackets each enqueue in the caller's stream order)
 // ---------------------------------------------------------------------------------
 // These kernels run while the replica kernels are resident.  Under lazy module loading (CUDA_MODULE_LOADING=LAZY, the
@@ -601,6 +614,7 @@ extern "C" cudaError_t apus_batch_load(void)
     if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, apus_consume_copy_kernel);
     if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, apus_consume_tail_kernel);
     if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, apus_consume_wait_kernel);
+    if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, apus_consume_mark_kernel);
     return e;
 }
 
@@ -650,5 +664,12 @@ extern "C" cudaError_t apus_consume_wait_enqueue(const uint8_t *region, apus_hos
 {
     apus_consume_wait_kernel<<<1, 32, 0, stream>>>(reinterpret_cast<const apus_ctrl_t *>(region), hw, epoch, min_entries,
                                                    timeout_ns, outcome);
+    return cudaGetLastError();
+}
+
+extern "C" cudaError_t apus_consume_mark_enqueue(const uint8_t *region, const apus_cons_state_t *st, uint64_t *mark,
+                                                 cudaStream_t stream)
+{
+    apus_consume_mark_kernel<<<1, 1, 0, stream>>>(reinterpret_cast<const apus_ctrl_t *>(region), st, mark);
     return cudaGetLastError();
 }

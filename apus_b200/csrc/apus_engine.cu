@@ -40,6 +40,8 @@ extern "C" cudaError_t apus_consume_enqueue(const apus_consume_args_t *a, cudaSt
 extern "C" cudaError_t apus_consume_wait_enqueue(const uint8_t *region, apus_hostwords_t *hw, uint64_t epoch,
                                                  uint32_t min_entries, uint64_t timeout_ns, uint32_t *outcome,
                                                  cudaStream_t stream);
+extern "C" cudaError_t apus_consume_mark_enqueue(const uint8_t *region, const apus_cons_state_t *st, uint64_t *mark,
+                                                 cudaStream_t stream);
 
 #define MAX_ROLES 160          /* CTAs of one fused launch: leader workers + local followers */
 static __thread char g_err[512];
@@ -189,6 +191,7 @@ struct apus_replica {
     cudaEvent_t ev_cons[2];       /* caller's stream -> cons_stream -> caller's stream */
     apus_cons_state_t *cons_st;   /* consume state + APUS_CONS_BLK_WORDS per consume block (index-ring capacity / block size) */
     pthread_mutex_t cons_mu;      /* one enqueue at a time: the two events are shared by every caller */
+    uint64_t cons_enqueued;       /* consume, wait and mark enqueues so far (under cons_mu): a seed needs none */
 };
 
 extern "C" int apus_abi_version(void) { return APUS_ABI_VERSION; }
@@ -1248,6 +1251,7 @@ static int consume_enqueue(apus_replica_t *r, apus_consume_args_t a, uint32_t ma
     a.st = r->cons_st; a.hw = r->hw_dev;
     DeviceGuard g(r->cfg.device);
     StageLock sl(&r->cons_mu);
+    r->cons_enqueued++;
     return side_stream_run((cudaStream_t)stream, r->cons_stream, r->ev_cons, "apus_consume_enqueue",
                            [&] { return apus_consume_enqueue(&a, r->cons_stream); });
 }
@@ -1326,6 +1330,7 @@ extern "C" int apus_consume_wait(apus_replica_t *r, uint32_t min_entries, uint32
     StageLock sl(&r->cons_mu);
     /* the epoch is read under cons_mu, in the order of the enqueues: a release after this call ends this wait */
     const uint64_t epoch = r->hw->cons_wait_epoch;
+    r->cons_enqueued++;
     return side_stream_run((cudaStream_t)stream, r->cons_stream, r->ev_cons, "apus_consume_wait_enqueue", [&] {
         return apus_consume_wait_enqueue(r->region, r->hw_dev, epoch, min_entries, 1000ull * timeout_us, outcome,
                                          r->cons_stream);
@@ -1349,6 +1354,21 @@ extern "C" int apus_consume_wait_status(apus_replica_t *r, uint64_t *outcome, ui
     if (outcome) *outcome = r->hw->cons_wait_outcome;
     if (available) *available = r->hw->cons_wait_avail;
     return APUS_OK;
+}
+
+extern "C" int apus_consume_mark(apus_replica_t *r, uint64_t *mark, void *stream)
+{
+    if (!r) return fail("null argument");
+    if (is_leader(r) && !(r->cfg.flags & APUS_F_APPLY_ANY_ROLE))
+        return fail("apus_consume_mark: consumption is a follower's (the leader's log is its own)");
+    if (!(r->cfg.flags & APUS_F_DEVICE_APPLY)) return fail("apus_consume_mark needs a replica created with APUS_F_DEVICE_APPLY");
+    if (!mark) return fail("null argument");
+    if ((uintptr_t)mark & 15u) return fail("apus_consume_mark: misaligned mark (16 B)");
+    DeviceGuard g(r->cfg.device);
+    StageLock sl(&r->cons_mu);
+    r->cons_enqueued++;
+    return side_stream_run((cudaStream_t)stream, r->cons_stream, r->ev_cons, "apus_consume_mark_enqueue",
+                           [&] { return apus_consume_mark_enqueue(r->region, r->cons_st, mark, r->cons_stream); });
 }
 
 extern "C" uint64_t apus_leader_suspect(apus_replica_t *r) { return r ? r->hw->leader_suspect : 0; }
@@ -1637,6 +1657,69 @@ static int copy_to_peer(apus_replica *r, uint8_t peer, size_t off, size_t len)
     return APUS_OK;
 }
 
+extern "C" int apus_consume_seed(apus_replica_t *r, uint64_t cursor_offset, uint64_t next_idx)
+{
+    if (!r) return fail("null argument");
+    const uint32_t need = APUS_F_DEVICE_APPLY | APUS_F_APPLY_ANY_ROLE;
+    if ((r->cfg.flags & need) != need)
+        return fail("apus_consume_seed needs a replica created with APUS_F_DEVICE_APPLY | APUS_F_APPLY_ANY_ROLE");
+    if (is_leader(r)) return fail("apus_consume_seed: a leader's consumers stand on its own log");
+    if (r->in_flight) return fail("apus_consume_seed: stop the kernel first");
+    if (cursor_offset >= r->log_len || next_idx == 0)
+        return fail("apus_consume_seed: cursor %llu outside the log of %llu B, or next idx 0", (unsigned long long)cursor_offset,
+                    (unsigned long long)r->log_len);
+    DeviceGuard g(r->cfg.device);
+    StageLock cl(&r->cons_mu);
+    apus_loghdr_t h; apus_ctrl_t c;
+    if (own_read(r, APUS_HDR_OFF, &h, sizeof h) != APUS_OK || own_read(r, 0, &c, sizeof c) != APUS_OK) return APUS_ERROR;
+    if (h.end != r->log_len || c.acked != 0) return fail("apus_consume_seed: the replica holds entries (its log must be empty)");
+    if (r->cons_enqueued) return fail("apus_consume_seed: consume work has been enqueued on this replica");
+    if (c.cons_cur[0] != 0 || c.cons_cur[1] != 1) return fail("apus_consume_seed: the consumers have moved");
+    /* the record names the seed and nothing past it: no entry is held until the leader's adjustment resends them */
+    c.cons_rec[0] = cursor_offset; c.cons_rec[1] = next_idx - 1;
+    c.cons_cur[0] = cursor_offset; c.cons_cur[1] = next_idx;
+    c.cons_seeded = 1;
+    const size_t from = offsetof(apus_ctrl_t, cons_rec), to = offsetof(apus_ctrl_t, cons_seeded) + 8;
+    if (own_write(r, from, (const uint8_t *)&c + from, to - from) != APUS_OK) return APUS_ERROR;
+    r->hw->cons_cursor = cursor_offset;
+    r->hw->cons_next_idx = next_idx;
+    return APUS_OK;
+}
+
+/* the idx of the entry that starts at my head: my next idx when my log is empty or my head is my end, 0 when no entry
+ * of mine starts there */
+static int head_idx(apus_replica *r, const apus_loghdr_t &mh, uint64_t mine, uint64_t *hidx)
+{
+    *hidx = 0;
+    if (mh.end == r->log_len || mh.head == mh.end) { *hidx = mine + 1; return APUS_OK; }
+    uint8_t eh[8];
+    uint64_t v, o, i2, t2; uint32_t s2;
+    if (own_read(r, r->entries_off + mh.head + E_IDX, eh, 8) != APUS_OK) return APUS_ERROR;
+    memcpy(&v, eh, 8);
+    if (v == 0 || v > mine || entry_at(r, -1, v, &o, &i2, &t2, &s2) != APUS_OK || o != mh.head || i2 != v) return APUS_OK;
+    *hidx = v;
+    return APUS_OK;
+}
+
+/* Whether {cur, nidx} inside [head, commit] of my log is a position my consumers can stand at: the one the consume tail
+ * kernel leaves behind entry nidx - 1, its end (0 for an entry that ends at the ring's end).  So entry nidx starts at
+ * cur; or entry nidx starts at 0 behind a wrap gap that begins at cur, where entry nidx - 1 ends; or no entry past cur
+ * is committed: cur is my commit offset and nidx is one past my committed entries. */
+static int consumer_boundary(apus_replica *r, uint64_t cur, uint64_t nidx, uint64_t commit, uint64_t committed, bool *ok)
+{
+    *ok = false;
+    if (cur == commit && nidx == committed + 1) { *ok = true; return APUS_OK; }
+    if (nidx > committed) return APUS_OK;
+    uint64_t o, i, t; uint32_t s;
+    if (entry_at(r, -1, nidx, &o, &i, &t, &s) != APUS_OK) return APUS_ERROR;
+    if (i != nidx) return APUS_OK;
+    if (o == cur) { *ok = true; return APUS_OK; }
+    if (o != 0 || nidx < 2) return APUS_OK;
+    if (entry_at(r, -1, nidx - 1, &o, &i, &t, &s) != APUS_OK) return APUS_ERROR;
+    *ok = i == nidx - 1 && o + s == cur;
+    return APUS_OK;
+}
+
 extern "C" int apus_ctl_adjust_follower(apus_replica_t *r, uint8_t peer, uint64_t sid, uint64_t *resent)
 {
     if (!r || peer >= r->cfg.group_size || peer == r->cfg.server_idx) return fail("bad argument");
@@ -1666,9 +1749,9 @@ extern "C" int apus_ctl_adjust_follower(apus_replica_t *r, uint8_t peer, uint64_
     /* a peer whose device consumers run in any role (cons_on == 2): nothing they have read, or may read on their
      * current record, is rewritten -- checked before anything is written */
     uint64_t rec[2] = { fc.cons_rec[0], fc.cons_rec[1] };
-    bool rewrite_rec = false;
+    bool rewrite_rec = false, seeded = false;
+    const uint64_t cur = fc.cons_cur[0], nidx = fc.cons_cur[1];
     if (fc.cons_on) {
-        const uint64_t cur = fc.cons_cur[0], nidx = fc.cons_cur[1];
         if (j > 0) {
             if (nidx - 1 > j || ring_dist_h(cur, rec[0], L) > ring_dist_h(cur, keep_end, L))
                 return fail("peer %u: its device consumers have read, or may read, past the last entry it shares with me "
@@ -1676,19 +1759,33 @@ extern "C" int apus_ctl_adjust_follower(apus_replica_t *r, uint8_t peer, uint64_
                             (unsigned long long)nidx);
             /* entries past what it holds after the resend have stale index words: the record may not name them */
             if (rec[1] > mine) { rec[1] = mine; rewrite_rec = true; }
-        } else {
-            /* it shares nothing with me: its consumers can go on only from my head (joining a device consumer needs a
-             * snapshot of its device state) */
-            uint64_t hidx = 0;
-            if (mh.end == L || mh.head == mh.end) hidx = mine + 1;
-            else {
-                uint8_t eh[8];
-                uint64_t o, i2, t2; uint32_t s2;
-                if (own_read(r, r->entries_off + mh.head + E_IDX, eh, 8) != APUS_OK) return APUS_ERROR;
-                memcpy(&hidx, eh, 8);
-                if (hidx == 0 || hidx > mine || entry_at(r, -1, hidx, &o, &i2, &t2, &s2) != APUS_OK || o != mh.head || i2 != hidx)
-                    hidx = 0;                                                     /* no entry of mine starts at my head */
+        } else if (fc.cons_seeded && fh.end == L && fc.acked == 0) {
+            /* a replacement whose consumers were seeded at the mark of a snapshot of some consumer's state
+             * (apus_consume_seed): it goes on from there if that position is one of my consumer positions in
+             * [head, commit].  A mark behind my head belongs to a snapshot older than my live log: take a newer one */
+            uint64_t hidx;
+            if (head_idx(r, mh, mine, &hidx) != APUS_OK) return APUS_ERROR;
+            if (nidx < hidx) {
+                snprintf(g_err, sizeof g_err, "peer %u was seeded at next idx %llu, behind my head (idx %llu): its snapshot "
+                         "is older than my log, seed it from a newer one", (unsigned)peer, (unsigned long long)nidx,
+                         (unsigned long long)hidx);
+                return APUS_RETRY;
             }
+            if (nidx > mc.committed + 1 || ring_dist_h(mh.head, cur, L) > ring_dist_h(mh.head, mh.commit, L))
+                return fail("peer %u was seeded at offset %llu, next idx %llu, past my commit (offset %llu, %llu entries) "
+                            "or outside my log: no log adjustment", (unsigned)peer, (unsigned long long)cur,
+                            (unsigned long long)nidx, (unsigned long long)mh.commit, (unsigned long long)mc.committed);
+            bool ok;
+            if (consumer_boundary(r, cur, nidx, mh.commit, mc.committed, &ok) != APUS_OK) return APUS_ERROR;
+            if (!ok)
+                return fail("peer %u was seeded at offset %llu, next idx %llu: no consumer of my log stands there (entry "
+                            "%llu does not start there, nor behind a wrap gap there): no log adjustment", (unsigned)peer,
+                            (unsigned long long)cur, (unsigned long long)nidx, (unsigned long long)nidx);
+            rec[0] = cur; rec[1] = nidx - 1; rewrite_rec = true; seeded = true;
+        } else {
+            /* it shares nothing with me and was not seeded: its consumers can go on only from my head */
+            uint64_t hidx;
+            if (head_idx(r, mh, mine, &hidx) != APUS_OK) return APUS_ERROR;
             if (cur != mh.head || nidx != hidx)
                 return fail("peer %u shares no entry with me and its device consumers stand at offset %llu, next idx %llu, "
                             "not at my head (offset %llu, idx %llu): no log adjustment", (unsigned)peer,
@@ -1738,6 +1835,9 @@ extern "C" int apus_ctl_adjust_follower(apus_replica_t *r, uint8_t peer, uint64_
     const uint64_t pc[2] = { mh.commit, r->cfg.term };
     if (peer_write(r, peer, offsetof(apus_ctrl_t, pub_commit), pc, 16) != APUS_OK) return APUS_ERROR;
     if (own_write(r, offsetof(apus_ctrl_t, ack) + 8u * peer, &mine, 8) != APUS_OK) return APUS_ERROR;
+    /* a seeded replacement's apply offset is its seed: the word still holds the lost replica's, which the pruning rule
+     * would read until the replacement's kernel reports its own */
+    if (seeded && own_write(r, offsetof(apus_ctrl_t, apply_off) + 8u * peer, &cur, 8) != APUS_OK) return APUS_ERROR;
     const uint64_t adj[3] = { sid, mh.end, mine };
     if (peer_write(r, peer, APUS_CTL_OFF + offsetof(apus_ctlwords_t, adj_end), &adj[1], 16) != APUS_OK) return APUS_ERROR;
     if (peer_write(r, peer, APUS_CTL_OFF + offsetof(apus_ctlwords_t, leader_sid), &adj[0], 8) != APUS_OK) return APUS_ERROR;

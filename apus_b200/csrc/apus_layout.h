@@ -125,7 +125,9 @@ typedef struct apus_ctrl {
                                     the apply offset the follower reports to the leader's pruning rule */
     uint64_t cons_on;            /* 1: this replica was created with APUS_F_DEVICE_APPLY (the control plane refuses it);
                                     2: ... with APUS_F_APPLY_ANY_ROLE too (log adjustment guards its consumers) */
-    uint64_t pad4[11];
+    uint64_t cons_seeded;        /* 1: apus_consume_seed started the consumers on an empty log at a snapshot's mark, and
+                                    a leader's adjustment may accept this replica from there; host-written only */
+    uint64_t pad4[10];
 } apus_ctrl_t;
 
 /* Control-plane words (N1: election, votes, log adjustment), at APUS_CTL_OFF inside the ctrl block -- the part of the

@@ -73,6 +73,7 @@ EXPORTS = [
     "apus_submit_device", "apus_device_submit_status", "apus_stream_wait_committed", "apus_committed_word",
     "apus_consume_device", "apus_consume_status", "apus_submit_device_packed", "apus_consume_device_packed",
     "apus_consume_wait", "apus_consume_wait_release", "apus_consume_wait_status",
+    "apus_consume_mark", "apus_consume_seed",
 ]
 
 
@@ -137,6 +138,8 @@ def load_library(path=LIB_PATH):
         L.apus_consume_wait.argtypes = [vp, u32, u32, vp, vp]
         L.apus_consume_wait_release.argtypes = [vp]
         L.apus_consume_wait_status.argtypes = [vp, C.POINTER(u64), C.POINTER(u64)]
+        L.apus_consume_mark.argtypes = [vp, vp, vp]
+        L.apus_consume_seed.argtypes = [vp, u64, u64]
     _lib = L
     return L
 
@@ -455,6 +458,38 @@ class Replica:
         o, a = u64(), u64()
         _ck(lib().apus_consume_wait_status(self.h, C.byref(o), C.byref(a)), "apus_consume_wait_status")
         return WaitStatus(int(o.value), int(a.value))
+
+    def consume_mark(self, out=None, stream=None):
+        """Write the consumers' position {cursor offset, idx of the next entry}, as the consume calls before it left it,
+        into a 2-word device tensor in `stream` order (apus_consume_mark), in the roles consume_device accepts.  A copy
+        of the application's state enqueued on `stream` right behind it is the state at that position: seed a
+        replacement replica with consume_seed(*mark) and give it the copy.  Next idx 0 marks a consumer stopped by
+        CONSUME_BAD_IDX.  `out`: an int64 or uint64 CUDA tensor [2] on this replica's device, 16 B aligned (allocated when
+        None); returned."""
+        import torch
+        dev = torch.device("cuda", self.device)
+        s = self._stream(stream)
+        if out is None:
+            with torch.cuda.stream(s):
+                out = torch.empty(2, dtype=torch.int64, device=dev)
+        if not isinstance(out, torch.Tensor):
+            raise ApusError("consume_mark: out must be a torch tensor")
+        if out.device != dev:
+            raise ApusError(f"consume_mark: out is on {out.device}, the replica is on {dev}")
+        if out.dtype not in (torch.int64, torch.uint64):
+            raise ApusError(f"consume_mark: out has dtype {out.dtype}, expected one of {(torch.int64, torch.uint64)}")
+        if tuple(out.shape) != (2,):
+            raise ApusError(f"consume_mark: out has shape {tuple(out.shape)}, expected (2,)")
+        if not out.is_contiguous():
+            raise ApusError("consume_mark: out is not contiguous")
+        _ck(lib().apus_consume_mark(self.h, out.data_ptr(), s.cuda_stream), "apus_consume_mark")
+        return out
+
+    def consume_seed(self, cursor, next_idx):
+        """Start the consumers of a fresh follower (F_DEVICE_APPLY | F_APPLY_ANY_ROLE, stopped, empty log, no consume call
+        yet) at a mark another replica's consume_mark wrote (apus_consume_seed); the leader's adjustment then accepts
+        it from there"""
+        _ck(lib().apus_consume_seed(self.h, int(cursor), int(next_idx)), "apus_consume_seed")
 
     def wait_committed_on_stream(self, ticket, stream=None):
         """make `stream` (default: the current stream of the leader's device) wait until `ticket` is committed"""

@@ -363,6 +363,30 @@ int  apus_consume_wait_release(apus_replica_t *r);
 /* the pinned words the latest consume wait that ran wrote: its APUS_WAIT_* outcome (UINT64_MAX before any wait has
  * run) and the committed entries past the cursor when it ended */
 int  apus_consume_wait_status(apus_replica_t *r, uint64_t *outcome, uint64_t *available);
+/* Snapshots of device consumers: what replaces a lost replica of a group that applies in GPU memory.  The application
+ * owns its state and copies it (device to device, CUDA IPC, or through the host); the engine names the log position
+ * that state corresponds to, and starts a replacement's consumers there.
+ * apus_consume_mark writes the consumer position {cursor offset, idx of the next entry}, as the consume calls enqueued
+ * before it left it, into `mark`: 16 B of device memory on the replica's GPU, 16 B aligned.  `stream` is a cudaStream_t
+ * (NULL = the legacy default stream), ordered exactly as for apus_consume_wait: the mark runs on the consume stream in
+ * call order with the consume calls, after everything enqueued on `stream` before the call, and `stream` waits for it.
+ * So a copy of the state enqueued on `stream` right behind the mark is the state at the marked position, and the group
+ * keeps running while it is taken.  A consumer stopped for good by APUS_CONSUME_BAD_IDX marks next idx 0, which no seed
+ * accepts.  The mark writes nothing the replica kernels read.  APUS_ERROR, with nothing enqueued, where the consume
+ * calls refuse the replica and for a null or misaligned `mark`. */
+int  apus_consume_mark(apus_replica_t *r, uint64_t *mark, void *stream);
+/* Start the consumers of a replacement at a mark: cursor and next idx := the mark, and the consumer record names
+ * nothing held past it (apus_consume_status reports the seed at once).  The leader's apus_ctl_adjust_follower then
+ * accepts this replica, although it shares no entry, if the mark is a consumer position of the leader's log between its
+ * head and its commit: the offset where entry next_idx starts, or where the wrap gap before it starts, or the commit
+ * offset with next_idx one past the committed entries.  The adjustment resends the live log, and the leader counts the
+ * seed as the replacement's apply offset in its pruning rule until the replacement's kernel reports its own; it returns
+ * APUS_RETRY, with nothing written, for a mark behind the leader's head (the snapshot is older than the live log: take a
+ * newer one), and APUS_ERROR, with nothing written, for a mark past its commit or at no consumer position.  APUS_ERROR,
+ * with nothing written, unless the replica was created with APUS_F_DEVICE_APPLY | APUS_F_APPLY_ANY_ROLE, is a follower
+ * whose kernel is stopped, holds no entry (empty log, nothing acked), has had no consume call, wait or mark enqueued,
+ * and unless cursor_offset < the log size and next_idx >= 1. */
+int  apus_consume_seed(apus_replica_t *r, uint64_t cursor_offset, uint64_t next_idx);
 /* failure detector: 0 while the leader's heartbeats arrive, else 1 + the term whose leader fell silent */
 uint64_t apus_leader_suspect(apus_replica_t *follower);
 /* %globaltimer (ns) of the leader kernel's latest commit (device clock; step timing of resident kernels) */
@@ -400,7 +424,8 @@ int  apus_ctl_last_entry(apus_replica_t *r, uint64_t *idx, uint64_t *term, uint6
  * offset index) peer to peer, and tell it to follow `sid` from there.  *resent = bytes copied.  A peer whose device
  * consumers run in any role (APUS_F_APPLY_ANY_ROLE) is refused, with nothing written, when its consumers have read
  * past the last entry it shares with me, or when it shares nothing with me and its consumers do not stand exactly at
- * my head; its consumer record is left naming no entry beyond what its offset index holds after the resend. */
+ * my head -- unless they were seeded at a snapshot's mark (apus_consume_seed, which says when such a peer is accepted);
+ * its consumer record is left naming no entry beyond what its offset index holds after the resend. */
 int  apus_ctl_adjust_follower(apus_replica_t *leader, uint8_t peer_idx, uint64_t sid, uint64_t *resent);
 /* role and term for the next launch.  Becoming leader takes over the log as this replica holds it (entry counters,
  * tail, submission ring); becoming follower adopts what the new leader's adjustment left (apus_ctl_view.adj_*).  With
