@@ -7,6 +7,7 @@
  *   consume  apus_consume_device / apus_consume_device_packed: head, count, scan, copy and tail
  *   wait     apus_consume_wait: one warp between consume calls, until enough entries are committed past the cursor
  *   mark     apus_consume_mark: one thread writes the consumer position, for a snapshot of the application's state
+ *   fence    apus_read_fence: one warp until this replica's state can answer a linearizable read (apus_fence.h)
  *
  * apus_engine.cu checks the arguments, accounts ring space, and brackets each enqueue below in the caller's stream
  * order.  The batch layouts are apus_layout.h; the slot format is apus_slot.h; the device helpers shared with the
@@ -19,6 +20,7 @@
 #include "apus_layout.h"
 #include "apus_slot.h"
 #include "apus_dev.h"
+#include "apus_fence.h"
 
 // ---------------------------------------------------------------------------------
 // block scans: the packing and the consume kernels run blocks of the same size
@@ -555,6 +557,24 @@ __device__ __forceinline__ uint64_t globaltimer_ns()
     return t;
 }
 
+// one step between two polls of a stream-ordered wait (consume waits, read fences), started at t0 on %globaltimer: the
+// release epoch every APUS_WAIT_RELEASE_POLL_NS (t_rel: when it was read last), the deadline, then a back-off sleep
+// (`sleep` doubles up to APUS_WAIT_SLEEP_MAX_NS).  true: the wait ends, with APUS_WAIT_RELEASED or APUS_WAIT_TIMED_OUT
+// in `why`.
+__device__ __forceinline__ bool wait_backoff(const apus_hostwords_t *hw, uint64_t epoch, uint64_t t0, uint64_t timeout_ns,
+                                             uint64_t &t_rel, uint32_t &sleep, uint32_t &why)
+{
+    const uint64_t now = globaltimer_ns();
+    if (now - t_rel >= APUS_WAIT_RELEASE_POLL_NS) {
+        t_rel = now;
+        if (ld_relaxed_sys(&hw->cons_wait_epoch) != epoch) { why = APUS_WAIT_RELEASED; return true; }
+    }
+    if (now - t0 >= timeout_ns) { why = APUS_WAIT_TIMED_OUT; return true; }
+    __nanosleep(sleep);
+    if (sleep < APUS_WAIT_SLEEP_MAX_NS) sleep <<= 1;
+    return false;
+}
+
 __global__ void apus_consume_wait_kernel(const apus_ctrl_t *ctrl, apus_hostwords_t *hw, uint64_t epoch,
                                          uint32_t min_entries, uint64_t timeout_ns, uint32_t *outcome)
 {
@@ -567,14 +587,7 @@ __global__ void apus_consume_wait_kernel(const apus_ctrl_t *ctrl, apus_hostwords
         cons_read(ctrl, committed, held);
         avail = cons_avail(held, ld_relaxed_sys(&ctrl->cons_cur[1]));
         if (avail >= min_entries) { why = APUS_WAIT_READY; break; }
-        const uint64_t now = globaltimer_ns();
-        if (now - t_rel >= APUS_WAIT_RELEASE_POLL_NS) {
-            t_rel = now;
-            if (ld_relaxed_sys(&hw->cons_wait_epoch) != epoch) { why = APUS_WAIT_RELEASED; break; }
-        }
-        if (now - t0 >= timeout_ns) { why = APUS_WAIT_TIMED_OUT; break; }
-        __nanosleep(sleep);
-        if (sleep < APUS_WAIT_SLEEP_MAX_NS) sleep <<= 1;
+        if (wait_backoff(hw, epoch, t0, timeout_ns, t_rel, sleep, why)) break;
     }
     if (outcome) *(volatile uint32_t *)outcome = why;
     st_relaxed_sys(&hw->cons_wait_outcome, why);
@@ -591,6 +604,65 @@ __global__ void apus_consume_mark_kernel(const apus_ctrl_t *ctrl, const apus_con
 {
     const uint64_t cursor = ld_relaxed_sys(&ctrl->cons_cur[0]), nidx = ld_relaxed_sys(&ctrl->cons_cur[1]);
     *reinterpret_cast<ulonglong2 *>(mark) = make_ulonglong2(cursor, st->error ? 0ull : nidx);
+}
+
+// ---------------------------------------------------------------------------------
+// READ FENCES (apus_read_fence): one warp on the consume stream; lane 0 takes the three steps of apus_fence.h.
+//   1. K: the entries-committed word of the leader's consumer record (cons_read's acquire), which its commit warp
+//      publishes only under APUS_F_APPLY_ANY_ROLE (cons_on == 2); otherwise, or with the leader not mapped, NOT_LEADER.
+//   2. after K (the acquire orders the loads below after it): the SID word of every member this replica maps; fewer
+//      than N/2 + 1 at term <= t ends NOT_LEADER (rf_confirmed).
+//   3. this replica's own record, polled as a consume wait polls (wait_backoff) until rf_ready: held >= K, and the
+//      entry the offset index names for idx `held` carries idx `held` (else it is another lap's: poll again) and a term
+//      >= t.  The header is read idx, term, idx, so that a term torn from an entry of a later lap is not taken.
+// F = held.  N + 2 loads of other replicas' words (the leader's cons_on and record, the SIDs), one local poll.  It
+// writes the caller's index (READY only) and outcome words and two pinned status words, nothing the replica kernels read.
+// ---------------------------------------------------------------------------------
+__global__ void apus_read_fence_kernel(apus_fence_args_t a)
+{
+    if (threadIdx.x != 0) return;
+    const uint64_t t0 = globaltimer_ns();
+    uint64_t F = 0;
+    uint32_t why = APUS_WAIT_NOT_LEADER;
+    const apus_ctrl_t *lead = NULL;
+#pragma unroll
+    for (uint32_t i = 0; i < APUS_MAX_SERVERS; i++)
+        if (i == a.leader) lead = reinterpret_cast<const apus_ctrl_t *>(a.member[i]);
+    if (lead && ld_relaxed_sys(&lead->cons_on) == 2) {
+        uint64_t k_off, K;
+        cons_read(lead, k_off, K);
+        uint32_t counted = 0;
+#pragma unroll
+        for (uint32_t i = 0; i < APUS_MAX_SERVERS; i++)
+            if (i < a.n && a.member[i])
+                counted += rf_member_counts(1, ld_relaxed_sys(a.member[i] + APUS_CTL_OFF + offsetof(apus_ctlwords_t, sid)),
+                                            a.term);
+        if (rf_confirmed(counted, a.n)) {
+            const apus_ctrl_t *own = reinterpret_cast<const apus_ctrl_t *>(a.region);
+            const uint32_t *index = reinterpret_cast<const uint32_t *>(a.region + APUS_INDEX_OFF);
+            const uint8_t *entries = a.region + a.entries_off;
+            uint64_t t_rel = t0;
+            uint32_t sleep = APUS_WAIT_SLEEP_MIN_NS;
+            for (;;) {
+                uint64_t held_off, held, e_idx = 0, e_term = 0;
+                cons_read(own, held_off, held);
+                if (held && held >= K) {
+                    const uint64_t off = ld_relaxed_sys_u32(&index[(uint32_t)held & a.idx_mask]) & ~APUS_IDX_HEAD_FLAG;
+                    if (off + APUS_HDR_BYTES <= a.log_len) {
+                        e_idx = ld_relaxed_sys_u64_any(entries, off + E_IDX);
+                        e_term = ld_relaxed_sys_u64_any(entries, off + E_TERM);
+                        if (ld_relaxed_sys_u64_any(entries, off + E_IDX) != e_idx) e_idx = 0;
+                    }
+                }
+                if (rf_ready(held, K, e_idx, e_term, a.term)) { F = held; why = APUS_WAIT_READY; break; }
+                if (wait_backoff(a.hw, a.epoch, t0, a.timeout_ns, t_rel, sleep, why)) break;
+            }
+        }
+    }
+    if (why == APUS_WAIT_READY) *(volatile uint64_t *)a.index = F;
+    if (a.outcome) *(volatile uint32_t *)a.outcome = why;
+    st_relaxed_sys(&a.hw->fence_outcome, why);
+    st_relaxed_sys(&a.hw->fence_index, F);
 }
 
 // ---------------------------------------------------------------------------------
@@ -615,6 +687,7 @@ extern "C" cudaError_t apus_batch_load(void)
     if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, apus_consume_tail_kernel);
     if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, apus_consume_wait_kernel);
     if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, apus_consume_mark_kernel);
+    if (e == cudaSuccess) e = cudaFuncGetAttributes(&fa, apus_read_fence_kernel);
     return e;
 }
 
@@ -671,5 +744,11 @@ extern "C" cudaError_t apus_consume_mark_enqueue(const uint8_t *region, const ap
                                                  cudaStream_t stream)
 {
     apus_consume_mark_kernel<<<1, 1, 0, stream>>>(reinterpret_cast<const apus_ctrl_t *>(region), st, mark);
+    return cudaGetLastError();
+}
+
+extern "C" cudaError_t apus_read_fence_enqueue(const apus_fence_args_t *a, cudaStream_t stream)
+{
+    apus_read_fence_kernel<<<1, 32, 0, stream>>>(*a);
     return cudaGetLastError();
 }

@@ -40,6 +40,7 @@ extern "C" cudaError_t apus_consume_enqueue(const apus_consume_args_t *a, cudaSt
 extern "C" cudaError_t apus_consume_wait_enqueue(const uint8_t *region, apus_hostwords_t *hw, uint64_t epoch,
                                                  uint32_t min_entries, uint64_t timeout_ns, uint32_t *outcome,
                                                  cudaStream_t stream);
+extern "C" cudaError_t apus_read_fence_enqueue(const apus_fence_args_t *a, cudaStream_t stream);
 extern "C" cudaError_t apus_consume_mark_enqueue(const uint8_t *region, const apus_cons_state_t *st, uint64_t *mark,
                                                  cudaStream_t stream);
 
@@ -189,10 +190,19 @@ struct apus_replica {
      * copy_stream never queue behind them */
     cudaStream_t cons_stream;
     cudaEvent_t ev_cons[2];       /* caller's stream -> cons_stream -> caller's stream */
+    cudaEvent_t ev_fence;         /* recorded on cons_stream right behind the latest read fence (under cons_mu) */
+    uint64_t fences;              /* read fences enqueued so far (under cons_mu) */
     apus_cons_state_t *cons_st;   /* consume state + APUS_CONS_BLK_WORDS per consume block (index-ring capacity / block size) */
     pthread_mutex_t cons_mu;      /* one enqueue at a time: the two events are shared by every caller */
     uint64_t cons_enqueued;       /* consume, wait and mark enqueues so far (under cons_mu): a seed needs none */
+    apus_replica *live_next;      /* the process's live replicas (g_live, under g_live_mu) */
 };
+
+/* Every live replica of this process, for the read fences: a fence reads the regions of the peers its replica maps, so
+ * apus_replica_destroy(p) unmaps p from every replica that maps it and waits for their pending fences before p's region
+ * is freed.  It and apus_read_fence hold g_live_mu while they do so (lock order: g_live_mu, then a replica's cons_mu). */
+static pthread_mutex_t g_live_mu = PTHREAD_MUTEX_INITIALIZER;
+static apus_replica *g_live = NULL;
 
 extern "C" int apus_abi_version(void) { return APUS_ABI_VERSION; }
 extern "C" const char *apus_last_error(void) { return g_err; }
@@ -289,6 +299,7 @@ static int replica_init(apus_replica *r, const apus_config_t *cfg, uint64_t log_
         pthread_mutex_init(&r->cons_mu, NULL);
         CK(cudaStreamCreateWithFlags(&r->cons_stream, cudaStreamNonBlocking));
         for (cudaEvent_t &e : r->ev_cons) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+        CK(cudaEventCreateWithFlags(&r->ev_fence, cudaEventDisableTiming));
         const size_t sb = sizeof(apus_cons_state_t) + 8ull * APUS_CONS_BLK_WORDS * ((cap + APUS_CONS_THREADS - 1) / APUS_CONS_THREADS);
         CK(cudaMalloc(&r->cons_st, sb));
         CK(cudaMemset(r->cons_st, 0, sb));
@@ -299,6 +310,7 @@ static int replica_init(apus_replica *r, const apus_config_t *cfg, uint64_t log_
     CK(cudaHostAlloc(&r->hw, sizeof(apus_hostwords_t), cudaHostAllocMapped | cudaHostAllocPortable));
     memset((void *)r->hw, 0, sizeof(apus_hostwords_t));
     r->hw->cons_wait_outcome = ~0ull;                                  /* no consume wait has run */
+    r->hw->fence_outcome = ~0ull;                                      /* no read fence has run */
     CK(cudaHostGetDevicePointer(&r->hw_dev, r->hw, 0));
     pthread_mutex_init(&r->stage_mu, NULL);
     r->stage_bytes = 1u << 20;
@@ -369,6 +381,10 @@ extern "C" int apus_replica_create(const apus_config_t *cfg, apus_replica_t **ou
         memcpy(g_err, keep, sizeof keep);
         return APUS_ERROR;
     }
+    pthread_mutex_lock(&g_live_mu);
+    r->live_next = g_live;
+    g_live = r;
+    pthread_mutex_unlock(&g_live_mu);
     *out = r;
     return APUS_OK;
 }
@@ -376,6 +392,32 @@ extern "C" int apus_replica_create(const apus_config_t *cfg, apus_replica_t **ou
 extern "C" void apus_replica_destroy(apus_replica_t *r)
 {
     if (!r) return;
+    /* fences of other replicas that read my region.  Out of the live list first: a fence enqueued from now on counts me
+     * as not connected.  Every replica of the process that maps me forgets my address, so that a replica created later
+     * at the same address is never taken for me.  One that has a fence still pending ends its consume waits and fences
+     * (the shared release epoch: a fence may sit behind a pending consume wait) and waits for its latest fence; one with
+     * no fence pending is left alone.  The wait is for work on its consume stream up to that fence, which ends within
+     * microseconds of the release unless that stream waits on a caller's stream; meanwhile g_live_mu is held, so
+     * replica creation, destruction and fences in this process wait too. */
+    {
+        StageLock ll(&g_live_mu);
+        for (apus_replica **p = &g_live; *p; p = &(*p)->live_next)
+            if (*p == r) { *p = r->live_next; break; }
+        for (apus_replica *q = g_live; q && r->region; q = q->live_next) {
+            bool maps = false;
+            for (int i = 0; i < APUS_MAX_SERVER_COUNT; i++)
+                if (i != q->cfg.server_idx && !q->peer_is_ipc[i] && q->peer_ptr[i] == (void *)r->region) {
+                    q->peer_ptr[i] = NULL;
+                    maps = true;
+                }
+            if (!maps || !q->fences) continue;
+            DeviceGuard gq(q->cfg.device);
+            if (cudaEventQuery(q->ev_fence) == cudaSuccess) continue;
+            cudaGetLastError();
+            consume_wait_release(q);
+            cudaEventSynchronize(q->ev_fence);
+        }
+    }
     DeviceGuard g(r->cfg.device);
     if (r->in_flight && r->hw) {
         r->hw->stop = 1;
@@ -411,7 +453,7 @@ extern "C" void apus_replica_destroy(apus_replica_t *r)
     if (r->d_ctx) cudaFree(r->d_ctx);
     if (r->ev_start) cudaEventDestroy(r->ev_start);
     if (r->ev_stop) cudaEventDestroy(r->ev_stop);
-    for (cudaEvent_t e : {r->ev_copy[0], r->ev_copy[1], r->ev_cons[0], r->ev_cons[1]})
+    for (cudaEvent_t e : {r->ev_copy[0], r->ev_copy[1], r->ev_cons[0], r->ev_cons[1], r->ev_fence})
         if (e) cudaEventDestroy(e);
     if (r->cons_st) cudaFree(r->cons_st);
     if (r->cons_stream) cudaStreamDestroy(r->cons_stream);
@@ -1369,6 +1411,53 @@ extern "C" int apus_consume_mark(apus_replica_t *r, uint64_t *mark, void *stream
     r->cons_enqueued++;
     return side_stream_run((cudaStream_t)stream, r->cons_stream, r->ev_cons, "apus_consume_mark_enqueue",
                            [&] { return apus_consume_mark_enqueue(r->region, r->cons_st, mark, r->cons_stream); });
+}
+
+extern "C" int apus_read_fence(apus_replica_t *r, uint32_t timeout_us, uint64_t *index, uint32_t *outcome, void *stream)
+{
+    if (!r) return fail("null argument");
+    const uint32_t need = APUS_F_DEVICE_APPLY | APUS_F_APPLY_ANY_ROLE;
+    if ((r->cfg.flags & need) != need)
+        return fail("apus_read_fence needs a replica created with APUS_F_DEVICE_APPLY | APUS_F_APPLY_ANY_ROLE");
+    if (timeout_us == 0 || timeout_us > APUS_WAIT_MAX_US)
+        return fail("apus_read_fence: timeout_us %u outside [1, %u]", timeout_us, APUS_WAIT_MAX_US);
+    if (!index) return fail("null argument");
+    if ((uintptr_t)index & 7u || (uintptr_t)outcome & 3u)
+        return fail("apus_read_fence: misaligned index (8 B) or outcome (4 B)");
+    for (int i = 0; i < APUS_MAX_SERVER_COUNT; i++)
+        if (r->peer_is_ipc[i] && r->peer_ptr[i])
+            return fail("apus_read_fence: peer %d is mapped through CUDA IPC (fences are for groups hosted in one process)", i);
+    apus_fence_args_t a;
+    memset(&a, 0, sizeof a);
+    a.region = r->region; a.hw = r->hw_dev; a.term = r->cfg.term;
+    a.entries_off = r->entries_off; a.log_len = r->log_len; a.timeout_ns = 1000ull * timeout_us;
+    a.index = index; a.outcome = outcome; a.idx_mask = r->idx_cap - 1;
+    a.n = r->cfg.group_size; a.leader = r->cfg.leader_idx;
+    DeviceGuard g(r->cfg.device);
+    /* under g_live_mu: a peer destroyed before this point is no longer mapped here (apus_replica_destroy clears it), and
+     * one destroyed after it waits for this fence */
+    StageLock ll(&g_live_mu);
+    for (int i = 0; i < a.n; i++) a.member[i] = (const uint8_t *)r->peer_ptr[i];
+    a.member[r->cfg.server_idx] = r->region;
+    StageLock sl(&r->cons_mu);
+    a.epoch = r->hw->cons_wait_epoch;               /* read under cons_mu, as a consume wait reads it */
+    r->cons_enqueued++;
+    r->fences++;
+    return side_stream_run((cudaStream_t)stream, r->cons_stream, r->ev_cons, "apus_read_fence_enqueue", [&] {
+        const cudaError_t e = apus_read_fence_enqueue(&a, r->cons_stream);
+        return e == cudaSuccess ? cudaEventRecord(r->ev_fence, r->cons_stream) : e;
+    });
+}
+
+extern "C" int apus_read_fence_status(apus_replica_t *r, uint64_t *outcome, uint64_t *index)
+{
+    if (!r) return fail("null argument");
+    const uint32_t need = APUS_F_DEVICE_APPLY | APUS_F_APPLY_ANY_ROLE;
+    if ((r->cfg.flags & need) != need)
+        return fail("apus_read_fence_status needs a replica created with APUS_F_DEVICE_APPLY | APUS_F_APPLY_ANY_ROLE");
+    if (outcome) *outcome = r->hw->fence_outcome;
+    if (index) *index = r->hw->fence_index;
+    return APUS_OK;
 }
 
 extern "C" uint64_t apus_leader_suspect(apus_replica_t *r) { return r ? r->hw->leader_suspect : 0; }

@@ -250,7 +250,10 @@ typedef struct apus_hostwords {
     volatile uint64_t cons_wait_outcome; /* consume wait -> host: APUS_WAIT_* of the latest wait that ran (UINT64_MAX:
                                             none has run yet) ... */
     volatile uint64_t cons_wait_avail;   /* ... and the committed entries past the cursor when it ended */
-    uint64_t pad1[3];
+    volatile uint64_t fence_outcome;     /* read fence -> host: APUS_WAIT_* / APUS_WAIT_NOT_LEADER of the latest fence that
+                                            ran (UINT64_MAX: none has run yet) ... */
+    volatile uint64_t fence_index;       /* ... and its read index (0 unless it ended READY) */
+    uint64_t pad1[1];
     volatile uint32_t stop;              /* host -> kernel */
     uint32_t pad2[31];
     volatile uint64_t host_apply;        /* host -> follower kernel (APUS_FLAG_HOST_APPLY): offset up to which the
@@ -351,6 +354,22 @@ typedef struct apus_consume_args {
     uint64_t *offsets;                        /* packed: max_n + 1 words */
     uint64_t  values_cap;
 } apus_consume_args_t;
+
+/* one read fence (apus_read_fence) as its kernel sees it: the group's regions as this replica maps them when the fence is
+ * enqueued (NULL = not connected, or a peer destroyed since), its own, and the term and leader it knew then */
+typedef struct apus_fence_args {
+    const uint8_t *member[APUS_MAX_SERVERS];  /* [i < n]: member i's region; [own idx] = region */
+    const uint8_t *region;                    /* this replica's region (ctrl block, index, entries) */
+    apus_hostwords_t *hw;                     /* status words and the release epoch (device address of the pinned page) */
+    uint64_t  epoch;                          /* the release epoch the fence was enqueued under */
+    uint64_t  term;                           /* t */
+    uint64_t  entries_off, log_len;
+    uint64_t  timeout_ns;
+    uint64_t *index;                          /* receives F on READY */
+    uint32_t *outcome;                        /* optional */
+    uint32_t  idx_mask;
+    uint8_t   n, leader, pad[2];
+} apus_fence_args_t;
 
 /* Device batches (apus_submit_device, apus_submit_device_packed): one batch as the packing kernels see it, in either
  * layout.  A packing block has as many threads as a consume block (the two share one block scan). */

@@ -23,6 +23,7 @@ F_DEVICE_APPLY = 0x200
 F_APPLY_ANY_ROLE = 0x400   # with F_DEVICE_APPLY: the device consumers work on a leader too, and through a take-over
 CONSUME_BAD_IDX = 1
 WAIT_READY, WAIT_TIMED_OUT, WAIT_RELEASED = 0, 1, 2      # outcomes of Replica.consume_wait (APUS_WAIT_*)
+WAIT_NOT_LEADER = 3        # ... and of Replica.read_fence: the leader it knew could not be confirmed
 UINT64_MAX = (1 << 64) - 1
 
 u64, u32, u16, u8, i64, i32 = C.c_uint64, C.c_uint32, C.c_uint16, C.c_uint8, C.c_int64, C.c_int32
@@ -55,6 +56,7 @@ class Stats(C.Structure):
 
 ConsumeStatus = namedtuple("ConsumeStatus", "cursor next_idx need_stride error")
 WaitStatus = namedtuple("WaitStatus", "outcome available")
+FenceStatus = namedtuple("FenceStatus", "outcome index")
 
 _lib = None
 
@@ -73,7 +75,7 @@ EXPORTS = [
     "apus_submit_device", "apus_device_submit_status", "apus_stream_wait_committed", "apus_committed_word",
     "apus_consume_device", "apus_consume_status", "apus_submit_device_packed", "apus_consume_device_packed",
     "apus_consume_wait", "apus_consume_wait_release", "apus_consume_wait_status",
-    "apus_consume_mark", "apus_consume_seed",
+    "apus_consume_mark", "apus_consume_seed", "apus_read_fence", "apus_read_fence_status",
 ]
 
 
@@ -140,6 +142,8 @@ def load_library(path=LIB_PATH):
         L.apus_consume_wait_status.argtypes = [vp, C.POINTER(u64), C.POINTER(u64)]
         L.apus_consume_mark.argtypes = [vp, vp, vp]
         L.apus_consume_seed.argtypes = [vp, u64, u64]
+        L.apus_read_fence.argtypes = [vp, u32, vp, vp, vp]
+        L.apus_read_fence_status.argtypes = [vp, C.POINTER(u64), C.POINTER(u64)]
     _lib = L
     return L
 
@@ -490,6 +494,40 @@ class Replica:
         yet) at a mark another replica's consume_mark wrote (apus_consume_seed); the leader's adjustment then accepts
         it from there"""
         _ck(lib().apus_consume_seed(self.h, int(cursor), int(next_idx)), "apus_consume_seed")
+
+    def read_fence(self, timeout_us, index=None, outcome=None, stream=None):
+        """Enqueue a read fence in `stream` order (apus_read_fence; F_DEVICE_APPLY | F_APPLY_ANY_ROLE): it ends
+        WAIT_READY once this replica holds every entry committed anywhere in the group before it began to run, and then
+        writes the read index F -- a state that has applied through idx F answers a linearizable read.  WAIT_NOT_LEADER:
+        the leader this replica knew could not be confirmed; WAIT_TIMED_OUT / WAIT_RELEASED as consume_wait.  `index`:
+        an int64 or uint64 CUDA tensor [1] on this replica's device (written on READY only); `outcome`: an int32 or
+        uint32 one; each allocated when None.  Returns (index, outcome)."""
+        import torch
+        dev = torch.device("cuda", self.device)
+        s = self._stream(stream)
+        with torch.cuda.stream(s):
+            if index is None:
+                index = torch.zeros(1, dtype=torch.int64, device=dev)
+            if outcome is None:
+                outcome = torch.full((1,), -1, dtype=torch.int32, device=dev)
+        for name, t, dts in (("index", index, (torch.int64, torch.uint64)), ("outcome", outcome, (torch.int32, torch.uint32))):
+            if not isinstance(t, torch.Tensor):
+                raise ApusError(f"read_fence: {name} must be a torch tensor")
+            if t.device != dev:
+                raise ApusError(f"read_fence: {name} is on {t.device}, the replica is on {dev}")
+            if t.dtype not in dts:
+                raise ApusError(f"read_fence: {name} has dtype {t.dtype}, expected one of {dts}")
+            if tuple(t.shape) != (1,):
+                raise ApusError(f"read_fence: {name} has shape {tuple(t.shape)}, expected (1,)")
+        _ck(lib().apus_read_fence(self.h, timeout_us, index.data_ptr(), outcome.data_ptr(), s.cuda_stream),
+            "apus_read_fence")
+        return index, outcome
+
+    def read_fence_status(self):
+        """(outcome of the latest read fence that ran, or UINT64_MAX before any; its read index, 0 unless READY)"""
+        o, i = u64(), u64()
+        _ck(lib().apus_read_fence_status(self.h, C.byref(o), C.byref(i)), "apus_read_fence_status")
+        return FenceStatus(int(o.value), int(i.value))
 
     def wait_committed_on_stream(self, ticket, stream=None):
         """make `stream` (default: the current stream of the leader's device) wait until `ticket` is committed"""

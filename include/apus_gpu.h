@@ -335,7 +335,8 @@ int  apus_consume_status(apus_replica_t *follower, uint64_t *cursor_offset, uint
 /* outcomes of apus_consume_wait */
 #define APUS_WAIT_READY      0u  /* at least min_entries committed entries lie past the consumer's cursor */
 #define APUS_WAIT_TIMED_OUT  1u
-#define APUS_WAIT_RELEASED   2u  /* ended by apus_consume_wait_release, apus_replicas_stop, apus_replica_set_role or destroy */
+#define APUS_WAIT_RELEASED   2u  /* ended by apus_consume_wait_release, apus_replicas_stop, apus_replica_set_role or destroy
+                                    (of this replica, or of a peer it maps while it has a read fence pending) */
 /* Make the consumers wait, in stream order and without the host, until at least min_entries committed entries lie past
  * the consumer's cursor (entries, not rows: NOOP, CONFIG and HEAD entries count), so that an application can enqueue
  * wait -> consume -> its own apply kernel many times ahead and synchronise only when it wants to.  Accepted in the roles
@@ -346,7 +347,8 @@ int  apus_consume_status(apus_replica_t *follower, uint64_t *cursor_offset, uint
  *     or on capacity as it always does;
  *   - the wait ends on whichever comes first: ready; a release (apus_consume_wait_release, apus_replicas_stop,
  *     apus_replica_set_role when a follower takes over, apus_replica_destroy: each ends every wait enqueued before it,
- *     none enqueued after it); or timeout_us, counted from when the wait begins to run on the stream;
+ *     none enqueued after it; the destroy of a peer this replica maps too, while a read fence is pending here); or
+ *     timeout_us, counted from when the wait begins to run on the stream;
  *   - it then writes its APUS_WAIT_* outcome to `outcome` (optional: a 4 B-aligned device word on the replica's GPU, for
  *     device code downstream to branch on) and to the status words (apus_consume_wait_status);
  *   - a consumer stopped for good by APUS_CONSUME_BAD_IDX gets no outcome of its own: its wait ends as the counts say,
@@ -387,6 +389,48 @@ int  apus_consume_mark(apus_replica_t *r, uint64_t *mark, void *stream);
  * whose kernel is stopped, holds no entry (empty log, nothing acked), has had no consume call, wait or mark enqueued,
  * and unless cursor_offset < the log size and next_idx >= 1. */
 int  apus_consume_seed(apus_replica_t *r, uint64_t cursor_offset, uint64_t next_idx);
+/* outcome of apus_read_fence besides the three above: the leader this replica knew could not be confirmed -- a majority
+ * of the group's SIDs carries a newer term, the leader is not connected, or it publishes no current consumer record */
+#define APUS_WAIT_NOT_LEADER (3u)     /* a fence's outcome only: apus_consume_wait never ends with it */
+/* Read fences: linearizable reads from any replica's device state (Raft's read index, section 6.4), for a group that
+ * applies in GPU memory on every replica (APUS_F_DEVICE_APPLY | APUS_F_APPLY_ANY_ROLE).  Let t and L be the term and the
+ * leader this replica knew when the fence was enqueued, N the group size.  The fence, in stream order:
+ *   1. takes K, the entries-committed word of L's consumer record (L's commit warp publishes it only under
+ *      APUS_F_APPLY_ANY_ROLE: no such record ends NOT_LEADER);
+ *   2. after that, reads the SID of every member this replica maps, itself included, and ends NOT_LEADER unless at
+ *      least N/2 + 1 of them are at term <= t.  This relies on the control plane moving a voter's SID to the
+ *      candidate's term BEFORE it acks the vote, as dare_entry.c's elect does: a control plane that acks votes without
+ *      moving the SID gets no guarantee from a fence;
+ *   3. waits until this replica holds committed entries through K, and the last of them carries a term >= t (a new
+ *      leader's commit may lag what an earlier leader committed until its blank CONFIG commits), then ends READY with
+ *      the read index F := the entries committed and held here.
+ * What F covers: every entry that L's consumer record named before the fence began to run (and every entry of an
+ * earlier term committed before then, through the own-term entry), and this replica holds the committed entries through
+ * F.  L's commit warp makes each commit advance visible elsewhere first: it stores the commit into every follower and
+ * the committed-tickets word (apus_committed_tickets, apus_wait_committed, apus_stream_wait_committed) a few stores
+ * before the consumer record, and for longer if L's context is descheduled in between.  A fence that begins in that
+ * window may end READY with F below a write whose commit was already seen that way.  For read-your-writes, the
+ * application compares F with its write's idx (rows carry idx and req_id) and enqueues another fence while F is short:
+ * the record follows within the same commit advance.  A consume call enqueued after a READY fence delivers through F
+ * (given a max_n that reaches it, and unless it stops on a long cmd or on capacity as it always may), and a state that
+ * has applied through F answers a read that is linearizable with respect to the commits L's record has published: the
+ * application compares its applied idx, which the rows carry, with F in its own read kernel.  A group that has
+ * committed nothing yet keeps a fence waiting.
+ * Runs exactly as apus_consume_wait does: on the consume stream under the same lock, in call order with the consume
+ * calls, waits and marks, after everything enqueued on `stream` (a cudaStream_t, NULL = the legacy default stream)
+ * before the call, and `stream` waits for it; it ends RELEASED at the same release points, TIMED_OUT after timeout_us
+ * from when it begins to run.  It then writes F to `index` (an 8 B-aligned device word on the replica's GPU; READY only,
+ * untouched otherwise), the outcome to `outcome` (optional, 4 B aligned) and both to the status words.
+ * Fences read other replicas' regions, so they are for groups hosted in one process: apus_replica_destroy(p) first
+ * unmaps p from every replica of the process that maps it (as apus_replica_disconnect would; a fence enqueued later
+ * counts p as not connected), and on each of them that has a fence pending it ends the consume waits and fences
+ * (APUS_WAIT_RELEASED) and waits for that fence.  APUS_ERROR, with nothing enqueued, for a replica without
+ * APUS_F_DEVICE_APPLY | APUS_F_APPLY_ANY_ROLE, a timeout_us of 0 or above 60 s, a null or misaligned `index`, a
+ * misaligned `outcome`, and a replica that maps any peer through CUDA IPC. */
+int  apus_read_fence(apus_replica_t *r, uint32_t timeout_us, uint64_t *index, uint32_t *outcome, void *stream);
+/* the pinned words the latest fence that ran wrote: its outcome (UINT64_MAX before any fence has run) and its read
+ * index (0 unless it ended READY) */
+int  apus_read_fence_status(apus_replica_t *r, uint64_t *outcome, uint64_t *index);
 /* failure detector: 0 while the leader's heartbeats arrive, else 1 + the term whose leader fell silent */
 uint64_t apus_leader_suspect(apus_replica_t *follower);
 /* %globaltimer (ns) of the leader kernel's latest commit (device clock; step timing of resident kernels) */
