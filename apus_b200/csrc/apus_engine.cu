@@ -1282,8 +1282,42 @@ extern "C" int apus_set_applied(apus_replica_t *r, uint64_t offset)
 }
 
 /* ---- device consumers: committed entries straight into device memory, in stream order ----------------------- */
+/* Which replicas each consumer call accepts.  CONS_STATUS (status and release): a replica created with
+ * APUS_F_DEVICE_APPLY.  CONS_STREAM (the calls that enqueue consume work): the same, but a leader only with
+ * APUS_F_APPLY_ANY_ROLE, and that refusal comes first.  CONS_ANY_ROLE (fences and seeds): both flags. */
+enum consumer_kind { CONS_STATUS, CONS_STREAM, CONS_ANY_ROLE };
+
+static int consumer_gate(const apus_replica *r, const char *what, consumer_kind kind)
+{
+    if (!r) return fail("null argument");
+    if (kind == CONS_ANY_ROLE) {
+        const uint32_t need = APUS_F_DEVICE_APPLY | APUS_F_APPLY_ANY_ROLE;
+        if ((r->cfg.flags & need) != need)
+            return fail("%s needs a replica created with APUS_F_DEVICE_APPLY | APUS_F_APPLY_ANY_ROLE", what);
+        return APUS_OK;
+    }
+    if (kind == CONS_STREAM && is_leader(r) && !(r->cfg.flags & APUS_F_APPLY_ANY_ROLE))
+        return fail("%s: consumption is a follower's (the leader's log is its own)", what);
+    if (!(r->cfg.flags & APUS_F_DEVICE_APPLY)) return fail("%s needs a replica created with APUS_F_DEVICE_APPLY", what);
+    return APUS_OK;
+}
+
+/* One enqueue on the consume stream, in the caller's stream order and in call order with every consume call, wait, mark
+ * and fence of this replica.  Under cons_mu it counts the enqueue (apus_consume_seed refuses a replica that has had
+ * one) and reads the release epoch that `enqueue(epoch)` hands to a wait or fence: read in the order of the enqueues, so
+ * that a release after this call ends what it enqueues. */
+template <typename Enqueue>
+static int cons_stream_run(apus_replica *r, void *stream, const char *what, Enqueue enqueue)
+{
+    DeviceGuard g(r->cfg.device);
+    StageLock sl(&r->cons_mu);
+    const uint64_t epoch = r->hw->cons_wait_epoch;
+    r->cons_enqueued++;
+    return side_stream_run((cudaStream_t)stream, r->cons_stream, r->ev_cons, what, [&] { return enqueue(epoch); });
+}
+
 /* what both layouts share, once the arguments are checked: max_n clipped to the index ring, and the five kernels on the
- * consume stream in the caller's stream order */
+ * consume stream */
 static int consume_enqueue(apus_replica_t *r, apus_consume_args_t a, uint32_t max_n, void *stream)
 {
     /* at most idx_cap entries lie between the cursor and what the follower holds (each is >= 64 B of one lap) */
@@ -1291,21 +1325,15 @@ static int consume_enqueue(apus_replica_t *r, apus_consume_args_t a, uint32_t ma
     a.region = r->region; a.entries_off = r->entries_off; a.log_len = r->log_len;
     a.idx_mask = r->idx_cap - 1; a.max_n = n; a.nblk = (n + APUS_CONS_THREADS - 1) / APUS_CONS_THREADS;
     a.st = r->cons_st; a.hw = r->hw_dev;
-    DeviceGuard g(r->cfg.device);
-    StageLock sl(&r->cons_mu);
-    r->cons_enqueued++;
-    return side_stream_run((cudaStream_t)stream, r->cons_stream, r->ev_cons, "apus_consume_enqueue",
-                           [&] { return apus_consume_enqueue(&a, r->cons_stream); });
+    return cons_stream_run(r, stream, "apus_consume_enqueue",
+                           [&](uint64_t) { return apus_consume_enqueue(&a, r->cons_stream); });
 }
 
 extern "C" int apus_consume_device(apus_replica_t *r, uint32_t max_n, uint64_t *idx, uint8_t *types,
                                    uint16_t *connection_ids, uint64_t *req_ids, uint16_t *lens, void *payloads,
                                    size_t stride, uint32_t *count, void *stream)
 {
-    if (!r) return fail("null argument");
-    if (is_leader(r) && !(r->cfg.flags & APUS_F_APPLY_ANY_ROLE))
-        return fail("apus_consume_device: consumption is a follower's (the leader's log is its own)");
-    if (!(r->cfg.flags & APUS_F_DEVICE_APPLY)) return fail("apus_consume_device needs a replica created with APUS_F_DEVICE_APPLY");
+    if (consumer_gate(r, "apus_consume_device", CONS_STREAM) != APUS_OK) return APUS_ERROR;
     if (max_n == 0) return fail("apus_consume_device: max_n is 0");
     if (!idx || !types || !connection_ids || !req_ids || !lens || !count || (!payloads && stride)) return fail("null argument");
     /* the kernels store whole elements: a misaligned array would fault on the device, so refuse it here */
@@ -1323,11 +1351,7 @@ extern "C" int apus_consume_device_packed(apus_replica_t *r, uint32_t max_n, uin
                                           uint16_t *connection_ids, uint64_t *req_ids, uint64_t *offsets, void *values,
                                           uint64_t values_cap, uint32_t *count, void *stream)
 {
-    if (!r) return fail("null argument");
-    if (is_leader(r) && !(r->cfg.flags & APUS_F_APPLY_ANY_ROLE))
-        return fail("apus_consume_device_packed: consumption is a follower's (the leader's log is its own)");
-    if (!(r->cfg.flags & APUS_F_DEVICE_APPLY))
-        return fail("apus_consume_device_packed needs a replica created with APUS_F_DEVICE_APPLY");
+    if (consumer_gate(r, "apus_consume_device_packed", CONS_STREAM) != APUS_OK) return APUS_ERROR;
     if (max_n == 0) return fail("apus_consume_device_packed: max_n is 0");
     if (!idx || !types || !connection_ids || !req_ids || !offsets || !count || (!values && values_cap))
         return fail("null argument");
@@ -1345,8 +1369,7 @@ extern "C" int apus_consume_device_packed(apus_replica_t *r, uint32_t max_n, uin
 extern "C" int apus_consume_status(apus_replica_t *r, uint64_t *cursor_offset, uint64_t *next_idx, uint64_t *need_stride,
                                    uint64_t *error)
 {
-    if (!r) return fail("null argument");
-    if (!(r->cfg.flags & APUS_F_DEVICE_APPLY)) return fail("apus_consume_status needs a replica created with APUS_F_DEVICE_APPLY");
+    if (consumer_gate(r, "apus_consume_status", CONS_STATUS) != APUS_OK) return APUS_ERROR;
     if (cursor_offset) *cursor_offset = r->hw->cons_cursor;
     if (next_idx) *next_idx = r->hw->cons_next_idx ? r->hw->cons_next_idx : 1;   /* before the first call: idx 1 */
     if (need_stride) *need_stride = r->hw->cons_need_stride;
@@ -1359,21 +1382,13 @@ extern "C" int apus_consume_status(apus_replica_t *r, uint64_t *cursor_offset, u
 extern "C" int apus_consume_wait(apus_replica_t *r, uint32_t min_entries, uint32_t timeout_us, uint32_t *outcome,
                                  void *stream)
 {
-    if (!r) return fail("null argument");
-    if (is_leader(r) && !(r->cfg.flags & APUS_F_APPLY_ANY_ROLE))
-        return fail("apus_consume_wait: consumption is a follower's (the leader's log is its own)");
-    if (!(r->cfg.flags & APUS_F_DEVICE_APPLY)) return fail("apus_consume_wait needs a replica created with APUS_F_DEVICE_APPLY");
+    if (consumer_gate(r, "apus_consume_wait", CONS_STREAM) != APUS_OK) return APUS_ERROR;
     if (min_entries == 0 || min_entries > r->idx_cap)
         return fail("apus_consume_wait: min_entries %u outside [1, %u] (the index ring's capacity)", min_entries, r->idx_cap);
     if (timeout_us == 0 || timeout_us > APUS_WAIT_MAX_US)
         return fail("apus_consume_wait: timeout_us %u outside [1, %u]", timeout_us, APUS_WAIT_MAX_US);
     if ((uintptr_t)outcome & 3u) return fail("apus_consume_wait: misaligned outcome (4 B)");
-    DeviceGuard g(r->cfg.device);
-    StageLock sl(&r->cons_mu);
-    /* the epoch is read under cons_mu, in the order of the enqueues: a release after this call ends this wait */
-    const uint64_t epoch = r->hw->cons_wait_epoch;
-    r->cons_enqueued++;
-    return side_stream_run((cudaStream_t)stream, r->cons_stream, r->ev_cons, "apus_consume_wait_enqueue", [&] {
+    return cons_stream_run(r, stream, "apus_consume_wait_enqueue", [&](uint64_t epoch) {
         return apus_consume_wait_enqueue(r->region, r->hw_dev, epoch, min_entries, 1000ull * timeout_us, outcome,
                                          r->cons_stream);
     });
@@ -1381,18 +1396,14 @@ extern "C" int apus_consume_wait(apus_replica_t *r, uint32_t min_entries, uint32
 
 extern "C" int apus_consume_wait_release(apus_replica_t *r)
 {
-    if (!r) return fail("null argument");
-    if (!(r->cfg.flags & APUS_F_DEVICE_APPLY))
-        return fail("apus_consume_wait_release needs a replica created with APUS_F_DEVICE_APPLY");
+    if (consumer_gate(r, "apus_consume_wait_release", CONS_STATUS) != APUS_OK) return APUS_ERROR;
     consume_wait_release(r);
     return APUS_OK;
 }
 
 extern "C" int apus_consume_wait_status(apus_replica_t *r, uint64_t *outcome, uint64_t *available)
 {
-    if (!r) return fail("null argument");
-    if (!(r->cfg.flags & APUS_F_DEVICE_APPLY))
-        return fail("apus_consume_wait_status needs a replica created with APUS_F_DEVICE_APPLY");
+    if (consumer_gate(r, "apus_consume_wait_status", CONS_STATUS) != APUS_OK) return APUS_ERROR;
     if (outcome) *outcome = r->hw->cons_wait_outcome;
     if (available) *available = r->hw->cons_wait_avail;
     return APUS_OK;
@@ -1400,25 +1411,16 @@ extern "C" int apus_consume_wait_status(apus_replica_t *r, uint64_t *outcome, ui
 
 extern "C" int apus_consume_mark(apus_replica_t *r, uint64_t *mark, void *stream)
 {
-    if (!r) return fail("null argument");
-    if (is_leader(r) && !(r->cfg.flags & APUS_F_APPLY_ANY_ROLE))
-        return fail("apus_consume_mark: consumption is a follower's (the leader's log is its own)");
-    if (!(r->cfg.flags & APUS_F_DEVICE_APPLY)) return fail("apus_consume_mark needs a replica created with APUS_F_DEVICE_APPLY");
+    if (consumer_gate(r, "apus_consume_mark", CONS_STREAM) != APUS_OK) return APUS_ERROR;
     if (!mark) return fail("null argument");
     if ((uintptr_t)mark & 15u) return fail("apus_consume_mark: misaligned mark (16 B)");
-    DeviceGuard g(r->cfg.device);
-    StageLock sl(&r->cons_mu);
-    r->cons_enqueued++;
-    return side_stream_run((cudaStream_t)stream, r->cons_stream, r->ev_cons, "apus_consume_mark_enqueue",
-                           [&] { return apus_consume_mark_enqueue(r->region, r->cons_st, mark, r->cons_stream); });
+    return cons_stream_run(r, stream, "apus_consume_mark_enqueue",
+                           [&](uint64_t) { return apus_consume_mark_enqueue(r->region, r->cons_st, mark, r->cons_stream); });
 }
 
 extern "C" int apus_read_fence(apus_replica_t *r, uint32_t timeout_us, uint64_t *index, uint32_t *outcome, void *stream)
 {
-    if (!r) return fail("null argument");
-    const uint32_t need = APUS_F_DEVICE_APPLY | APUS_F_APPLY_ANY_ROLE;
-    if ((r->cfg.flags & need) != need)
-        return fail("apus_read_fence needs a replica created with APUS_F_DEVICE_APPLY | APUS_F_APPLY_ANY_ROLE");
+    if (consumer_gate(r, "apus_read_fence", CONS_ANY_ROLE) != APUS_OK) return APUS_ERROR;
     if (timeout_us == 0 || timeout_us > APUS_WAIT_MAX_US)
         return fail("apus_read_fence: timeout_us %u outside [1, %u]", timeout_us, APUS_WAIT_MAX_US);
     if (!index) return fail("null argument");
@@ -1433,17 +1435,14 @@ extern "C" int apus_read_fence(apus_replica_t *r, uint32_t timeout_us, uint64_t 
     a.entries_off = r->entries_off; a.log_len = r->log_len; a.timeout_ns = 1000ull * timeout_us;
     a.index = index; a.outcome = outcome; a.idx_mask = r->idx_cap - 1;
     a.n = r->cfg.group_size; a.leader = r->cfg.leader_idx;
-    DeviceGuard g(r->cfg.device);
-    /* under g_live_mu: a peer destroyed before this point is no longer mapped here (apus_replica_destroy clears it), and
-     * one destroyed after it waits for this fence */
+    /* under g_live_mu (taken before cons_mu): a peer destroyed before this point is no longer mapped here
+     * (apus_replica_destroy clears it), and one destroyed after it waits for this fence */
     StageLock ll(&g_live_mu);
     for (int i = 0; i < a.n; i++) a.member[i] = (const uint8_t *)r->peer_ptr[i];
     a.member[r->cfg.server_idx] = r->region;
-    StageLock sl(&r->cons_mu);
-    a.epoch = r->hw->cons_wait_epoch;               /* read under cons_mu, as a consume wait reads it */
-    r->cons_enqueued++;
-    r->fences++;
-    return side_stream_run((cudaStream_t)stream, r->cons_stream, r->ev_cons, "apus_read_fence_enqueue", [&] {
+    return cons_stream_run(r, stream, "apus_read_fence_enqueue", [&](uint64_t epoch) {
+        a.epoch = epoch;
+        r->fences++;
         const cudaError_t e = apus_read_fence_enqueue(&a, r->cons_stream);
         return e == cudaSuccess ? cudaEventRecord(r->ev_fence, r->cons_stream) : e;
     });
@@ -1451,10 +1450,7 @@ extern "C" int apus_read_fence(apus_replica_t *r, uint32_t timeout_us, uint64_t 
 
 extern "C" int apus_read_fence_status(apus_replica_t *r, uint64_t *outcome, uint64_t *index)
 {
-    if (!r) return fail("null argument");
-    const uint32_t need = APUS_F_DEVICE_APPLY | APUS_F_APPLY_ANY_ROLE;
-    if ((r->cfg.flags & need) != need)
-        return fail("apus_read_fence_status needs a replica created with APUS_F_DEVICE_APPLY | APUS_F_APPLY_ANY_ROLE");
+    if (consumer_gate(r, "apus_read_fence_status", CONS_ANY_ROLE) != APUS_OK) return APUS_ERROR;
     if (outcome) *outcome = r->hw->fence_outcome;
     if (index) *index = r->hw->fence_index;
     return APUS_OK;
@@ -1748,10 +1744,7 @@ static int copy_to_peer(apus_replica *r, uint8_t peer, size_t off, size_t len)
 
 extern "C" int apus_consume_seed(apus_replica_t *r, uint64_t cursor_offset, uint64_t next_idx)
 {
-    if (!r) return fail("null argument");
-    const uint32_t need = APUS_F_DEVICE_APPLY | APUS_F_APPLY_ANY_ROLE;
-    if ((r->cfg.flags & need) != need)
-        return fail("apus_consume_seed needs a replica created with APUS_F_DEVICE_APPLY | APUS_F_APPLY_ANY_ROLE");
+    if (consumer_gate(r, "apus_consume_seed", CONS_ANY_ROLE) != APUS_OK) return APUS_ERROR;
     if (is_leader(r)) return fail("apus_consume_seed: a leader's consumers stand on its own log");
     if (r->in_flight) return fail("apus_consume_seed: stop the kernel first");
     if (cursor_offset >= r->log_len || next_idx == 0)

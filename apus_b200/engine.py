@@ -27,6 +27,7 @@ WAIT_NOT_LEADER = 3        # ... and of Replica.read_fence: the leader it knew c
 UINT64_MAX = (1 << 64) - 1
 
 u64, u32, u16, u8, i64, i32 = C.c_uint64, C.c_uint32, C.c_uint16, C.c_uint8, C.c_int64, C.c_int32
+vp, p64 = C.c_void_p, C.POINTER(C.c_uint64)
 
 
 class ApusError(RuntimeError):
@@ -60,27 +61,77 @@ FenceStatus = namedtuple("FenceStatus", "outcome index")
 
 _lib = None
 
-EXPORTS = [
-    "apus_abi_version", "apus_last_error", "apus_device_count", "apus_replica_create",
-    "apus_replica_destroy", "apus_replica_export", "apus_replica_connect", "apus_replicas_launch",
-    "apus_replica_wait", "apus_replica_last_launch_ms", "apus_replicas_stop", "apus_submit",
-    "apus_submit_batch", "apus_submit_defer", "apus_submit_flush", "apus_committed_tickets",
-    "apus_progress", "apus_wait_committed", "apus_closed_loop", "apus_log_offsets", "apus_log_read", "apus_get_stats",
-    "apus_latency_samples", "apus_set_head", "apus_remote_apply_offsets",
-    "apus_submit_uniform", "apus_submit_synth", "apus_synth_byte", "apus_submit_release", "apus_set_applied",
-    "apus_log_read_range", "apus_leader_suspect", "apus_last_commit_ns",
-    "apus_ctl_read", "apus_ctl_set_sid", "apus_ctl_reset_votes", "apus_ctl_clear_vote_request", "apus_ctl_send_vote_request",
-    "apus_ctl_send_vote_ack", "apus_ctl_last_entry", "apus_ctl_adjust_follower", "apus_replica_set_role",
-    "apus_replica_disconnect", "apus_follower_beats", "apus_device_numa_node", "apus_group_multicast", "apus_ctl_heartbeat",
-    "apus_submit_device", "apus_device_submit_status", "apus_stream_wait_committed", "apus_committed_word",
-    "apus_consume_device", "apus_consume_status", "apus_submit_device_packed", "apus_consume_device_packed",
-    "apus_consume_wait", "apus_consume_wait_release", "apus_consume_wait_status",
-    "apus_consume_mark", "apus_consume_seed", "apus_read_fence", "apus_read_fence_status",
-]
+# Every function include/apus_gpu.h declares, in its order: name -> (restype, argtypes).  load_library applies them all,
+# so that no caller depends on ctypes' default of a 32-bit int; tests/test_abi.py checks each against the header.
+SIGNATURES = {
+    "apus_abi_version": (C.c_int, []),
+    "apus_last_error": (C.c_char_p, []),
+    "apus_device_count": (C.c_int, []),
+    "apus_device_numa_node": (C.c_int, [C.c_int]),
+    "apus_replica_create": (C.c_int, [C.POINTER(Config), C.POINTER(vp)]),
+    "apus_replica_destroy": (None, [vp]),
+    "apus_replica_export": (C.c_int, [vp, C.POINTER(PeerHandle)]),
+    "apus_replica_connect": (C.c_int, [vp, u8, C.POINTER(PeerHandle)]),
+    "apus_group_multicast": (C.c_int, [C.POINTER(vp), C.c_int]),
+    "apus_replicas_launch": (C.c_int, [C.POINTER(vp), C.c_int, u64]),
+    "apus_replica_wait": (C.c_int, [vp, i64]),
+    "apus_replica_last_launch_ms": (C.c_int, [vp, C.POINTER(C.c_float)]),
+    "apus_replicas_stop": (C.c_int, [C.POINTER(vp), C.c_int]),
+    "apus_submit": (C.c_int, [vp, u8, u16, u64, vp, u16, p64]),
+    "apus_submit_batch": (C.c_int, [vp, u32, vp, vp, vp, vp, vp, C.c_size_t, p64]),
+    "apus_submit_uniform": (C.c_int, [vp, u32, u8, u16, u64, u16, vp, C.c_size_t, p64]),
+    "apus_submit_synth": (C.c_int, [vp, u32, u8, u16, u64, u16, u32, p64]),
+    "apus_synth_byte": (u8, [u32, u64, u32]),
+    "apus_submit_device": (C.c_int, [vp, u32, vp, vp, vp, vp, vp, C.c_size_t, vp, p64]),
+    "apus_submit_device_packed": (C.c_int, [vp, u32, vp, vp, vp, vp, vp, u64, vp, p64]),
+    "apus_device_submit_status": (C.c_int, [vp, p64, p64]),
+    "apus_submit_defer": (C.c_int, [vp, C.c_int]),
+    "apus_submit_flush": (C.c_int, [vp]),
+    "apus_submit_release": (C.c_int, [vp, u64]),
+    "apus_committed_tickets": (u64, [vp]),
+    "apus_progress": (C.c_int, [vp, p64, p64]),
+    "apus_wait_committed": (C.c_int, [vp, u64, i64]),
+    "apus_stream_wait_committed": (C.c_int, [vp, u64, vp]),
+    "apus_committed_word": (vp, [vp]),
+    "apus_closed_loop": (C.c_int, [vp, u32, u16, u16, u64, vp]),
+    "apus_log_offsets": (C.c_int, [vp, C.POINTER(LogOffsets)]),
+    "apus_log_read": (C.c_int, [vp, u64, u64, vp]),
+    "apus_get_stats": (C.c_int, [vp, C.POINTER(Stats)]),
+    "apus_latency_samples": (C.c_int, [vp, vp, u32, C.POINTER(u32)]),
+    "apus_set_applied": (C.c_int, [vp, u64]),
+    "apus_log_read_range": (C.c_int, [vp, u64, u64, vp, u64, p64]),
+    "apus_consume_device": (C.c_int, [vp, u32, vp, vp, vp, vp, vp, vp, C.c_size_t, vp, vp]),
+    "apus_consume_device_packed": (C.c_int, [vp, u32, vp, vp, vp, vp, vp, vp, u64, vp, vp]),
+    "apus_consume_status": (C.c_int, [vp, p64, p64, p64, p64]),
+    "apus_consume_wait": (C.c_int, [vp, u32, u32, vp, vp]),
+    "apus_consume_wait_release": (C.c_int, [vp]),
+    "apus_consume_wait_status": (C.c_int, [vp, p64, p64]),
+    "apus_consume_mark": (C.c_int, [vp, vp, vp]),
+    "apus_consume_seed": (C.c_int, [vp, u64, u64]),
+    "apus_read_fence": (C.c_int, [vp, u32, vp, vp, vp]),
+    "apus_read_fence_status": (C.c_int, [vp, p64, p64]),
+    "apus_leader_suspect": (u64, [vp]),
+    "apus_last_commit_ns": (u64, [vp]),
+    "apus_ctl_read": (C.c_int, [vp, vp]),
+    "apus_ctl_set_sid": (C.c_int, [vp, u64]),
+    "apus_ctl_reset_votes": (C.c_int, [vp]),
+    "apus_ctl_clear_vote_request": (C.c_int, [vp, u8]),
+    "apus_ctl_send_vote_request": (C.c_int, [vp, u8, u64, u64, u64, vp]),
+    "apus_ctl_send_vote_ack": (C.c_int, [vp, u8, u64]),
+    "apus_ctl_heartbeat": (C.c_int, [vp, p64]),
+    "apus_ctl_last_entry": (C.c_int, [vp, p64, p64, p64, p64]),
+    "apus_ctl_adjust_follower": (C.c_int, [vp, u8, u64, p64]),
+    "apus_replica_set_role": (C.c_int, [vp, u8, u64]),
+    "apus_follower_beats": (C.c_int, [vp, p64]),
+    "apus_replica_disconnect": (C.c_int, [vp, u8]),
+    "apus_set_head": (C.c_int, [vp, u64]),
+    "apus_remote_apply_offsets": (C.c_int, [vp, p64]),
+}
+EXPORTS = list(SIGNATURES)
 
 
 def load_library(path=LIB_PATH):
-    """Load libapus_gpu.so; raises (no fallback) when it is missing."""
+    """Load libapus_gpu.so and give every ABI function its signature; raises (no fallback) when it is missing."""
     global _lib
     if _lib is not None:
         return _lib
@@ -88,62 +139,12 @@ def load_library(path=LIB_PATH):
         raise ApusError(f"{path} not built: run `python -c 'import __graft_entry__ as g; g.build()'` "
                         "(make -C apus_b200/csrc). There is no CPU fallback.")
     L = C.CDLL(path)
-    vp = C.c_void_p
-    L.apus_abi_version.restype = C.c_int
-    L.apus_last_error.restype = C.c_char_p
-    L.apus_device_count.restype = C.c_int
-    L.apus_replica_create.argtypes = [C.POINTER(Config), C.POINTER(vp)]
-    L.apus_replica_destroy.argtypes = [vp]
-    L.apus_replica_destroy.restype = None
-    L.apus_replica_export.argtypes = [vp, C.POINTER(PeerHandle)]
-    L.apus_replica_connect.argtypes = [vp, u8, C.POINTER(PeerHandle)]
-    L.apus_replicas_launch.argtypes = [C.POINTER(vp), C.c_int, u64]
-    L.apus_replica_wait.argtypes = [vp, i64]
-    L.apus_replica_last_launch_ms.argtypes = [vp, C.POINTER(C.c_float)]
-    L.apus_replicas_stop.argtypes = [C.POINTER(vp), C.c_int]
-    L.apus_submit.argtypes = [vp, u8, u16, u64, vp, u16, C.POINTER(u64)]
-    L.apus_submit_batch.argtypes = [vp, u32, vp, vp, vp, vp, vp, C.c_size_t, C.POINTER(u64)]
-    L.apus_submit_defer.argtypes = [vp, C.c_int]
-    L.apus_submit_flush.argtypes = [vp]
-    L.apus_committed_tickets.argtypes = [vp]
-    L.apus_committed_tickets.restype = u64
-    L.apus_wait_committed.argtypes = [vp, u64, i64]
-    L.apus_closed_loop.argtypes = [vp, u32, u16, u16, u64, vp]
-    L.apus_progress.argtypes = [vp, C.POINTER(u64), C.POINTER(u64)]
-    L.apus_log_offsets.argtypes = [vp, C.POINTER(LogOffsets)]
-    L.apus_log_read.argtypes = [vp, u64, u64, vp]
-    L.apus_get_stats.argtypes = [vp, C.POINTER(Stats)]
-    L.apus_latency_samples.argtypes = [vp, vp, u32, C.POINTER(u32)]
-    L.apus_set_head.argtypes = [vp, u64]
-    L.apus_remote_apply_offsets.argtypes = [vp, C.POINTER(u64)]
-    if hasattr(L, "apus_submit_uniform"):       # ABI 2
-        L.apus_submit_uniform.argtypes = [vp, u32, u8, u16, u64, u16, vp, C.c_size_t, C.POINTER(u64)]
-        L.apus_submit_synth.argtypes = [vp, u32, u8, u16, u64, u16, u32, C.POINTER(u64)]
-        L.apus_synth_byte.argtypes = [u32, u64, u32]
-        L.apus_synth_byte.restype = u8
-        L.apus_submit_release.argtypes = [vp, u64]
-        L.apus_set_applied.argtypes = [vp, u64]
-        L.apus_log_read_range.argtypes = [vp, u64, u64, vp, u64, C.POINTER(u64)]
-        L.apus_leader_suspect.argtypes = [vp]
-        L.apus_leader_suspect.restype = u64
-        L.apus_last_commit_ns.argtypes = [vp]
-        L.apus_last_commit_ns.restype = u64
-        L.apus_submit_device.argtypes = [vp, u32, vp, vp, vp, vp, vp, C.c_size_t, vp, C.POINTER(u64)]
-        L.apus_device_submit_status.argtypes = [vp, C.POINTER(u64), C.POINTER(u64)]
-        L.apus_stream_wait_committed.argtypes = [vp, u64, vp]
-        L.apus_committed_word.argtypes = [vp]
-        L.apus_committed_word.restype = vp
-        L.apus_consume_device.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp, C.c_size_t, vp, vp]
-        L.apus_consume_status.argtypes = [vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]
-        L.apus_submit_device_packed.argtypes = [vp, u32, vp, vp, vp, vp, vp, u64, vp, C.POINTER(u64)]
-        L.apus_consume_device_packed.argtypes = [vp, u32, vp, vp, vp, vp, vp, vp, u64, vp, vp]
-        L.apus_consume_wait.argtypes = [vp, u32, u32, vp, vp]
-        L.apus_consume_wait_release.argtypes = [vp]
-        L.apus_consume_wait_status.argtypes = [vp, C.POINTER(u64), C.POINTER(u64)]
-        L.apus_consume_mark.argtypes = [vp, vp, vp]
-        L.apus_consume_seed.argtypes = [vp, u64, u64]
-        L.apus_read_fence.argtypes = [vp, u32, vp, vp, vp]
-        L.apus_read_fence_status.argtypes = [vp, C.POINTER(u64), C.POINTER(u64)]
+    for name, (restype, argtypes) in SIGNATURES.items():
+        try:
+            fn = getattr(L, name)
+        except AttributeError:
+            raise ApusError(f"{path} does not export {name}: rebuild it (make -C apus_b200/csrc)") from None
+        fn.restype, fn.argtypes = restype, argtypes
     _lib = L
     return L
 
@@ -161,6 +162,23 @@ def _ck(rc, what):
     raise ApusError(f"{what}: {msg}")
 
 
+def _check_tensors(what, dev, spec):
+    """Raise ApusError for the first (name, tensor, dtypes, shape) of `spec` whose tensor is not a contiguous torch tensor
+    on `dev` with one of `dtypes` and that shape (None: any 1-D shape): the device calls hand raw pointers to kernels."""
+    import torch
+    for name, t, dtypes, shape in spec:
+        if not isinstance(t, torch.Tensor):
+            raise ApusError(f"{what}: {name} must be a torch tensor")
+        if t.device != dev:
+            raise ApusError(f"{what}: {name} is on {t.device}, the replica is on {dev}")
+        if t.dtype not in dtypes:
+            raise ApusError(f"{what}: {name} has dtype {t.dtype}, expected one of {dtypes}")
+        if (tuple(t.shape) != shape) if shape is not None else t.dim() != 1:
+            raise ApusError(f"{what}: {name} has shape {tuple(t.shape)}, expected {'1-D' if shape is None else shape}")
+        if not t.is_contiguous():
+            raise ApusError(f"{what}: {name} is not contiguous")
+
+
 class Replica:
     def __init__(self, device, server_idx, group_size, leader_idx=0, term=1, log_size=0,
                  ring_mode=RING_HOST_MAPPED, ring_slots=0, ring_bytes=0, flags=None, leader_ctas=0,
@@ -168,7 +186,7 @@ class Replica:
         cfg = Config()
         cfg.leader_ctas = leader_ctas
         cfg.hb_period_us, cfg.hb_timeout_us = hb_period_us, hb_timeout_us
-        cfg.struct_size = C.sizeof(Config) if lib().apus_abi_version() >= 2 else 48
+        cfg.struct_size = C.sizeof(Config)
         cfg.device, cfg.server_idx, cfg.group_size, cfg.leader_idx = device, server_idx, group_size, leader_idx
         cfg.ring_mode, cfg.term, cfg.log_size = ring_mode, term, log_size
         cfg.ring_slots, cfg.ring_bytes = ring_slots, ring_bytes
@@ -265,21 +283,10 @@ class Replica:
         if payloads is None or not isinstance(payloads, torch.Tensor) or payloads.dim() != 2:
             raise ApusError("submit_device: payloads must be a 2-D uint8 CUDA tensor [n, stride]")
         n, stride = payloads.shape
-        spec = (("types", types, (torch.uint8,)), ("conns", conns, (torch.int16, torch.uint16)),
-                ("req_ids", req_ids, (torch.int64,)), ("lens", lens, (torch.int16, torch.uint16, torch.int32)),
-                ("payloads", payloads, (torch.uint8,)))
-        for name, t, dtypes in spec:
-            if not isinstance(t, torch.Tensor):
-                raise ApusError(f"submit_device: {name} must be a torch tensor")
-            if t.device != dev:
-                raise ApusError(f"submit_device: {name} is on {t.device}, the leader is on {dev}")
-            if t.dtype not in dtypes:
-                raise ApusError(f"submit_device: {name} has dtype {t.dtype}, expected one of {dtypes}")
-            if t.shape[0] != n or (name != "payloads" and t.dim() != 1):
-                raise ApusError(f"submit_device: {name} has shape {tuple(t.shape)}, expected [{n}]" +
-                                (f" x {stride}" if name == "payloads" else ""))
-            if not t.is_contiguous():
-                raise ApusError(f"submit_device: {name} is not contiguous")
+        _check_tensors("submit_device", dev, (
+            ("types", types, (torch.uint8,), (n,)), ("conns", conns, (torch.int16, torch.uint16), (n,)),
+            ("req_ids", req_ids, (torch.int64,), (n,)), ("lens", lens, (torch.int16, torch.uint16, torch.int32), (n,)),
+            ("payloads", payloads, (torch.uint8,), (n, stride))))
         s = self._stream(stream)
         if lens.dtype == torch.int32:
             # the ABI takes uint16 lengths: a length outside [0, stride] must stay > stride after the narrowing
@@ -307,21 +314,10 @@ class Replica:
         if not isinstance(types, torch.Tensor) or types.dim() != 1:
             raise ApusError("submit_device_packed: types must be a 1-D uint8 CUDA tensor [n]")
         n = types.shape[0]
-        spec = (("types", types, (torch.uint8,), (n,)), ("conns", conns, (torch.int16, torch.uint16), (n,)),
-                ("req_ids", req_ids, (torch.int64,), (n,)), ("offsets", offsets, (torch.int64,), (n + 1,)),
-                ("values", values, (torch.uint8,), None))
-        for name, t, dtypes, shape in spec:
-            if not isinstance(t, torch.Tensor):
-                raise ApusError(f"submit_device_packed: {name} must be a torch tensor")
-            if t.device != dev:
-                raise ApusError(f"submit_device_packed: {name} is on {t.device}, the leader is on {dev}")
-            if t.dtype not in dtypes:
-                raise ApusError(f"submit_device_packed: {name} has dtype {t.dtype}, expected one of {dtypes}")
-            if (tuple(t.shape) != shape) if shape else t.dim() != 1:
-                raise ApusError(f"submit_device_packed: {name} has shape {tuple(t.shape)}, expected "
-                                f"{list(shape) if shape else '1-D'}")
-            if not t.is_contiguous():
-                raise ApusError(f"submit_device_packed: {name} is not contiguous")
+        _check_tensors("submit_device_packed", dev, (
+            ("types", types, (torch.uint8,), (n,)), ("conns", conns, (torch.int16, torch.uint16), (n,)),
+            ("req_ids", req_ids, (torch.int64,), (n,)), ("offsets", offsets, (torch.int64,), (n + 1,)),
+            ("values", values, (torch.uint8,), None)))
         s = self._stream(stream)
         nv = values.numel()
         t = u64()
@@ -357,22 +353,12 @@ class Replica:
                        torch.empty(1, dtype=torch.int32, device=dev))
         if len(out) != 7:
             raise ApusError("consume_device: out must be (idx, types, conns, req_ids, lens, payloads, count)")
-        spec = (("idx", (torch.int64,), (max_n,)), ("types", (torch.uint8,), (max_n,)),
-                ("conns", (torch.int16, torch.uint16), (max_n,)), ("req_ids", (torch.int64,), (max_n,)),
-                ("lens", (torch.int16, torch.uint16), (max_n,)), ("payloads", (torch.uint8,), (max_n, stride)),
-                ("count", (torch.int32, torch.uint32), (1,)))
-        for (name, dtypes, shape), t in zip(spec, out):
-            if not isinstance(t, torch.Tensor):
-                raise ApusError(f"consume_device: {name} must be a torch tensor")
-            if t.device != dev:
-                raise ApusError(f"consume_device: {name} is on {t.device}, the replica is on {dev}")
-            if t.dtype not in dtypes:
-                raise ApusError(f"consume_device: {name} has dtype {t.dtype}, expected one of {dtypes}")
-            if tuple(t.shape) != shape:
-                raise ApusError(f"consume_device: {name} has shape {tuple(t.shape)}, expected {shape}")
-            if not t.is_contiguous():
-                raise ApusError(f"consume_device: {name} is not contiguous")
         idx, types, conns, req_ids, lens, payloads, count = out
+        _check_tensors("consume_device", dev, (
+            ("idx", idx, (torch.int64,), (max_n,)), ("types", types, (torch.uint8,), (max_n,)),
+            ("conns", conns, (torch.int16, torch.uint16), (max_n,)), ("req_ids", req_ids, (torch.int64,), (max_n,)),
+            ("lens", lens, (torch.int16, torch.uint16), (max_n,)),
+            ("payloads", payloads, (torch.uint8,), (max_n, stride)), ("count", count, (torch.int32, torch.uint32), (1,))))
         _ck(lib().apus_consume_device(self.h, max_n, idx.data_ptr(), types.data_ptr(), conns.data_ptr(),
                                       req_ids.data_ptr(), lens.data_ptr(), payloads.data_ptr() if stride else None,
                                       stride, count.data_ptr(), s.cuda_stream), "apus_consume_device")
@@ -397,22 +383,12 @@ class Replica:
                        torch.empty(1, dtype=torch.int32, device=dev))
         if len(out) != 7:
             raise ApusError("consume_device_packed: out must be (idx, types, conns, req_ids, offsets, values, count)")
-        spec = (("idx", (torch.int64,), (max_n,)), ("types", (torch.uint8,), (max_n,)),
-                ("conns", (torch.int16, torch.uint16), (max_n,)), ("req_ids", (torch.int64,), (max_n,)),
-                ("offsets", (torch.int64,), (max_n + 1,)), ("values", (torch.uint8,), (values_cap,)),
-                ("count", (torch.int32, torch.uint32), (1,)))
-        for (name, dtypes, shape), t in zip(spec, out):
-            if not isinstance(t, torch.Tensor):
-                raise ApusError(f"consume_device_packed: {name} must be a torch tensor")
-            if t.device != dev:
-                raise ApusError(f"consume_device_packed: {name} is on {t.device}, the replica is on {dev}")
-            if t.dtype not in dtypes:
-                raise ApusError(f"consume_device_packed: {name} has dtype {t.dtype}, expected one of {dtypes}")
-            if tuple(t.shape) != shape:
-                raise ApusError(f"consume_device_packed: {name} has shape {tuple(t.shape)}, expected {shape}")
-            if not t.is_contiguous():
-                raise ApusError(f"consume_device_packed: {name} is not contiguous")
         idx, types, conns, req_ids, offsets, values, count = out
+        _check_tensors("consume_device_packed", dev, (
+            ("idx", idx, (torch.int64,), (max_n,)), ("types", types, (torch.uint8,), (max_n,)),
+            ("conns", conns, (torch.int16, torch.uint16), (max_n,)), ("req_ids", req_ids, (torch.int64,), (max_n,)),
+            ("offsets", offsets, (torch.int64,), (max_n + 1,)), ("values", values, (torch.uint8,), (values_cap,)),
+            ("count", count, (torch.int32, torch.uint32), (1,))))
         _ck(lib().apus_consume_device_packed(self.h, max_n, idx.data_ptr(), types.data_ptr(), conns.data_ptr(),
                                              req_ids.data_ptr(), offsets.data_ptr(),
                                              values.data_ptr() if values_cap else None, values_cap, count.data_ptr(),
@@ -437,17 +413,7 @@ class Replica:
         dev = torch.device("cuda", self.device)
         s = self._stream(stream)
         if outcome is not None:
-            if not isinstance(outcome, torch.Tensor):
-                raise ApusError("consume_wait: outcome must be a torch tensor")
-            if outcome.device != dev:
-                raise ApusError(f"consume_wait: outcome is on {outcome.device}, the replica is on {dev}")
-            if outcome.dtype not in (torch.int32, torch.uint32):
-                raise ApusError(f"consume_wait: outcome has dtype {outcome.dtype}, expected one of "
-                                f"{(torch.int32, torch.uint32)}")
-            if tuple(outcome.shape) != (1,):
-                raise ApusError(f"consume_wait: outcome has shape {tuple(outcome.shape)}, expected (1,)")
-            if not outcome.is_contiguous():
-                raise ApusError("consume_wait: outcome is not contiguous")
+            _check_tensors("consume_wait", dev, (("outcome", outcome, (torch.int32, torch.uint32), (1,)),))
         _ck(lib().apus_consume_wait(self.h, min_entries, timeout_us, None if outcome is None else outcome.data_ptr(),
                                     s.cuda_stream), "apus_consume_wait")
         return outcome
@@ -476,16 +442,7 @@ class Replica:
         if out is None:
             with torch.cuda.stream(s):
                 out = torch.empty(2, dtype=torch.int64, device=dev)
-        if not isinstance(out, torch.Tensor):
-            raise ApusError("consume_mark: out must be a torch tensor")
-        if out.device != dev:
-            raise ApusError(f"consume_mark: out is on {out.device}, the replica is on {dev}")
-        if out.dtype not in (torch.int64, torch.uint64):
-            raise ApusError(f"consume_mark: out has dtype {out.dtype}, expected one of {(torch.int64, torch.uint64)}")
-        if tuple(out.shape) != (2,):
-            raise ApusError(f"consume_mark: out has shape {tuple(out.shape)}, expected (2,)")
-        if not out.is_contiguous():
-            raise ApusError("consume_mark: out is not contiguous")
+        _check_tensors("consume_mark", dev, (("out", out, (torch.int64, torch.uint64), (2,)),))
         _ck(lib().apus_consume_mark(self.h, out.data_ptr(), s.cuda_stream), "apus_consume_mark")
         return out
 
@@ -510,15 +467,8 @@ class Replica:
                 index = torch.zeros(1, dtype=torch.int64, device=dev)
             if outcome is None:
                 outcome = torch.full((1,), -1, dtype=torch.int32, device=dev)
-        for name, t, dts in (("index", index, (torch.int64, torch.uint64)), ("outcome", outcome, (torch.int32, torch.uint32))):
-            if not isinstance(t, torch.Tensor):
-                raise ApusError(f"read_fence: {name} must be a torch tensor")
-            if t.device != dev:
-                raise ApusError(f"read_fence: {name} is on {t.device}, the replica is on {dev}")
-            if t.dtype not in dts:
-                raise ApusError(f"read_fence: {name} has dtype {t.dtype}, expected one of {dts}")
-            if tuple(t.shape) != (1,):
-                raise ApusError(f"read_fence: {name} has shape {tuple(t.shape)}, expected (1,)")
+        _check_tensors("read_fence", dev, (("index", index, (torch.int64, torch.uint64), (1,)),
+                                           ("outcome", outcome, (torch.int32, torch.uint32), (1,))))
         _ck(lib().apus_read_fence(self.h, timeout_us, index.data_ptr(), outcome.data_ptr(), s.cuda_stream),
             "apus_read_fence")
         return index, outcome
@@ -633,7 +583,6 @@ def pin_to_device_node(device: int):
     """Run this process on the CPUs of the NUMA node next to `device` (its pinned rings are then allocated there too).
     Returns the node, or None when the topology is not exposed."""
     try:
-        lib().apus_device_numa_node.argtypes = [C.c_int]
         node = int(lib().apus_device_numa_node(device))
         if node < 0:
             return None
@@ -715,7 +664,6 @@ class Group:
     def multicast(self):
         """Bind the replicas' regions (created with F_FABRIC, one GPU each) to an NVSwitch multicast object."""
         arr = (C.c_void_p * self.n)(*[r.h for r in self.replicas])
-        lib().apus_group_multicast.argtypes = [C.POINTER(C.c_void_p), C.c_int]
         _ck(lib().apus_group_multicast(arr, self.n), "apus_group_multicast")
 
     def prologue(self):

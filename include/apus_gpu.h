@@ -391,7 +391,7 @@ int  apus_consume_mark(apus_replica_t *r, uint64_t *mark, void *stream);
 int  apus_consume_seed(apus_replica_t *r, uint64_t cursor_offset, uint64_t next_idx);
 /* outcome of apus_read_fence besides the three above: the leader this replica knew could not be confirmed -- a majority
  * of the group's SIDs carries a newer term, the leader is not connected, or it publishes no current consumer record */
-#define APUS_WAIT_NOT_LEADER (3u)     /* a fence's outcome only: apus_consume_wait never ends with it */
+#define APUS_WAIT_NOT_LEADER 3u  /* a fence's outcome only: apus_consume_wait never ends with it */
 /* Read fences: linearizable reads from any replica's device state (Raft's read index, section 6.4), for a group that
  * applies in GPU memory on every replica (APUS_F_DEVICE_APPLY | APUS_F_APPLY_ANY_ROLE).  Let t and L be the term and the
  * leader this replica knew when the fence was enqueued, N the group size.  The fence, in stream order:

@@ -14,7 +14,7 @@ import scenarios
 import streams as S
 from apus_b200 import engine as E
 
-u8, u64, vp = C.c_uint8, C.c_uint64, C.c_void_p
+u64 = C.c_uint64
 
 
 def mask_others(img, ents, me):
@@ -186,16 +186,6 @@ class Pair:
             self.check_not_committed(*before)
 
 
-def ctl(eng):
-    L = eng.lib()
-    L.apus_ctl_send_vote_ack.argtypes = [vp, u8, u64]
-    L.apus_ctl_last_entry.argtypes = [vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]
-    L.apus_replica_set_role.argtypes = [vp, u8, u64]
-    L.apus_ctl_adjust_follower.argtypes = [vp, u8, u64, C.POINTER(u64)]
-    L.apus_replica_disconnect.argtypes = [vp, u8]
-    return L
-
-
 def sid(term, leader, idx):
     return (term << 9) | ((1 if leader else 0) << 8) | idx
 
@@ -331,7 +321,7 @@ def elect(eng, g, c, survivors, winner, voters, term):
     oracle cluster `c` shadowing it.  `survivors`: every replica but the dead leader.  Returns ({survivor: commit
     offset}, {voter: shared end}, {voter: (from, to) of a non-empty resent range})."""
     L, dead = g.replicas[0].log_len, g.leader_idx
-    lib = ctl(eng)
+    lib = eng.lib()
     rep = g.replicas
     for i in survivors:
         E._ck(lib.apus_replica_disconnect(rep[i].h, dead), "apus_replica_disconnect")

@@ -1,6 +1,7 @@
-"""CPU-side checks of the drop-in boundary: the shared library loads and exports
-every symbol include/apus_gpu.h declares; without a GPU every entry point fails
-loudly (there is no CPU fallback)."""
+"""CPU-side checks of the drop-in boundary: the shared library loads and exports every symbol include/apus_gpu.h
+declares, the binding gives each the header's signature, the outcome values and the layout words the consumer calls
+use stay where the header and apus_layout.h put them, and without a GPU every entry point fails loudly (there is no
+CPU fallback)."""
 import ctypes as C
 import os
 import re
@@ -9,6 +10,10 @@ import subprocess
 import pytest
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+# C scalar types of the header -> the ctypes type that passes them at full width
+SCALARS = {"uint8_t": C.c_uint8, "uint16_t": C.c_uint16, "uint32_t": C.c_uint32, "uint64_t": C.c_uint64,
+           "int": C.c_int, "int64_t": C.c_int64, "size_t": C.c_size_t}
 
 
 @pytest.fixture(scope="module")
@@ -19,10 +24,28 @@ def built():
     return engine
 
 
-def declared_symbols():
+def header(strip_comments=False):
     txt = open(os.path.join(ROOT, "include", "apus_gpu.h")).read()
-    txt = re.sub(r"/\*.*?\*/", "", txt, flags=re.S)
-    return sorted(set(re.findall(r"\b(apus_[a-z_0-9]+)\s*\(", txt)))
+    return re.sub(r"/\*.*?\*/", "", txt, flags=re.S) if strip_comments else txt
+
+
+def declared_symbols():
+    return sorted(set(re.findall(r"\b(apus_[a-z_0-9]+)\s*\(", header(strip_comments=True))))
+
+
+def prototypes():
+    """{name: (return type, [parameter declarations])} of every function the header declares"""
+    out = {}
+    for m in re.finditer(r"^([A-Za-z_][\w \t*]*?)\s*\b(apus_\w+)\s*\(([^()]*)\)\s*;", header(strip_comments=True),
+                         flags=re.M):
+        params = [" ".join(p.split()) for p in m.group(3).split(",")]
+        out[m.group(2)] = (" ".join(m.group(1).split()), [] if params == ["void"] else params)
+    return out
+
+
+def layout_block(name):
+    txt = open(os.path.join(ROOT, "apus_b200", "csrc", "apus_layout.h")).read()
+    return txt[txt.index(f"typedef struct {name} {{"):txt.index(f"}} {name}_t;")]
 
 
 def test_header_symbols_exported(built):
@@ -33,6 +56,88 @@ def test_header_symbols_exported(built):
         assert hasattr(lib, s), f"{s} declared in include/apus_gpu.h but not exported"
     assert sorted(built.EXPORTS) == syms
     assert lib.apus_abi_version() == 2
+
+
+def test_signatures_match_the_header(built):
+    """every prototype of the header has its entry in the binding's table: the same number of parameters, the same
+    scalar widths, a pointer type for each pointer or array, and the return type"""
+    protos = prototypes()
+    assert sorted(protos) == declared_symbols()
+    assert sorted(built.SIGNATURES) == sorted(protos)
+
+    def is_pointer(t):
+        return t in (C.c_void_p, C.c_char_p) or issubclass(t, C._Pointer)
+
+    for name, (ret, params) in protos.items():
+        restype, argtypes = built.SIGNATURES[name]
+        if ret == "const char *":
+            assert restype is C.c_char_p, name
+        elif "*" in ret:
+            assert restype is C.c_void_p, (name, ret, restype)
+        else:
+            assert restype is (None if ret == "void" else SCALARS[ret]), (name, ret, restype)
+        assert len(argtypes) == len(params), (name, params, argtypes)
+        for k, (p, t) in enumerate(zip(params, argtypes)):
+            if "*" in p or "[" in p:
+                assert is_pointer(t), (name, k, p, t)
+            else:
+                assert t is SCALARS[p.rsplit(" ", 1)[0]], (name, k, p, t)
+
+
+def test_snapshot_call_prototypes():
+    """the exact prototypes of apus_consume_mark and apus_consume_seed"""
+    hdr = header()
+    assert re.search(r"int\s+apus_consume_mark\(apus_replica_t \*r, uint64_t \*mark, void \*stream\);", hdr)
+    assert re.search(r"int\s+apus_consume_seed\(apus_replica_t \*r, uint64_t cursor_offset, uint64_t next_idx\);", hdr)
+
+
+def test_wait_outcomes_match_the_header(built):
+    """the outcomes of consume waits and read fences: exactly these four defines, and the binding's WAIT_* are them"""
+    defs = dict(re.findall(r"#define\s+(APUS_WAIT_\w+)\s+(\S+)", header()))
+    assert defs == {"APUS_WAIT_READY": "0u", "APUS_WAIT_TIMED_OUT": "1u", "APUS_WAIT_RELEASED": "2u",
+                    "APUS_WAIT_NOT_LEADER": "3u"}, defs
+    assert (built.WAIT_READY, built.WAIT_TIMED_OUT, built.WAIT_RELEASED, built.WAIT_NOT_LEADER) == (0, 1, 2, 3)
+
+
+def test_the_seed_word_takes_a_spare_word():
+    """cons_seeded follows cons_on, in what was padding: every word before it keeps its offset, the block its size"""
+    block = layout_block("apus_ctrl")
+    tail = re.findall(r"uint64_t\s+(\w+)(?:\[(\d+)\])?;", block[block.index("uint64_t cons_rec"):])
+    assert tail == [("cons_rec", "2"), ("cons_cur", "2"), ("cons_on", ""), ("cons_seeded", ""), ("pad4", "10")], tail
+
+
+def test_fence_status_words_take_spare_host_words():
+    at, off = {}, 0
+    for name, cnt in re.findall(r"uint64_t\s+(\w+)(?:\[(\d+)\])?;", layout_block("apus_hostwords")):
+        at[name] = off
+        off += 8 * (int(cnt) if cnt else 1)
+    # the words after the consume waits' three stay where they were: stop at 8 * 32
+    assert at["fence_outcome"] == at["cons_wait_avail"] + 8 and at["fence_index"] == at["fence_outcome"] + 8
+    assert at["pad1"] + 8 == 256, at
+
+
+def test_null_replica_is_refused(built):
+    """every call that checks which replicas may consume refuses a null replica first, whatever its other arguments"""
+    lib = built.load_library()
+    buf = (C.c_uint64 * 16)()
+    a = C.addressof(buf)
+    w = [C.byref(C.c_uint64()) for _ in range(4)]
+    calls = {
+        "apus_consume_device": (1, a, a, a, a, a, a, 8, a, None),
+        "apus_consume_device_packed": (1, a, a, a, a, a, a, 8, a, None),
+        "apus_consume_status": (w[0], w[1], w[2], w[3]),
+        "apus_consume_wait": (1, 1000, a, None),
+        "apus_consume_wait_release": (),
+        "apus_consume_wait_status": (w[0], w[1]),
+        "apus_consume_mark": (a, None),
+        "apus_consume_seed": (0, 1),
+        "apus_read_fence": (1000, a, a, None),
+        "apus_read_fence_status": (w[0], w[1]),
+    }
+    for name, args in calls.items():
+        assert name in built.EXPORTS, name
+        assert getattr(lib, name)(None, *args) == built.APUS_ERROR, name
+        assert lib.apus_last_error() == b"null argument", (name, lib.apus_last_error())
 
 
 def test_nm_shows_kernel_and_c_abi(built):

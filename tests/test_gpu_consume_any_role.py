@@ -34,7 +34,7 @@ from apus_b200 import engine as E  # noqa: E402
 from consumers import (ANY, Consumer, PackedConsumer, catch_up, check_rows, close_all, consumer_group,  # noqa: E402
                        drain, heads_against_reports, idx_cap, oracle_rows, wait_forwarded_all)
 from engine_util import MODES, QUIET_S, devices_for, eng, run_case, submit_all, tensors, wait_for  # noqa: E402,F401
-from shadow import Takeover, check_heads, ctl, elect, lap_stream, sid, watch_commits  # noqa: E402
+from shadow import Takeover, check_heads, elect, lap_stream, sid, watch_commits  # noqa: E402
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(900)]
 
@@ -550,7 +550,7 @@ def region_bytes(rep, off, n):
 
 
 def case_argument_checks(eng, orc):
-    lib = ctl(eng)
+    lib = eng.lib()
     n, L = 3, 1 << 20
     devs = devices_for(eng, n)
     for i in (0, 1):

@@ -435,10 +435,8 @@ def test_argument_checks(eng):
         assert E.lib().apus_consume_device(reps[1].h, 4, ptrs[0], ptrs[1], ptrs[2], ptrs[3], ptrs[4], None, 0, ptrs[6],
                                            s) == E.APUS_OK
         torch.cuda.synchronize(reps[1].device)
-        E.lib().apus_replica_set_role.argtypes = [C.c_void_p, C.c_uint8, C.c_uint64]
         with pytest.raises(E.ApusError, match="keeps its role"):
             E._ck(E.lib().apus_replica_set_role(reps[1].h, 1, 2), "apus_replica_set_role")
-        E.lib().apus_ctl_adjust_follower.argtypes = [C.c_void_p, C.c_uint8, C.c_uint64, C.POINTER(C.c_uint64)]
         got = C.c_uint64()
         with pytest.raises(E.ApusError, match="consumes on the device"):
             E._ck(E.lib().apus_ctl_adjust_follower(reps[0].h, 1, 5, C.byref(got)), "apus_ctl_adjust_follower")

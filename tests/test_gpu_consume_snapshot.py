@@ -31,7 +31,7 @@ import streams as S  # noqa: E402
 from apus_b200 import engine as E  # noqa: E402
 from consumers import ANY, Consumer, PackedConsumer, check_rows, idx_cap, new_stream  # noqa: E402
 from engine_util import MODES, devices_for, eng, run_case, wait_for  # noqa: E402,F401
-from shadow import ctl, sid  # noqa: E402
+from shadow import sid  # noqa: E402
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(900)]
 
@@ -258,7 +258,7 @@ class Group:
 
     def __init__(self, eng, n, L, layout, lens):
         self.eng, self.n, self.L, self.layout, self.lens = eng, n, L, layout, lens
-        self.lib = ctl(eng)
+        self.lib = eng.lib()
         self.devs = devices_for(eng, n)
         self.reps = EU.connected([E.Replica(self.devs[i], i, n, 0, 1, L, E.RING_HOST_MAPPED, 1 << 14, 1 << 22,
                                             MODES["index_earlyack"] | ANY | (E.F_AUTOPRUNE if i == 0 else 0), 4)

@@ -29,7 +29,7 @@ import streams as S  # noqa: E402
 from apus_b200 import engine as E  # noqa: E402
 from consumers import ANY, Consumer, catch_up, check_rows, close_all, consumer_group, new_stream, oracle_rows  # noqa: E402
 from engine_util import MODES, devices_for, eng, run_case, tensors  # noqa: E402,F401
-from shadow import ctl, elect, sid  # noqa: E402
+from shadow import elect, sid  # noqa: E402
 
 pytestmark = [pytest.mark.gpu, pytest.mark.timeout(900)]
 
@@ -295,8 +295,7 @@ def case_own_term(eng, orc):
     import torch
     n, L = 3, 1 << 20
     g = _group(eng, n, L)
-    lib = ctl(eng)
-    lib.apus_ctl_set_sid.argtypes = [E.C.c_void_p, E.u64]
+    lib = eng.lib()
     c = None
     try:
         st = {i: new_stream(g.replicas[i].device) for i in (1, 2)}
@@ -370,8 +369,7 @@ def _fence(rep, stream, timeout_us=5_000_000):
 def case_deposed(eng, orc):
     n, L = 5, 1 << 20
     g = _group(eng, n, L)
-    lib = ctl(eng)
-    lib.apus_ctl_set_sid.argtypes = [E.C.c_void_p, E.u64]
+    lib = eng.lib()
     try:
         st = {i: new_stream(g.replicas[i].device) for i in range(n)}
         EU.launch_each(eng, g.replicas, FOREVER)

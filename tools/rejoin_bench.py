@@ -154,10 +154,6 @@ def main():
     if not torch.cuda.is_available() or A.lib().apus_device_count() < 1:
         raise SystemExit("rejoin_bench.py: no CUDA device; the engine has no CPU fallback")
     lib = A.lib()
-    lib.apus_ctl_adjust_follower.argtypes = [ctypes.c_void_p, ctypes.c_uint8, ctypes.c_uint64,
-                                             ctypes.POINTER(ctypes.c_uint64)]
-    lib.apus_replica_disconnect.argtypes = [ctypes.c_void_p, ctypes.c_uint8]
-    lib.apus_replica_set_role.argtypes = [ctypes.c_void_p, ctypes.c_uint8, ctypes.c_uint64]
     # every torch kernel the appliers use, loaded before the replica kernels are resident
     for dt in (torch.uint8, torch.int16, torch.int32, torch.int64):
         torch.zeros(16, dtype=dt, device="cuda:0").clone().add_(1)
