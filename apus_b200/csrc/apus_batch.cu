@@ -274,20 +274,11 @@ __global__ void apus_bell_kernel(uint64_t *bell, uint64_t upto)
 // found through the offset index, never by walking bytes; they never wrap (the ghost-header rule places them at 0), so
 // each cmd is one contiguous run.
 // ---------------------------------------------------------------------------------
-#define CONS_OK        0u
-#define CONS_LATER     1u    // not committed (yet): the examination ends here, quietly
-#define CONS_BAD_IDX   2u    // the entry at the index word does not carry the expected idx
+#define CONS_OK        APUS_CONS_OK
+#define CONS_LATER     APUS_CONS_LATER    // not committed (yet): the examination ends here, quietly
+#define CONS_BAD_IDX   APUS_CONS_BAD      // the entry at the index word does not carry the expected idx
 #define CONS_TOO_LONG  3u    // CSM-like with a cmd longer than the row stride (strided calls)
 #define CONS_NONE      0xffffffffu
-
-__device__ __forceinline__ uint32_t ld_relaxed_sys_u8_any(const uint8_t *entries, uint64_t at)
-{
-    return (ld_relaxed_sys_u32(entries + (at & ~3ull)) >> (8 * (at & 3ull))) & 0xffu;
-}
-__device__ __forceinline__ uint32_t ld_relaxed_sys_u16_any(const uint8_t *entries, uint64_t at)
-{
-    return ld_relaxed_sys_u8_any(entries, at) | (ld_relaxed_sys_u8_any(entries, at + 1) << 8);
-}
 
 struct ConsEntry {
     uint64_t off;
@@ -298,22 +289,10 @@ struct ConsEntry {
 // stop is the scan kernel's)
 __device__ __forceinline__ ConsEntry cons_classify(const apus_consume_args_t &a, const apus_cons_state_t &s, uint64_t j)
 {
-    const uint8_t *entries = a.region + a.entries_off;
-    const uint32_t *index = reinterpret_cast<const uint32_t *>(a.region + APUS_INDEX_OFF);
-    const uint64_t L = a.log_len;
     ConsEntry e = {0, 0, 0, CONS_OK};
-    e.off = ld_relaxed_sys_u32(&index[(uint32_t)(s.next_idx + j) & a.idx_mask]) & ~APUS_IDX_HEAD_FLAG;
-    if (ring_dist(s.cursor, e.off, L) >= ring_dist(s.cursor, s.committed, L)) { e.status = CONS_LATER; return e; }
-    if (e.off + APUS_HDR_BYTES > L || ld_relaxed_sys_u64_any(entries, e.off + E_IDX) != s.next_idx + j) {
-        e.status = CONS_BAD_IDX;
-        return e;
-    }
-    e.ty = ld_relaxed_sys_u8_any(entries, e.off + E_TYPE);
-    if (has_cmd(e.ty)) {
-        e.len = ld_relaxed_sys_u16_any(entries, e.off + E_DATA);
-        if (e.off + entry_stride(e.ty, e.len) > L) e.status = CONS_BAD_IDX;   // not an entry this log could hold
-        else if (!a.offsets && e.len > a.stride) e.status = CONS_TOO_LONG;
-    }
+    e.status = apus_cons_locate(a.region + a.entries_off, reinterpret_cast<const uint32_t *>(a.region + APUS_INDEX_OFF),
+                                a.idx_mask, a.log_len, s.cursor, s.committed, s.next_idx + j, &e.off, &e.ty, &e.len);
+    if (e.status == CONS_OK && !a.offsets && e.len > a.stride) e.status = CONS_TOO_LONG;   // (len is 0 without a cmd)
     return e;
 }
 
@@ -323,9 +302,9 @@ __global__ void apus_consume_head_kernel(apus_consume_args_t a)
     apus_cons_state_t *s = a.st;
     const apus_ctrl_t *ctrl = reinterpret_cast<const apus_ctrl_t *>(a.region);
     uint64_t committed, held;
-    cons_read(ctrl, committed, held);
-    const uint64_t cursor = ld_relaxed_sys(&ctrl->cons_cur[0]), nidx = ld_relaxed_sys(&ctrl->cons_cur[1]);
-    const uint64_t avail = cons_avail(held, nidx);
+    apus_cons_read(ctrl->cons_rec, committed, held);
+    const uint64_t cursor = apus_ld_relaxed_sys(&ctrl->cons_cur[0]), nidx = apus_ld_relaxed_sys(&ctrl->cons_cur[1]);
+    const uint64_t avail = apus_cons_avail(held, nidx);
     s->cursor = cursor; s->next_idx = nidx; s->committed = committed;
     s->m = s->error ? 0 : (avail < a.max_n ? avail : a.max_n);
 }
@@ -343,7 +322,7 @@ __global__ void __launch_bounds__(APUS_CONS_THREADS) apus_consume_count_kernel(a
     if (j < s.m) e = cons_classify(a, s, j);
     if (j < s.m && e.status != CONS_OK) atomicMin(&first, (uint32_t)j);
     __syncthreads();
-    const bool row = j < s.m && e.status == CONS_OK && has_cmd(e.ty) && j < first;
+    const bool row = j < s.m && e.status == CONS_OK && apus_has_cmd(e.ty) && j < first;
     const uint32_t rows = __syncthreads_count(row);
     uint64_t *blk = reinterpret_cast<uint64_t *>(a.st + 1) + APUS_CONS_BLK_WORDS * blockIdx.x;
     if (threadIdx.x == 0) blk[0] = rows;
@@ -401,7 +380,7 @@ __global__ void __launch_bounds__(APUS_CONS_THREADS) apus_consume_scan_kernel(ap
             const uint64_t own = blk[APUS_CONS_BLK_WORDS * bcap + 1], base = blk[APUS_CONS_BLK_WORDS * bcap + 2];
             ConsEntry e = {0, 0, 0, CONS_LATER};
             if (j < s->m && j < (uint32_t)own) e = cons_classify(a, *s, j);
-            const uint64_t v = e.status == CONS_OK && has_cmd(e.ty) ? e.len : 0u;
+            const uint64_t v = e.status == CONS_OK && apus_has_cmd(e.ty) ? e.len : 0u;
             uint64_t total;
             const uint64_t incl = block_incl_sum(v, &total);
             if (base + incl > a.values_cap && v) atomicMin(&tcap, threadIdx.x);
@@ -424,7 +403,7 @@ __global__ void __launch_bounds__(APUS_CONS_THREADS) apus_consume_scan_kernel(ap
         const uint64_t j = (uint64_t)bcap * APUS_CONS_THREADS + threadIdx.x;
         ConsEntry e = {0, 0, 0, CONS_LATER};
         if (threadIdx.x < tcap) e = cons_classify(a, *s, j);
-        cap_rows = __syncthreads_count(threadIdx.x < tcap && e.status == CONS_OK && has_cmd(e.ty));
+        cap_rows = __syncthreads_count(threadIdx.x < tcap && e.status == CONS_OK && apus_has_cmd(e.ty));
     }
     __syncthreads();
     if (threadIdx.x == 0) {
@@ -443,43 +422,9 @@ __global__ void __launch_bounds__(APUS_CONS_THREADS) apus_consume_scan_kernel(ap
         uint64_t cur = s->cursor;
         if (n_exam) {
             const ConsEntry e = cons_classify(a, *s, n_exam - 1);
-            cur = e.off + entry_stride(e.ty, e.len);
-            if (cur == a.log_len) cur = 0;
+            cur = apus_cons_cursor_after(e.off, e.ty, e.len, a.log_len);
         }
         s->rows = rows; s->n_exam = n_exam; s->new_cursor = cur; s->need_stride = need; s->bytes = s_bytes;
-    }
-}
-
-// `len` bytes from src (log bytes, any alignment) to dst (any alignment), by the `nthr` threads `c` of a group: each
-// writes 16 B-aligned destination chunks, built from the one or two aligned 16 B source chunks that hold them.  Only
-// chunks holding a wanted byte are loaded (they lie inside the entry); destination bytes outside [dst, dst + len) are
-// not written.
-__device__ __forceinline__ void cons_copy_cmd(uint8_t *dst, const uint8_t *src, uint32_t len, uint32_t c, uint32_t nthr)
-{
-    if (!len) return;
-    const uint64_t d = (uint64_t)(uintptr_t)dst, d16 = d & ~15ull, de = d + len;
-    const uint64_t sb = (uint64_t)(uintptr_t)src - (d - d16);         // source address of destination byte d16
-    const uint64_t s_lo = (uint64_t)(uintptr_t)src, s_hi = s_lo + len;
-    const uint32_t nch = (uint32_t)(((de + 15ull) & ~15ull) - d16) >> 4;
-    for (uint32_t q = c; q < nch; q += nthr) {
-        const uint64_t s = sb + 16ull * q, s16 = s & ~15ull;
-        const uint32_t sh = (uint32_t)(s & 15ull);
-        const uint64_t want_lo = s > s_lo ? s : s_lo, want_hi = (s + 16 < s_hi) ? s + 16 : s_hi;
-        uint4 c0 = make_uint4(0, 0, 0, 0), c1 = make_uint4(0, 0, 0, 0);
-        if (want_lo < s16 + 16) c0 = ld_relaxed_sys_v4(reinterpret_cast<const void *>(s16));
-        if (sh && want_hi > s16 + 16) c1 = ld_relaxed_sys_v4(reinterpret_cast<const void *>(s16 + 16));
-        const uint64_t a0 = c0.x | ((uint64_t)c0.y << 32), a1 = c0.z | ((uint64_t)c0.w << 32);
-        const uint64_t a2 = c1.x | ((uint64_t)c1.y << 32), a3 = c1.z | ((uint64_t)c1.w << 32);
-        const uint32_t k = sh >> 3, b = 8u * (sh & 7u);
-        const uint64_t w0 = k ? a1 : a0, w1 = k ? a2 : a1, w2 = k ? a3 : a2;
-        const uint64_t r0 = b ? (w0 >> b) | (w1 << (64u - b)) : w0, r1 = b ? (w1 >> b) | (w2 << (64u - b)) : w1;
-        const uint64_t o = d16 + 16ull * q;
-        if (o >= d && o + 16 <= de) {
-            st_v4(reinterpret_cast<void *>(o), make_uint4((uint32_t)r0, (uint32_t)(r0 >> 32), (uint32_t)r1, (uint32_t)(r1 >> 32)));
-        } else {
-            for (uint32_t i = 0; i < 16; i++)
-                if (o + i >= d && o + i < de) st_u8(reinterpret_cast<void *>(o + i), (uint32_t)(((i < 8 ? r0 : r1) >> (8 * (i & 7))) & 0xffu));
-        }
     }
 }
 
@@ -497,7 +442,7 @@ __global__ void __launch_bounds__(APUS_CONS_THREADS) apus_consume_copy_kernel(ap
     const uint64_t j = (uint64_t)blockIdx.x * APUS_CONS_THREADS + threadIdx.x;
     ConsEntry e = {0, 0, 0, CONS_LATER};
     if (j < s.n_exam) e = cons_classify(a, s, j);
-    const bool live = j < s.n_exam && has_cmd(e.ty);
+    const bool live = j < s.n_exam && apus_has_cmd(e.ty);
     uint32_t tot;
     const uint64_t row = blk[0] + cons_block_excl(live, &tot);
     uint64_t dst = row * a.stride;
@@ -509,8 +454,8 @@ __global__ void __launch_bounds__(APUS_CONS_THREADS) apus_consume_copy_kernel(ap
     if (live) {
         a.idx[row] = s.next_idx + j;
         a.types[row] = (uint8_t)e.ty;
-        a.conns[row] = (uint16_t)ld_relaxed_sys_u16_any(entries, e.off + E_CLTID);
-        a.req_ids[row] = ld_relaxed_sys_u64_any(entries, e.off + E_REQID);
+        a.conns[row] = (uint16_t)apus_ld_u16_any(entries, e.off + E_CLTID);
+        a.req_ids[row] = apus_ld_u64_any(entries, e.off + E_REQID);
         if (a.offsets) a.offsets[row] = dst;
         else a.lens[row] = (uint16_t)e.len;
     }
@@ -519,7 +464,7 @@ __global__ void __launch_bounds__(APUS_CONS_THREADS) apus_consume_copy_kernel(ap
     const uint32_t c = threadIdx.x & 7u;
     for (uint32_t i = threadIdx.x >> 3; i < APUS_CONS_THREADS; i += APUS_CONS_THREADS / 8)
         if (s_len[i] != CONS_NONE)
-            cons_copy_cmd(a.payloads + s_dst[i], entries + s_off[i] + E_CMD, s_len[i], c, 8);
+            apus_copy_cmd(a.payloads + s_dst[i], entries + s_off[i] + E_CMD, s_len[i], c, 8);
 }
 
 // 5: the row count and (packed) offsets[rows], then -- every read of the examined entries has completed with the copy kernel -- the cursor the
@@ -531,11 +476,11 @@ __global__ void apus_consume_tail_kernel(apus_consume_args_t a)
     *a.count = (uint32_t)s->rows;
     if (a.offsets) a.offsets[s->rows] = s->bytes;
     const uint64_t nidx = s->next_idx + s->n_exam;
-    st_relaxed_sys_2x64(ctrl->cons_cur, s->new_cursor, nidx);
-    st_relaxed_sys(&a.hw->cons_cursor, s->new_cursor);
-    st_relaxed_sys(&a.hw->cons_next_idx, nidx);
-    st_relaxed_sys(&a.hw->cons_need_stride, s->need_stride);
-    st_relaxed_sys(&a.hw->cons_error, s->error);
+    apus_st_relaxed_sys_2x64(ctrl->cons_cur, s->new_cursor, nidx);
+    apus_st_relaxed_sys(&a.hw->cons_cursor, s->new_cursor);
+    apus_st_relaxed_sys(&a.hw->cons_next_idx, nidx);
+    apus_st_relaxed_sys(&a.hw->cons_need_stride, s->need_stride);
+    apus_st_relaxed_sys(&a.hw->cons_error, s->error);
 }
 
 // ---------------------------------------------------------------------------------
@@ -546,17 +491,6 @@ __global__ void apus_consume_tail_kernel(apus_consume_args_t a)
 // waiting consumer does not load L2 beside the resident replica kernels, and reads the host's release word over PCIe
 // only every APUS_WAIT_RELEASE_POLL_NS.  It writes nothing the replica kernels read.
 // ---------------------------------------------------------------------------------
-#define APUS_WAIT_SLEEP_MIN_NS     32u
-#define APUS_WAIT_SLEEP_MAX_NS     1024u      // bounds the delay a wait adds to commit-to-applied latency
-#define APUS_WAIT_RELEASE_POLL_NS  20000ull
-
-__device__ __forceinline__ uint64_t globaltimer_ns()
-{
-    uint64_t t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-    return t;
-}
-
 // one step between two polls of a stream-ordered wait (consume waits, read fences), started at t0 on %globaltimer: the
 // release epoch every APUS_WAIT_RELEASE_POLL_NS (t_rel: when it was read last), the deadline, then a back-off sleep
 // (`sleep` doubles up to APUS_WAIT_SLEEP_MAX_NS).  true: the wait ends, with APUS_WAIT_RELEASED or APUS_WAIT_TIMED_OUT
@@ -564,14 +498,10 @@ __device__ __forceinline__ uint64_t globaltimer_ns()
 __device__ __forceinline__ bool wait_backoff(const apus_hostwords_t *hw, uint64_t epoch, uint64_t t0, uint64_t timeout_ns,
                                              uint64_t &t_rel, uint32_t &sleep, uint32_t &why)
 {
-    const uint64_t now = globaltimer_ns();
-    if (now - t_rel >= APUS_WAIT_RELEASE_POLL_NS) {
-        t_rel = now;
-        if (ld_relaxed_sys(&hw->cons_wait_epoch) != epoch) { why = APUS_WAIT_RELEASED; return true; }
-    }
+    const uint64_t now = apus_globaltimer_ns();
+    if (apus_poll_word_moved(&hw->cons_wait_epoch, epoch, now, t_rel)) { why = APUS_WAIT_RELEASED; return true; }
     if (now - t0 >= timeout_ns) { why = APUS_WAIT_TIMED_OUT; return true; }
-    __nanosleep(sleep);
-    if (sleep < APUS_WAIT_SLEEP_MAX_NS) sleep <<= 1;
+    apus_poll_sleep(sleep);
     return false;
 }
 
@@ -579,19 +509,19 @@ __global__ void apus_consume_wait_kernel(const apus_ctrl_t *ctrl, apus_hostwords
                                          uint32_t min_entries, uint64_t timeout_ns, uint32_t *outcome)
 {
     if (threadIdx.x != 0) return;
-    const uint64_t t0 = globaltimer_ns();
+    const uint64_t t0 = apus_globaltimer_ns();
     uint64_t t_rel = t0, avail;
     uint32_t why, sleep = APUS_WAIT_SLEEP_MIN_NS;
     for (;;) {
         uint64_t committed, held;
-        cons_read(ctrl, committed, held);
-        avail = cons_avail(held, ld_relaxed_sys(&ctrl->cons_cur[1]));
+        apus_cons_read(ctrl->cons_rec, committed, held);
+        avail = apus_cons_avail(held, apus_ld_relaxed_sys(&ctrl->cons_cur[1]));
         if (avail >= min_entries) { why = APUS_WAIT_READY; break; }
         if (wait_backoff(hw, epoch, t0, timeout_ns, t_rel, sleep, why)) break;
     }
     if (outcome) *(volatile uint32_t *)outcome = why;
-    st_relaxed_sys(&hw->cons_wait_outcome, why);
-    st_relaxed_sys(&hw->cons_wait_avail, avail);
+    apus_st_relaxed_sys(&hw->cons_wait_outcome, why);
+    apus_st_relaxed_sys(&hw->cons_wait_avail, avail);
 }
 
 // ---------------------------------------------------------------------------------
@@ -602,13 +532,13 @@ __global__ void apus_consume_wait_kernel(const apus_ctrl_t *ctrl, apus_hostwords
 // ---------------------------------------------------------------------------------
 __global__ void apus_consume_mark_kernel(const apus_ctrl_t *ctrl, const apus_cons_state_t *st, uint64_t *mark)
 {
-    const uint64_t cursor = ld_relaxed_sys(&ctrl->cons_cur[0]), nidx = ld_relaxed_sys(&ctrl->cons_cur[1]);
+    const uint64_t cursor = apus_ld_relaxed_sys(&ctrl->cons_cur[0]), nidx = apus_ld_relaxed_sys(&ctrl->cons_cur[1]);
     *reinterpret_cast<ulonglong2 *>(mark) = make_ulonglong2(cursor, st->error ? 0ull : nidx);
 }
 
 // ---------------------------------------------------------------------------------
 // READ FENCES (apus_read_fence): one warp on the consume stream; lane 0 takes the three steps of apus_fence.h.
-//   1. K: the entries-committed word of the leader's consumer record (cons_read's acquire), which its commit warp
+//   1. K: the entries-committed word of the leader's consumer record (apus_cons_read's acquire), which its commit warp
 //      publishes only under APUS_F_APPLY_ANY_ROLE (cons_on == 2); otherwise, or with the leader not mapped, NOT_LEADER.
 //   2. after K (the acquire orders the loads below after it): the SID word of every member this replica maps; fewer
 //      than N/2 + 1 at term <= t ends NOT_LEADER (rf_confirmed).
@@ -621,21 +551,21 @@ __global__ void apus_consume_mark_kernel(const apus_ctrl_t *ctrl, const apus_con
 __global__ void apus_read_fence_kernel(apus_fence_args_t a)
 {
     if (threadIdx.x != 0) return;
-    const uint64_t t0 = globaltimer_ns();
+    const uint64_t t0 = apus_globaltimer_ns();
     uint64_t F = 0;
     uint32_t why = APUS_WAIT_NOT_LEADER;
     const apus_ctrl_t *lead = NULL;
 #pragma unroll
     for (uint32_t i = 0; i < APUS_MAX_SERVERS; i++)
         if (i == a.leader) lead = reinterpret_cast<const apus_ctrl_t *>(a.member[i]);
-    if (lead && ld_relaxed_sys(&lead->cons_on) == 2) {
+    if (lead && apus_ld_relaxed_sys(&lead->cons_on) == 2) {
         uint64_t k_off, K;
-        cons_read(lead, k_off, K);
+        apus_cons_read(lead->cons_rec, k_off, K);
         uint32_t counted = 0;
 #pragma unroll
         for (uint32_t i = 0; i < APUS_MAX_SERVERS; i++)
             if (i < a.n && a.member[i])
-                counted += rf_member_counts(1, ld_relaxed_sys(a.member[i] + APUS_CTL_OFF + offsetof(apus_ctlwords_t, sid)),
+                counted += rf_member_counts(1, apus_ld_relaxed_sys(a.member[i] + APUS_CTL_OFF + offsetof(apus_ctlwords_t, sid)),
                                             a.term);
         if (rf_confirmed(counted, a.n)) {
             const apus_ctrl_t *own = reinterpret_cast<const apus_ctrl_t *>(a.region);
@@ -645,13 +575,13 @@ __global__ void apus_read_fence_kernel(apus_fence_args_t a)
             uint32_t sleep = APUS_WAIT_SLEEP_MIN_NS;
             for (;;) {
                 uint64_t held_off, held, e_idx = 0, e_term = 0;
-                cons_read(own, held_off, held);
+                apus_cons_read(own->cons_rec, held_off, held);
                 if (held && held >= K) {
-                    const uint64_t off = ld_relaxed_sys_u32(&index[(uint32_t)held & a.idx_mask]) & ~APUS_IDX_HEAD_FLAG;
+                    const uint64_t off = apus_ld_relaxed_sys_u32(&index[(uint32_t)held & a.idx_mask]) & ~APUS_IDX_HEAD_FLAG;
                     if (off + APUS_HDR_BYTES <= a.log_len) {
-                        e_idx = ld_relaxed_sys_u64_any(entries, off + E_IDX);
-                        e_term = ld_relaxed_sys_u64_any(entries, off + E_TERM);
-                        if (ld_relaxed_sys_u64_any(entries, off + E_IDX) != e_idx) e_idx = 0;
+                        e_idx = apus_ld_u64_any(entries, off + E_IDX);
+                        e_term = apus_ld_u64_any(entries, off + E_TERM);
+                        if (apus_ld_u64_any(entries, off + E_IDX) != e_idx) e_idx = 0;
                     }
                 }
                 if (rf_ready(held, K, e_idx, e_term, a.term)) { F = held; why = APUS_WAIT_READY; break; }
@@ -661,8 +591,8 @@ __global__ void apus_read_fence_kernel(apus_fence_args_t a)
     }
     if (why == APUS_WAIT_READY) *(volatile uint64_t *)a.index = F;
     if (a.outcome) *(volatile uint32_t *)a.outcome = why;
-    st_relaxed_sys(&a.hw->fence_outcome, why);
-    st_relaxed_sys(&a.hw->fence_index, F);
+    apus_st_relaxed_sys(&a.hw->fence_outcome, why);
+    apus_st_relaxed_sys(&a.hw->fence_index, F);
 }
 
 // ---------------------------------------------------------------------------------

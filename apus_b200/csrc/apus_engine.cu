@@ -28,6 +28,7 @@
 #include "apus_slot.h"
 
 extern "C" cudaError_t apus_launch_roles(const apus_role_t *d_roles, int n_roles, cudaStream_t stream);
+extern "C" cudaError_t apus_kernels_load(void);
 extern "C" size_t apus_kernel_smem_bytes(void);
 extern "C" cudaError_t apus_batch_load(void);
 extern "C" cudaError_t apus_synth_enqueue(apus_slot_t *ring, uint32_t mask, uint8_t *pay, uint64_t first_slot, uint32_t n,
@@ -195,6 +196,8 @@ struct apus_replica {
     apus_cons_state_t *cons_st;   /* consume state + APUS_CONS_BLK_WORDS per consume block (index-ring capacity / block size) */
     pthread_mutex_t cons_mu;      /* one enqueue at a time: the two events are shared by every caller */
     uint64_t cons_enqueued;       /* consume, wait and mark enqueues so far (under cons_mu): a seed needs none */
+    int      attached;            /* a resident consumer moves the cursor (apus_consumer_attach; under cons_mu) ... */
+    cudaStream_t attach_stream;   /* ... launched on this stream */
     apus_replica *live_next;      /* the process's live replicas (g_live, under g_live_mu) */
 };
 
@@ -235,6 +238,14 @@ static inline int is_leader(const apus_replica *r) { return r->cfg.server_idx ==
 static inline void consume_wait_release(apus_replica *r)
 {
     if (r->hw) __atomic_fetch_add(&r->hw->cons_wait_epoch, 1ull, __ATOMIC_SEQ_CST);
+}
+
+/* end the attached resident consumer: move its stop word and wait for the stream it was launched on (under cons_mu) */
+static void consumer_stop(apus_replica *r)
+{
+    __atomic_fetch_add(&r->hw->consumer_stop, 1ull, __ATOMIC_SEQ_CST);
+    cudaStreamSynchronize(r->attach_stream);
+    r->attached = 0;
 }
 
 static int ensure_host_ring(apus_replica *r)
@@ -419,6 +430,12 @@ extern "C" void apus_replica_destroy(apus_replica_t *r)
         }
     }
     DeviceGuard g(r->cfg.device);
+    /* a resident consumer reads the region and the pinned words, and freeing memory waits for every kernel on the GPU:
+     * end it first */
+    if (r->cons_stream) {
+        StageLock cl(&r->cons_mu);
+        if (r->attached) consumer_stop(r);
+    }
     if (r->in_flight && r->hw) {
         r->hw->stop = 1;
         cudaEventSynchronize(r->launch_owner ? r->launch_owner->ev_stop : r->ev_stop);
@@ -1307,10 +1324,12 @@ static int consumer_gate(const apus_replica *r, const char *what, consumer_kind 
  * one) and reads the release epoch that `enqueue(epoch)` hands to a wait or fence: read in the order of the enqueues, so
  * that a release after this call ends what it enqueues. */
 template <typename Enqueue>
-static int cons_stream_run(apus_replica *r, void *stream, const char *what, Enqueue enqueue)
+static int cons_stream_run(apus_replica *r, void *stream, const char *what, Enqueue enqueue, bool moves_cursor = true)
 {
     DeviceGuard g(r->cfg.device);
     StageLock sl(&r->cons_mu);
+    if (moves_cursor && r->attached)
+        return fail("%s: a resident consumer is attached (apus_consumer_detach first): it alone moves the cursor", what);
     const uint64_t epoch = r->hw->cons_wait_epoch;
     r->cons_enqueued++;
     return side_stream_run((cudaStream_t)stream, r->cons_stream, r->ev_cons, what, [&] { return enqueue(epoch); });
@@ -1445,7 +1464,7 @@ extern "C" int apus_read_fence(apus_replica_t *r, uint32_t timeout_us, uint64_t 
         r->fences++;
         const cudaError_t e = apus_read_fence_enqueue(&a, r->cons_stream);
         return e == cudaSuccess ? cudaEventRecord(r->ev_fence, r->cons_stream) : e;
-    });
+    }, false);
 }
 
 extern "C" int apus_read_fence_status(apus_replica_t *r, uint64_t *outcome, uint64_t *index)
@@ -1453,6 +1472,44 @@ extern "C" int apus_read_fence_status(apus_replica_t *r, uint64_t *outcome, uint
     if (consumer_gate(r, "apus_read_fence_status", CONS_ANY_ROLE) != APUS_OK) return APUS_ERROR;
     if (outcome) *outcome = r->hw->fence_outcome;
     if (index) *index = r->hw->fence_index;
+    return APUS_OK;
+}
+
+extern "C" int apus_consumer_attach(apus_replica_t *r, void *stream, apus_consumer_view_t *out)
+{
+    if (consumer_gate(r, "apus_consumer_attach", CONS_STREAM) != APUS_OK) return APUS_ERROR;
+    if (!out) return fail("null argument");
+    DeviceGuard g(r->cfg.device);
+    StageLock sl(&r->cons_mu);
+    if (r->attached) return fail("apus_consumer_attach: a resident consumer is attached already (one per replica)");
+    CK(cudaStreamSynchronize(r->cons_stream));           /* consume work enqueued before: its cursor is where we start */
+    CK(apus_kernels_load());                             /* no lazy load of ours may wait for the consumer from here on */
+    apus_consumer_view_t v;
+    memset(&v, 0, sizeof v);
+    v.entries = r->region + r->entries_off;
+    v.log_len = r->log_len;
+    v.index = reinterpret_cast<const uint32_t *>(r->region + APUS_INDEX_OFF);
+    v.idx_mask = r->idx_cap - 1;
+    v.rec = reinterpret_cast<const uint64_t *>(r->region + offsetof(apus_ctrl_t, cons_rec));
+    v.cur = reinterpret_cast<uint64_t *>(r->region + offsetof(apus_ctrl_t, cons_cur));
+    v.error = &r->cons_st->error;
+    v.status = const_cast<uint64_t *>(&r->hw_dev->cons_cursor);
+    v.stop = const_cast<const uint64_t *>(&r->hw_dev->consumer_stop);
+    v.stop_epoch = r->hw->consumer_stop;
+    r->attached = 1;
+    r->attach_stream = (cudaStream_t)stream;
+    *out = v;
+    return APUS_OK;
+}
+
+extern "C" int apus_consumer_detach(apus_replica_t *r)
+{
+    if (!r) return fail("null argument");
+    DeviceGuard g(r->cfg.device);
+    if (!(r->cfg.flags & APUS_F_DEVICE_APPLY)) return fail("apus_consumer_detach: no resident consumer is attached");
+    StageLock sl(&r->cons_mu);
+    if (!r->attached) return fail("apus_consumer_detach: no resident consumer is attached");
+    consumer_stop(r);
     return APUS_OK;
 }
 

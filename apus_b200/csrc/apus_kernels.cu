@@ -89,7 +89,7 @@ __device__ __forceinline__ uint64_t adopt_head(uint64_t head, uint64_t carried, 
 {
     if (carried >= L) return head;
     const uint64_t ne = (new_end == L) ? 0 : new_end;
-    return (ring_dist(head, carried, L) <= ring_dist(head, ne, L)) ? carried : head;     // only forward, only inside the used region
+    return (apus_ring_dist(head, carried, L) <= apus_ring_dist(head, ne, L)) ? carried : head;     // only forward, only inside the used region
 }
 // the little-endian u64 of the 8 bytes at p, any alignment: the head offset a HEAD entry carries
 __device__ __forceinline__ uint64_t le_u64(const uint8_t *p)
@@ -307,16 +307,16 @@ __device__ __noinline__ void cta_fetch_chunks(uint8_t *dst, const uint8_t *src, 
 {
     uint32_t c = tid;
     for (; c + 3u * nthr < nchunks; c += 4u * nthr) {
-        const uint4 v0 = ld_relaxed_sys_v4(src + 16ull * c);
-        const uint4 v1 = ld_relaxed_sys_v4(src + 16ull * (c + nthr));
-        const uint4 v2 = ld_relaxed_sys_v4(src + 16ull * (c + 2u * nthr));
-        const uint4 v3 = ld_relaxed_sys_v4(src + 16ull * (c + 3u * nthr));
+        const uint4 v0 = apus_ld_relaxed_sys_v4(src + 16ull * c);
+        const uint4 v1 = apus_ld_relaxed_sys_v4(src + 16ull * (c + nthr));
+        const uint4 v2 = apus_ld_relaxed_sys_v4(src + 16ull * (c + 2u * nthr));
+        const uint4 v3 = apus_ld_relaxed_sys_v4(src + 16ull * (c + 3u * nthr));
         reinterpret_cast<uint4 *>(dst)[c] = v0;
         reinterpret_cast<uint4 *>(dst)[c + nthr] = v1;
         reinterpret_cast<uint4 *>(dst)[c + 2u * nthr] = v2;
         reinterpret_cast<uint4 *>(dst)[c + 3u * nthr] = v3;
     }
-    for (; c < nchunks; c += nthr) reinterpret_cast<uint4 *>(dst)[c] = ld_relaxed_sys_v4(src + 16ull * c);
+    for (; c < nchunks; c += nthr) reinterpret_cast<uint4 *>(dst)[c] = apus_ld_relaxed_sys_v4(src + 16ull * c);
 }
 
 // What T2 needs to know about the whole fetched batch, reduced by every producer thread over the descriptors it
@@ -335,7 +335,7 @@ struct DescReduce {
 __device__ __forceinline__ void note_desc(LeaderShared *S, DescReduce &R, uint32_t k, const uint4 v)
 {
     const uint32_t to = v.z, ty = (to >> APUS_SLOT_TYPE_SHIFT) & APUS_SLOT_TYPE_MASK, len = v.w & 0xffffu;
-    const uint32_t es = entry_stride(ty, len), xb = (to & APUS_SLOT_EXT) ? ((data_bytes(ty, len) + 15u) & ~15u) : 0u;
+    const uint32_t es = apus_entry_stride(ty, len), xb = (to & APUS_SLOT_EXT) ? ((data_bytes(ty, len) + 15u) & ~15u) : 0u;
     S->ty[k] = (uint8_t)ty;
     S->flg[k] = (uint8_t)(((to & APUS_SLOT_EXT) ? 1u : 0u) | ((to & APUS_SLOT_WRAP) ? 2u : 0u));
     S->es[k] = es;
@@ -372,7 +372,7 @@ __device__ __noinline__ void cta_fetch_slots(LeaderShared *S, uint8_t *slots, co
             // instead costs real reads -- over PCIe, hundreds of them at one host address)
             const uint32_t qi = q + i * NT, k = qi / 6u, r = qi - 6u * k;
             v[i] = make_uint4(0, 0, 0, 0);
-            if (qi < nq) v[i] = ld_relaxed_sys_v4(src + (size_t)k * APUS_SLOT_BYTES + 16u * (r < 3u ? r : r + 1u));
+            if (qi < nq) v[i] = apus_ld_relaxed_sys_v4(src + (size_t)k * APUS_SLOT_BYTES + 16u * (r < 3u ? r : r + 1u));
         }
 #pragma unroll
         for (uint32_t i = 0; i < 8; i++) {
@@ -444,7 +444,7 @@ __device__ __noinline__ void t1_scan(LeaderShared *S, int tid)
 __device__ __forceinline__ uint64_t ld_apply(const apus_devctx_t *__restrict__ cx, const apus_ctrl_t *ctrl,
                                              const apus_loghdr_t *hdr, int i)
 {
-    return (i == cx->idx || !cx->peer[i]) ? ld_relaxed_sys(&hdr->apply) : ld_relaxed_sys(&ctrl->apply_off[i]);
+    return (i == cx->idx || !cx->peer[i]) ? apus_ld_relaxed_sys(&hdr->apply) : apus_ld_relaxed_sys(&ctrl->apply_off[i]);
 }
 
 // T2b (inside the place turn): place the next sub-tile of the fetched batch (entries kbase..nf) --
@@ -461,7 +461,7 @@ __device__ __noinline__ void leader_place(const apus_devctx_t *__restrict__ cx, 
 
     uint64_t head = S->st.head;                                // refreshed by the caller while blocked
     const uint64_t pos0 = (end == L) ? 0 : end;               // empty log starts at 0 (dare_log.h:216-219)
-    uint64_t used = (end == L) ? 0 : ring_dist(head, end, L);
+    uint64_t used = (end == L) ? 0 : apus_ring_dist(head, end, L);
     // ---- device-side log pruning (log_pruning / force_log_pruning, dare_server.c:1996-2122):
     //      head := the smallest apply offset in the group, published through a HEAD entry
     uint32_t autoh = 0;
@@ -478,7 +478,7 @@ __device__ __noinline__ void leader_place(const apus_devctx_t *__restrict__ cx, 
         L - pos0 >= APUS_HDR_BYTES) {
         uint64_t d = 0;                                   // distance apply -> end, per replica
         if (lane < N) {
-            d = ring_dist(S->ap[lane], end, L);
+            d = apus_ring_dist(S->ap[lane], end, L);
             if (d > used) d = used;                       // never behind the current head (or stale read-ahead)
         }
 #pragma unroll
@@ -486,7 +486,7 @@ __device__ __noinline__ void leader_place(const apus_devctx_t *__restrict__ cx, 
             const uint64_t o = __shfl_xor_sync(0xffffffffu, d, sft);
             d = o > d ? o : d;
         }
-        if (d == 0) d = ring_dist(S->st.tail, end, L);    // leave one entry (dare_server.c:2031-2034)
+        if (d == 0) d = apus_ring_dist(S->st.tail, end, L);    // leave one entry (dare_server.c:2031-2034)
         if (d <= used && used - d >= (L >> 3)) {
             autoh = 1;
             new_head = (end >= d) ? end - d : L - (d - end);
@@ -531,7 +531,7 @@ __device__ __noinline__ void leader_place(const apus_devctx_t *__restrict__ cx, 
             const uint64_t left = L - pos0;
             if (es0 > left && used + left + es0 + reserve < L) {
                 S->gap = 1;
-                S->ghost = (left >= APUS_HDR_BYTES && has_cmd(S->ty[kbase])) ? 1u : 0u;   // header fits: ghost stays behind
+                S->ghost = (left >= APUS_HDR_BYTES && apus_has_cmd(S->ty[kbase])) ? 1u : 0u;   // header fits: ghost stays behind
                 b = L;
             } else {
                 S->blocked = 1;        // back-pressure: wait for head to advance
@@ -551,11 +551,11 @@ __device__ __noinline__ void leader_place(const apus_devctx_t *__restrict__ cx, 
             S->was_blocked = 0;
             S->after_gap = S->gap;
             // commit the placement to the state this CTA carries
-            if (autoh) st_relaxed_sys(&hdr->head, new_head);
+            if (autoh) apus_st_relaxed_sys(&hdr->head, new_head);
             if (autoh) S->st.head = new_head;
             if (S->host_head_k != 0xffffffffu && S->host_head_k >= kbase && S->host_head_k < kbase + m) {
                 const uint64_t nh = adopt_head(S->st.head, le_u64(sl[S->host_head_k].inl), b, L);
-                if (nh != S->st.head) { S->st.head = nh; st_relaxed_sys(&hdr->head, nh); }
+                if (nh != S->st.head) { S->st.head = nh; apus_st_relaxed_sys(&hdr->head, nh); }
             }
             if (S->gap) {
                 S->st.end = 0; S->st_hwm = L;
@@ -593,7 +593,7 @@ __device__ __forceinline__ bool place_acquire(apus_seq_t *seq, uint64_t stamp, P
         ld_relaxed_sys_2x64(seq->rec_tail, s2, tf);
         ld_relaxed_sys_2x64(seq->rec_head, s3, r.head);
         if (s0 == stamp && s1 == stamp && s2 == stamp && s3 == stamp) break;
-        if ((++spins & 0x3ffu) == 0 && ld_relaxed_sys(&seq->abort_flag)) return false;
+        if ((++spins & 0x3ffu) == 0 && apus_ld_relaxed_sys(&seq->abort_flag)) return false;
     }
     r.wrapped = (tf & APUS_REC_WRAPPED) != 0;
     r.prev_head = (tf & APUS_REC_PREV_HEAD) != 0;
@@ -603,11 +603,11 @@ __device__ __forceinline__ bool place_acquire(apus_seq_t *seq, uint64_t stamp, P
 // one thread: hand the place turn to the claim that starts at slot `stamp`
 __device__ __forceinline__ void place_handoff(apus_seq_t *seq, uint64_t stamp, const PlaceRec &r)
 {
-    st_relaxed_sys_2x64(seq->rec_placed, stamp, r.placed);
-    st_relaxed_sys_2x64(seq->rec_end, stamp, r.end);
-    st_relaxed_sys_2x64(seq->rec_tail, stamp,
+    apus_st_relaxed_sys_2x64(seq->rec_placed, stamp, r.placed);
+    apus_st_relaxed_sys_2x64(seq->rec_end, stamp, r.end);
+    apus_st_relaxed_sys_2x64(seq->rec_tail, stamp,
                         r.tail | (r.wrapped ? APUS_REC_WRAPPED : 0ull) | (r.prev_head ? APUS_REC_PREV_HEAD : 0ull));
-    st_relaxed_sys_2x64(seq->rec_head, stamp, r.head);
+    apus_st_relaxed_sys_2x64(seq->rec_head, stamp, r.head);
 }
 
 // lane 0 of the tile path: wait for publish turn `stamp` (unless it is mine already: `h` then holds its record number), then for room in
@@ -626,21 +626,21 @@ __device__ __forceinline__ bool pub_acquire(apus_seq_t *seq, uint64_t stamp, boo
             // acquire: a predecessor that published self-certified data fenced it before this hand-over
             ld_acquire_gpu_2x64(seq->pub_turn, sq, h);
             if (sq == stamp) break;
-            if ((++spins & 0x3ffu) == 0 && ld_relaxed_sys(&seq->abort_flag)) { ok = false; break; }
+            if ((++spins & 0x3ffu) == 0 && apus_ld_relaxed_sys(&seq->abort_flag)) { ok = false; break; }
         }
         if (timed) wait_ns += globaltimer_ns() - t0;
     }
     uint32_t spins = 0;
     while (ok && h - tail_seen >= APUS_PUBRING_RECORDS - 2) {
-        tail_seen = ld_relaxed_sys(&seq->pub_tail);
-        if ((++spins & 0x3ffu) == 0 && ld_relaxed_sys(&seq->abort_flag)) ok = false;
+        tail_seen = apus_ld_relaxed_sys(&seq->pub_tail);
+        if ((++spins & 0x3ffu) == 0 && apus_ld_relaxed_sys(&seq->abort_flag)) ok = false;
     }
     return ok;
 }
 // one thread: hand the publish turn to the claim that starts at slot `stamp`; `h` is the record it will write
 __device__ __forceinline__ void pub_handoff(apus_seq_t *seq, uint64_t stamp, uint64_t h)
 {
-    st_relaxed_sys_2x64(seq->pub_turn, stamp, h);
+    apus_st_relaxed_sys_2x64(seq->pub_turn, stamp, h);
 }
 // lanes 16..23: publish record h, one 16 B {h + 1, value} pair per lane (the PR_* fields of apus_layout.h)
 __device__ __forceinline__ void pub_record(apus_pubrec_t *ring, uint64_t h, int lane, uint64_t cum, uint64_t end,
@@ -651,7 +651,7 @@ __device__ __forceinline__ void pub_record(apus_pubrec_t *ring, uint64_t h, int 
     const int q = lane - 16;
     const uint64_t val = q == PR_CUM ? cum : q == PR_END ? end : q == PR_TICKETS ? tickets : q == PR_T0 ? t0
                        : q == PR_TAIL ? tail : q == PR_HWM ? hwm : q == PR_NEXTIDX ? next_idx : bytes;
-    st_relaxed_sys_2x64(&ring[h & PUBMASK].w[2 * q], h + 1, val);
+    apus_st_relaxed_sys_2x64(&ring[h & PUBMASK].w[2 * q], h + 1, val);
 }
 // warp: lane l looks at pair l & 7 of record rn0 + l / 8, for the first `nrec` (<= 4) records; v is the lane's value.
 // Returns how many of them, in order from rn0, are valid (all eight pairs stamped with their record number + 1).
@@ -701,10 +701,10 @@ __device__ __forceinline__ void push_chunk(uint8_t *entries, uint8_t *mc_entries
         if (mc_entries) {
             mst_v4(mc_entries + lo, v);
         } else {
-            st_v4(entries + lo, v);
+            apus_st_v4(entries + lo, v);
 #pragma unroll 1
             for (int f = 0; f < N; f++)
-                if (peer_entries[f]) st_v4(peer_entries[f] + lo, v);
+                if (peer_entries[f]) apus_st_v4(peer_entries[f] + lo, v);
         }
     } else {
 #pragma unroll 1
@@ -713,10 +713,10 @@ __device__ __forceinline__ void push_chunk(uint8_t *entries, uint8_t *mc_entries
             if (o < a || o >= b) continue;
             const uint32_t w = (j < 4) ? v.x : (j < 8) ? v.y : (j < 12) ? v.z : v.w;
             const uint32_t byte = (w >> (8 * (j & 3))) & 0xff;
-            st_u8(entries + o, byte);
+            apus_st_u8(entries + o, byte);
 #pragma unroll 1
             for (int f = 0; f < N; f++)
-                if (peer_entries[f]) st_u8(peer_entries[f] + o, byte);
+                if (peer_entries[f]) apus_st_u8(peer_entries[f] + o, byte);
         }
     }
 }
@@ -767,17 +767,17 @@ __device__ __noinline__ int leader_express(const apus_devctx_t *__restrict__ cx,
     const uint64_t t_deq = (cx->flags & (APUS_FLAG_STATS | APUS_FLAG_PROFILE)) ? globaltimer_ns() : 0;
 
     if (!have_slot && lane < 8)
-        sv = ld_relaxed_sys_v4(reinterpret_cast<const uint8_t *>(cx->sub_slots + (claimed & cx->sub_mask)) + 16u * lane);
+        sv = apus_ld_relaxed_sys_v4(reinterpret_cast<const uint8_t *>(cx->sub_slots + (claimed & cx->sub_mask)) + 16u * lane);
     const uint32_t to = __shfl_sync(0xffffffffu, sv.z, 0), lw = __shfl_sync(0xffffffffu, sv.w, 0);
     const uint32_t ty = (to >> APUS_SLOT_TYPE_SHIFT) & APUS_SLOT_TYPE_MASK, len = lw & 0xffffu, clt = lw >> 16;
     const uint64_t req_id = (uint64_t)__shfl_sync(0xffffffffu, sv.x, 0) | ((uint64_t)__shfl_sync(0xffffffffu, sv.y, 0) << 32);
-    if (!has_cmd(ty) || (to & APUS_SLOT_EXT)) return 1;
+    if (!apus_has_cmd(ty) || (to & APUS_SLOT_EXT)) return 1;
     const uint32_t es = APUS_HDR_BYTES + len, nb = 2u + len;
 
     // the followers' ack counts (is everybody caught up?) are needed only when the entry is published: in flight meanwhile
     const bool isf = lane < N && lane != me && cx->peer[lane];
     uint64_t ackv = 0;
-    if (isf) ackv = ld_relaxed_sys(&ctrl->ack[lane]);
+    if (isf) ackv = apus_ld_relaxed_sys(&ctrl->ack[lane]);
 
     // ---- place turn (tail and prev_head are not needed here: the entry goes behind `end`, and I hand on my own) ----
     PlaceRec r = X.rec;
@@ -793,7 +793,7 @@ __device__ __noinline__ int leader_express(const apus_devctx_t *__restrict__ cx,
     const bool wrapped = r.wrapped;
     const uint64_t placed = r.placed;
     const uint64_t pos0 = (r.end == L) ? 0 : r.end;
-    const uint64_t used = (r.end == L) ? 0 : ring_dist(r.head, r.end, L);
+    const uint64_t used = (r.end == L) ? 0 : apus_ring_dist(r.head, r.end, L);
     const bool autoprune = (cx->flags & APUS_FLAG_AUTOPRUNE) != 0;
     const uint64_t reserve = autoprune ? APUS_HDR_BYTES : 0;
     // Pruning is the tile machine's business (it appends the HEAD entry): once the ring is half used every request is
@@ -824,7 +824,7 @@ __device__ __noinline__ int leader_express(const apus_devctx_t *__restrict__ cx,
         uint4 oldv = make_uint4(0, 0, 0, 0);
         if (wrapped) {
             if (pf_pos == a) oldv = pf;
-            else if (lane < (int)nch) oldv = ld_relaxed_sys_v4(entries + lo);
+            else if (lane < (int)nch) oldv = apus_ld_relaxed_sys_v4(entries + lo);
         }
         const int j = lane - 3;                                       // data image chunk of this lane
         const int srcl = (j < 0) ? 0 : ((j < 2) ? j + 1 : ((j + 2) & 31));   // slot chunk holding image bytes [16j, 16j+16)
@@ -839,7 +839,7 @@ __device__ __noinline__ int leader_express(const apus_devctx_t *__restrict__ cx,
         // entry at an odd offset (ragged payloads): byte-granular composition in shared memory
         uint8_t *img = scratch, *xsl = scratch + 256;
         if (lane < (int)nch)
-            reinterpret_cast<uint4 *>(img)[lane] = wrapped ? ld_relaxed_sys_v4(entries + lo) : make_uint4(0, 0, 0, 0);
+            reinterpret_cast<uint4 *>(img)[lane] = wrapped ? apus_ld_relaxed_sys_v4(entries + lo) : make_uint4(0, 0, 0, 0);
         if (lane == 1 || lane == 2) reinterpret_cast<uint4 *>(xsl)[lane - 1] = sv;   // inline image bytes 0..31
         if (lane >= 4 && lane <= 6) reinterpret_cast<uint4 *>(xsl)[lane - 2] = sv;   // ... 32..79
         __syncwarp();
@@ -880,7 +880,7 @@ __device__ __noinline__ int leader_express(const apus_devctx_t *__restrict__ cx,
             for (;;) {
                 ld_acquire_gpu_2x64(seq->pub_turn, sq, h);
                 if (sq == claimed) break;
-                if ((++spins & 0x3ffu) == 0 && ld_relaxed_sys(&seq->abort_flag)) { ab = 1; break; }
+                if ((++spins & 0x3ffu) == 0 && apus_ld_relaxed_sys(&seq->abort_flag)) { ab = 1; break; }
             }
         }
         ab = __shfl_sync(0xffffffffu, ab, 0);
@@ -890,8 +890,8 @@ __device__ __noinline__ int leader_express(const apus_devctx_t *__restrict__ cx,
     if (lane == 0) {
         uint32_t spins = 0;
         while (h - S->pub_tail_seen >= APUS_PUBRING_RECORDS - 2) {
-            S->pub_tail_seen = ld_relaxed_sys(&seq->pub_tail);
-            if ((++spins & 0x3ffu) == 0 && ld_relaxed_sys(&seq->abort_flag)) { ab = 1; break; }
+            S->pub_tail_seen = apus_ld_relaxed_sys(&seq->pub_tail);
+            if ((++spins & 0x3ffu) == 0 && apus_ld_relaxed_sys(&seq->abort_flag)) { ab = 1; break; }
         }
     }
     if (__shfl_sync(0xffffffffu, ab, 0)) return 2;
@@ -907,11 +907,11 @@ __device__ __noinline__ int leader_express(const apus_devctx_t *__restrict__ cx,
     if (isf) {
         apus_ctrl_t *pc = reinterpret_cast<apus_ctrl_t *>(cx->peer[lane]);
         if (cert) {
-            st_relaxed_sys_2x64(&pc->pub_csum, cs + cs_key(cumt), a);
-            st_relaxed_sys_2x64(&pc->pub_end, ne | APUS_PUB_CERT, cumt);
+            apus_st_relaxed_sys_2x64(&pc->pub_csum, cs + cs_key(cumt), a);
+            apus_st_relaxed_sys_2x64(&pc->pub_end, ne | APUS_PUB_CERT, cumt);
         } else {
             __threadfence_system();                                  // data before tail (I1), the classic way
-            st_relaxed_sys_2x64(&pc->pub_end, ne, cumt);
+            apus_st_relaxed_sys_2x64(&pc->pub_end, ne, cumt);
         }
     }
     pub_record(pubring, h, lane, cum, ne, claimed + 1, t_deq, a, nw ? L : b, idx + 1, (uint64_t)es * (uint64_t)(N - 1));
@@ -963,7 +963,7 @@ __device__ __forceinline__ bool tail_pub_verify(const TailPub &p, uint64_t old_e
     uint64_t cs = 0;
     if (nch <= 12) {
         if (lane >= 4 && lane < 4 + (int)nch) cs = cs_chunk(spec, spec_lo, a, b);
-    } else if (lane < (int)nch) cs = cs_chunk(ld_relaxed_sys_v4(entries + a16 + 16ull * lane), a16 + 16ull * lane, a, b);
+    } else if (lane < (int)nch) cs = cs_chunk(apus_ld_relaxed_sys_v4(entries + a16 + 16ull * lane), a16 + 16ull * lane, a, b);
 #pragma unroll
     for (int sft = 16; sft > 0; sft >>= 1) cs += __shfl_xor_sync(0xffffffffu, cs, sft);
     return (cs + cs_key(term_word(p.cum, term))) == p.csum;
@@ -997,9 +997,9 @@ __device__ __forceinline__ uint64_t commit_pub_offset(uint64_t off, uint64_t ter
 // ticket target) that count belongs to -- so that the follower can leave once it has acked and applied all of them
 __device__ __forceinline__ void fin_publish(apus_ctrl_t *pc, uint64_t entries, uint64_t target)
 {
-    st_relaxed_sys(&pc->fin_entries, entries);
+    apus_st_relaxed_sys(&pc->fin_entries, entries);
     __threadfence_system();
-    st_relaxed_sys(&pc->fin_target, target);
+    apus_st_relaxed_sys(&pc->fin_target, target);
 }
 // follower warp: has the leader ended the launch `target`?  `entries` is then its count of entries (every lane)
 __device__ __forceinline__ bool fin_read(const apus_ctrl_t *ctrl, uint64_t target, int lane, uint64_t &entries)
@@ -1007,7 +1007,7 @@ __device__ __forceinline__ bool fin_read(const apus_ctrl_t *ctrl, uint64_t targe
     uint64_t ft = 0;
     if (lane == 0) ft = ld_acquire_sys(&ctrl->fin_target);
     if (__shfl_sync(0xffffffffu, ft, 0) != target) return false;
-    entries = ld_relaxed_sys(&ctrl->fin_entries);
+    entries = apus_ld_relaxed_sys(&ctrl->fin_entries);
     return true;
 }
 
@@ -1019,7 +1019,7 @@ __device__ __forceinline__ uint32_t cw_probe(CommitWarp &C, int lane, uint64_t &
     if (nvalid) {
         C.published = pubrec_field(rv, nvalid - 1, PR_CUM);
         C.seen += nvalid;
-        if (lane == 0) st_relaxed_sys(&C.ctrl->pub_seen, C.published);
+        if (lane == 0) apus_st_relaxed_sys(&C.ctrl->pub_seen, C.published);
     }
     return nvalid;
 }
@@ -1029,7 +1029,7 @@ __device__ __forceinline__ uint32_t cw_probe(CommitWarp &C, int lane, uint64_t &
 __device__ __forceinline__ uint64_t cw_quorum(const CommitWarp &C, int lane)
 {
     uint64_t v = 0;
-    if (lane < C.N && lane != C.me) v = ld_relaxed_sys(&C.ctrl->ack[lane]);
+    if (lane < C.N && lane != C.me) v = apus_ld_relaxed_sys(&C.ctrl->ack[lane]);
     if (lane == C.me) v = C.published;
     // rank: how many replicas hold at least what I hold
     int cnt = 0;
@@ -1090,13 +1090,13 @@ __device__ __forceinline__ void cw_commit(const apus_devctx_t *__restrict__ cx, 
     apus_ctrl_t *ctrl = C.ctrl;
     apus_loghdr_t *hdr = C.hdr;
     const uint64_t off = r.end, tickets = r.tickets;
-    if (C.peer) st_relaxed_sys_2x64(C.peer->pub_commit, off, cx->term);
+    if (C.peer) apus_st_relaxed_sys_2x64(C.peer->pub_commit, off, cx->term);
     if (lane == 0) {
         // {commit offset, committed tickets}: ONE 16 B store into pinned host memory -- this is what
         // releases the proxy.c:160 spinners; a 16 B host load sees a consistent pair
-        st_relaxed_sys_2x64(&C.hw->commit_off, off, tickets);
-        st_relaxed_sys(&C.hw->consumed, tickets);                 // submission-ring space
-        st_relaxed_sys(&C.hw->last_commit_ns, globaltimer_ns());
+        apus_st_relaxed_sys_2x64(&C.hw->commit_off, off, tickets);
+        apus_st_relaxed_sys(&C.hw->consumed, tickets);                 // submission-ring space
+        apus_st_relaxed_sys(&C.hw->last_commit_ns, globaltimer_ns());
         if (cx->flags & APUS_FLAG_APPLY_ANY_ROLE) {
             // my own device consumers: acquire the PR_END pair of every record this advance commits (each stored
             // behind its own writer's fence), then release the consumer record over them (apus_dev.h).  Before
@@ -1105,10 +1105,10 @@ __device__ __forceinline__ void cw_commit(const apus_devctx_t *__restrict__ cx, 
             for (uint64_t h = t0; h != C.tail; h++) ld_acquire_gpu_2x64(&C.ring[h & PUBMASK].w[2 * PR_END], st_, end_);
             cons_publish_gpu(ctrl, off, C.committed);
         }
-        st_relaxed_sys(&C.seq->pub_tail, C.tail);                 // publish-ring space
+        apus_st_relaxed_sys(&C.seq->pub_tail, C.tail);                 // publish-ring space
         hdr->commit = off;
         // leader applies = update_state; with device consumers my apply offset is their cursor (cw_forward_apply)
-        if (!(cx->flags & APUS_FLAG_APPLY_ANY_ROLE)) st_relaxed_sys(&hdr->apply, off);
+        if (!(cx->flags & APUS_FLAG_APPLY_ANY_ROLE)) apus_st_relaxed_sys(&hdr->apply, off);
         hdr->end = off; hdr->tail = r.tail; hdr->old_end = off;
         ctrl->committed = C.committed; ctrl->committed_tickets = tickets; ctrl->lat_count = C.lat_count;
         ctrl->published = C.committed; ctrl->consumed = tickets; ctrl->next_idx = r.next_idx; ctrl->hwm = r.hwm;
@@ -1127,7 +1127,7 @@ __device__ __forceinline__ void cw_heartbeat(const apus_devctx_t *__restrict__ c
         const uint64_t now = globaltimer_ns();
         if (now - C.last_hb >= cx->hb_period_ns) {
             C.last_hb = now; C.hb_beat++;
-            if (C.peer) st_relaxed_sys(&C.peer->hb, term_word(C.hb_beat, cx->term));
+            if (C.peer) apus_st_relaxed_sys(&C.peer->hb, term_word(C.hb_beat, cx->term));
         }
     }
 }
@@ -1138,7 +1138,7 @@ __device__ __forceinline__ void cw_heartbeat(const apus_devctx_t *__restrict__ c
 __device__ __forceinline__ void cw_forward_apply(const apus_devctx_t *__restrict__ cx, const CommitWarp &C, int lane, bool last)
 {
     if ((cx->flags & APUS_FLAG_APPLY_ANY_ROLE) && lane == 0 && (last || (C.spins & 0x3fu) == 0))
-        st_relaxed_sys(&C.hdr->apply, ld_relaxed_sys(&C.ctrl->cons_cur[0]));
+        apus_st_relaxed_sys(&C.hdr->apply, apus_ld_relaxed_sys(&C.ctrl->cons_cur[0]));
 }
 
 // exit decision: 1 every worker finished and nothing is in flight, 2 abort (or the watchdog), 0 go on
@@ -1150,11 +1150,11 @@ __device__ __forceinline__ int cw_exit(const apus_devctx_t *__restrict__ cx, Com
         if (!new_records && C.tail == C.seen && C.committed == C.published && ld_acquire_gpu(&seq->workers_done) == cx->n_workers) {
             ex = 3;
         } else if ((++C.spins & 0x3ffu) == 0) {
-            if (ld_relaxed_sys(&seq->abort_flag)) ex = 2;
+            if (apus_ld_relaxed_sys(&seq->abort_flag)) ex = 2;
             else if (globaltimer_ns() - C.last_progress > WATCHDOG_NS && (C.tail != C.seen || C.committed != C.published) &&
-                     (cx->target != ~0ull || ld_relaxed_sys_u32(&C.hw->stop))) {
-                st_relaxed_sys(&C.hw->error, APUS_KERR_WATCHDOG_COMMIT);
-                st_relaxed_sys(&seq->abort_flag, 1);
+                     (cx->target != ~0ull || apus_ld_relaxed_sys_u32(&C.hw->stop))) {
+                apus_st_relaxed_sys(&C.hw->error, APUS_KERR_WATCHDOG_COMMIT);
+                apus_st_relaxed_sys(&seq->abort_flag, 1);
                 ex = 2;
             }
         }
@@ -1241,21 +1241,21 @@ __device__ __forceinline__ void t0_claim(const apus_devctx_t *__restrict__ cx, L
     uint64_t claimed = 0;
     const bool poll_slot = cx->slot_poll != 0 && wid == 0;
     const bool express_on = (cx->flags & APUS_FLAG_NO_EXPRESS) == 0;
-    if (wid == 0 && lane == 0) st_relaxed_sys(&seq->w0_idle, 1);
+    if (wid == 0 && lane == 0) apus_st_relaxed_sys(&seq->w0_idle, 1);
     for (;;) {
         // worker 0 polls the NEXT SLOT itself (lanes 0..7, one 128 B read over PCIe) while lane 0 looks at the
         // claim counter and the doorbell: a lone request is in registers one PCIe round trip after the host wrote it
         uint4 sv = make_uint4(0, 0, 0, 0);
         const uint64_t sv_for = xguess;
         if (poll_slot && lane < 8)
-            sv = ld_relaxed_sys_v4(reinterpret_cast<const uint8_t *>(cx->sub_slots + (xguess & cx->sub_mask)) + 16u * lane);
+            sv = apus_ld_relaxed_sys_v4(reinterpret_cast<const uint8_t *>(cx->sub_slots + (xguess & cx->sub_mask)) + 16u * lane);
         // (a second poll in flight does not help: two loads of one line from one SM are merged, the younger one
         //  returns the older one's sample, and the extra load only lengthens the loop)
         // idle-time prefetch: the bytes the log holds where the NEXT entry will go (its holes keep them); the offset
         // is known as long as this warp placed the latest entry
         if (express_on && X.have_place && X.rec.end != cx->log_len && X.rec.wrapped && pf_pos != X.rec.end &&
             (X.rec.end & 15ull) == 0 && X.rec.end + 16ull * 12 <= cx->log_len) {
-            if (lane < 12) pf = ld_relaxed_sys_v4(entries + X.rec.end + 16ull * lane);
+            if (lane < 12) pf = apus_ld_relaxed_sys_v4(entries + X.rec.end + 16ull * lane);
             pf_pos = X.rec.end;
         }
         // lane 0: one round trip of independent loads (the averages are small: their low 32 bits hold them); the
@@ -1263,11 +1263,11 @@ __device__ __forceinline__ void t0_claim(const apus_devctx_t *__restrict__ cx, L
         uint32_t ctl = 0, aes = 0, axb = 0;
         uint64_t t = 0, w0i = 0, ab = 0;
         if (lane == 0) {
-            if ((spins & 0x3fu) == 0) ab = ld_relaxed_sys(&seq->abort_flag);
-            t = cx->doorbell_relay ? ld_relaxed_sys(&seq->doorbell) : ld_relaxed_sys(cx->sub_tail);
-            claimed = ld_relaxed_sys(&seq->claimed_slots);
-            if (wid != 0) w0i = ld_relaxed_sys(&seq->w0_idle);
-            aes = ld_relaxed_sys_u32(&seq->avg_es); axb = ld_relaxed_sys_u32(&seq->avg_xb);
+            if ((spins & 0x3fu) == 0) ab = apus_ld_relaxed_sys(&seq->abort_flag);
+            t = cx->doorbell_relay ? apus_ld_relaxed_sys(&seq->doorbell) : apus_ld_relaxed_sys(cx->sub_tail);
+            claimed = apus_ld_relaxed_sys(&seq->claimed_slots);
+            if (wid != 0) w0i = apus_ld_relaxed_sys(&seq->w0_idle);
+            aes = apus_ld_relaxed_sys_u32(&seq->avg_es); axb = apus_ld_relaxed_sys_u32(&seq->avg_xb);
             // worker 0 waits for its slot poll (a PCIe round trip) in every pass anyway: there, a doorbell that shows
             // requests is re-read with acquire at once, under the poll, and not beside the compare-and-swap
             if (poll_slot && t > claimed) t = cx->doorbell_relay ? ld_acquire_gpu(&seq->doorbell) : ld_acquire_sys(cx->sub_tail);
@@ -1323,7 +1323,7 @@ __device__ __forceinline__ void t0_claim(const apus_devctx_t *__restrict__ cx, L
                     if (was == claimed) { won = 1; break; }
                     claimed = was;
                     if (claimed >= cx->target) break;
-                    if ((lost & 0x3fu) == 0x3fu && ld_relaxed_sys(&seq->abort_flag)) break;
+                    if ((lost & 0x3fu) == 0x3fu && apus_ld_relaxed_sys(&seq->abort_flag)) break;
                     avail = t > claimed ? t - claimed : 0;
                     // a lone request: worker 0 waits for its slot poll (the next pass), the others leave it to worker 0
                     if (avail == 1 && ((poll_slot && express_on) || (wid != 0 && w0i))) avail = 0;
@@ -1354,10 +1354,10 @@ __device__ __forceinline__ void t0_claim(const apus_devctx_t *__restrict__ cx, L
             // stop / watchdog (the abort flag is not raised on a stop: this worker holds no turn)
             uint32_t stopf = 0;
             if (lane == 0) {
-                if (ld_relaxed_sys_u32(&hw->stop)) stopf = 1;
+                if (apus_ld_relaxed_sys_u32(&hw->stop)) stopf = 1;
                 else if (cx->target != ~0ull && globaltimer_ns() - last_progress > WATCHDOG_NS) {
-                    st_relaxed_sys(&hw->error, APUS_KERR_WATCHDOG_LEADER);
-                    st_relaxed_sys(&seq->abort_flag, 1); stopf = 1;
+                    apus_st_relaxed_sys(&hw->error, APUS_KERR_WATCHDOG_LEADER);
+                    apus_st_relaxed_sys(&seq->abort_flag, 1); stopf = 1;
                 }
                 P.flush(ctrl);
             }
@@ -1368,7 +1368,7 @@ __device__ __forceinline__ void t0_claim(const apus_devctx_t *__restrict__ cx, L
     if (X.hold) express_release(seq, X, lane);
     X.have_place = 0; pf_pos = ~0ull;                  // other workers may place in between
     if (lane == 0) {
-        if (wid == 0) st_relaxed_sys(&seq->w0_idle, 0);
+        if (wid == 0) apus_st_relaxed_sys(&seq->w0_idle, 0);
         if (P.on) { P.tn[0] += globaltimer_ns() - tw0; P.tn[6]++; }
         if (n) S->slot0 = claimed;
         S->n_fetch = n; S->finish = fin;
@@ -1412,7 +1412,7 @@ __device__ __forceinline__ void place_fast(const apus_devctx_t *__restrict__ cx,
     if (!got) { S->abort = 1; S->fast = 1; S->blocked = 0; return; }   // no stamp: nothing may be placed
 
     const uint64_t pos0 = (r.end == L) ? 0 : r.end;
-    const uint64_t used = (r.end == L) ? 0 : ring_dist(r.head, r.end, L);
+    const uint64_t used = (r.end == L) ? 0 : apus_ring_dist(r.head, r.end, L);
     const uint64_t total = S->cum_es[nf - 1];
     const bool autoprune = (cx->flags & APUS_FLAG_AUTOPRUNE) != 0;
     const uint64_t reserve = autoprune ? APUS_HDR_BYTES : 0;
@@ -1425,11 +1425,11 @@ __device__ __forceinline__ void place_fast(const apus_devctx_t *__restrict__ cx,
         }
         uint64_t d = 0;
         for (int i = 0; i < cx->group_size; i++) {
-            uint64_t di = ring_dist(S->ap[i], r.end, L);
+            uint64_t di = apus_ring_dist(S->ap[i], r.end, L);
             if (di > used) di = used;
             d = di > d ? di : d;
         }
-        if (d == 0) d = ring_dist(r.tail, r.end, L);
+        if (d == 0) d = apus_ring_dist(r.tail, r.end, L);
         prune_due = (d <= used && used - d >= (L >> 3));
     }
     const bool fits = !prune_due && pos0 + total <= L && total <= APUS_LEADER_IMG_BYTES - 16u - (pos0 & 15u) &&
@@ -1448,7 +1448,7 @@ __device__ __forceinline__ void place_fast(const apus_devctx_t *__restrict__ cx,
     uint64_t headv = r.head;
     if (S->host_head_k != 0xffffffffu) {          // a HEAD entry submitted by the host carries the new head
         const uint64_t nh = adopt_head(headv, le_u64(sl[S->host_head_k].inl), ne, L);
-        if (nh != headv) { headv = nh; st_relaxed_sys(&hdr->head, nh); }
+        if (nh != headv) { headv = nh; apus_st_relaxed_sys(&hdr->head, nh); }
     }
     // hand the turn on at once ...
     const PlaceRec nr = {r.placed + nf, ne, nt, headv, nw, false};
@@ -1548,7 +1548,7 @@ __device__ __noinline__ void t3_prefill(const apus_devctx_t *__restrict__ cx, Le
 #pragma unroll
             for (int q = 0; q < 4; q++) {
                 v[q] = make_uint4(0, 0, 0, 0);
-                if (!fresh && lo[q] >= a16 && lo[q] < hi16) v[q] = ld_relaxed_sys_v4(entries + lo[q]);
+                if (!fresh && lo[q] >= a16 && lo[q] < hi16) v[q] = apus_ld_relaxed_sys_v4(entries + lo[q]);
             }
 #pragma unroll
             for (int q = 0; q < 4; q++)
@@ -1688,7 +1688,7 @@ __device__ __forceinline__ void t6_publish(const apus_devctx_t *__restrict__ cx,
     if (S->abort) return;
     if (pubs) {
         apus_ctrl_t *pc = reinterpret_cast<apus_ctrl_t *>(cx->peer[lane]);
-        st_relaxed_sys_2x64(&pc->pub_end, S->new_end, term_word(S->cum_after, cx->term));
+        apus_st_relaxed_sys_2x64(&pc->pub_end, S->new_end, term_word(S->cum_after, cx->term));
     }
     pub_record(pubring, S->pub_h, lane, S->cum_after, S->new_end, S->slot0 + S->kbase + S->m, S->t_dequeue,
                S->tail_after, S->hwm_after, S->idx0 + S->m + S->auto_head, (S->b - S->a + gap_bytes) * (uint64_t)(N - 1));
@@ -1745,13 +1745,13 @@ __device__ void leader_main(const apus_devctx_t *__restrict__ cx, const uint32_t
         else if (wid == 1 && cx->doorbell_relay && lane == 0) {
             // doorbell relay: the only poller of the host-mapped doorbell (one PCIe read in flight instead
             // of one per idle worker -- those reads also slow every system fence down); workers poll the mirror
-            uint64_t last = ld_relaxed_sys(&seq->doorbell);
+            uint64_t last = apus_ld_relaxed_sys(&seq->doorbell);
             uint32_t spins = 0;
             for (;;) {
                 const uint64_t t = ld_acquire_sys(cx->sub_tail);
                 if (t != last) { st_release_gpu(&seq->doorbell, t); last = t; }   // slots were written before the doorbell
                 if ((++spins & 0x3fu) == 0 &&
-                    (ld_relaxed_sys(&seq->abort_flag) || ld_relaxed_sys(&seq->workers_done) >= cx->n_workers)) break;
+                    (apus_ld_relaxed_sys(&seq->abort_flag) || apus_ld_relaxed_sys(&seq->workers_done) >= cx->n_workers)) break;
             }
         }
         return;
@@ -1781,8 +1781,8 @@ __device__ void leader_main(const apus_devctx_t *__restrict__ cx, const uint32_t
         P.phase(1);
         if (tid == 32) {
             // entry-size statistics of this claim (sizes the next one)
-            st_relaxed_sys(&seq->avg_es, (S->cum_es[nf - 1] + nf - 1) / nf);
-            st_relaxed_sys(&seq->avg_xb, (S->cum_xb[nf - 1] + nf - 1) / nf);
+            apus_st_relaxed_sys(&seq->avg_es, (S->cum_es[nf - 1] + nf - 1) / nf);
+            apus_st_relaxed_sys(&seq->avg_xb, (S->cum_xb[nf - 1] + nf - 1) / nf);
         }
         bool have_pub_turn = false, have_place_turn = false, aborted = false;
         uint64_t gap_bytes = 0;      // bytes of a wrap gap replicated ahead of the next publish
@@ -1798,10 +1798,10 @@ __device__ void leader_main(const apus_devctx_t *__restrict__ cx, const uint32_t
             if (S->blocked) {   // no space before head: poll again
                 if (tid == 0) {
                     // (a stop raises the abort flag here: this worker holds the place turn, the others wait for it)
-                    if (ld_relaxed_sys_u32(&hw->stop) || ld_relaxed_sys(&seq->abort_flag)) { st_relaxed_sys(&seq->abort_flag, 1); S->finish = 1; }
+                    if (apus_ld_relaxed_sys_u32(&hw->stop) || apus_ld_relaxed_sys(&seq->abort_flag)) { apus_st_relaxed_sys(&seq->abort_flag, 1); S->finish = 1; }
                     else if (cx->target != ~0ull && globaltimer_ns() - last_progress > WATCHDOG_NS) {
-                        st_relaxed_sys(&hw->error, APUS_KERR_WATCHDOG_LEADER);
-                        st_relaxed_sys(&seq->abort_flag, 1); S->finish = 1;
+                        apus_st_relaxed_sys(&hw->error, APUS_KERR_WATCHDOG_LEADER);
+                        apus_st_relaxed_sys(&seq->abort_flag, 1); S->finish = 1;
                     }
                 }
                 if (tid < N) S->ap[tid] = ld_apply(cx, ctrl, hdr, tid);
@@ -1875,19 +1875,19 @@ __device__ __forceinline__ bool f_housekeeping(const apus_devctx_t *__restrict__
     uint32_t stopf = 0;
     uint64_t ha = W.host_applied;
     if (lane == 0) {
-        if (ld_relaxed_sys_u32(&A.hw->stop)) stopf = 1;
+        if (apus_ld_relaxed_sys_u32(&A.hw->stop)) stopf = 1;
         else if (cx->target != ~0ull && globaltimer_ns() - R.last_progress > WATCHDOG_NS) {
-            st_relaxed_sys(&A.hw->error, APUS_KERR_WATCHDOG_FOLLOWER);
+            apus_st_relaxed_sys(&A.hw->error, APUS_KERR_WATCHDOG_FOLLOWER);
             stopf = 1;
         }
         // failure detector (hb_receive_cb, dare_server.c:866-993): the leader's beats stopped
         if (cx->hb_timeout_ns && !W.suspected && globaltimer_ns() - W.last_hb_t > cx->hb_timeout_ns)
-            st_relaxed_sys(&A.hw->leader_suspect, 1 + cx->term);
-        if (A.flags & APUS_FLAG_HOST_APPLY) ha = ld_relaxed_sys(&A.hw->host_apply);
-        else if (A.flags & APUS_FLAG_DEVICE_APPLY) ha = ld_relaxed_sys(&A.ctrl->cons_cur[0]);
+            apus_st_relaxed_sys(&A.hw->leader_suspect, 1 + cx->term);
+        if (A.flags & APUS_FLAG_HOST_APPLY) ha = apus_ld_relaxed_sys(&A.hw->host_apply);
+        else if (A.flags & APUS_FLAG_DEVICE_APPLY) ha = apus_ld_relaxed_sys(&A.ctrl->cons_cur[0]);
     }
     if (cx->hb_timeout_ns && globaltimer_ns() - W.last_hb_t > cx->hb_timeout_ns) W.suspected = true;
-    if (lane == 0) st_relaxed_sys(&A.lctrl->fbeat[A.me], ++W.fbeat);          // I am alive (leader's failure detector)
+    if (lane == 0) apus_st_relaxed_sys(&A.lctrl->fbeat[A.me], ++W.fbeat);          // I am alive (leader's failure detector)
     stopf = __shfl_sync(0xffffffffu, stopf, 0);
     ha = __shfl_sync(0xffffffffu, ha, 0);
     if ((A.flags & (APUS_FLAG_HOST_APPLY | APUS_FLAG_DEVICE_APPLY)) && ha != W.host_applied) {
@@ -1895,7 +1895,7 @@ __device__ __forceinline__ bool f_housekeeping(const apus_devctx_t *__restrict__
         // replica reports to the leader's pruning rule is what the HOST has replayed, or what the device consumers
         // have finished reading (the consume work moves its cursor only after its last read of those entries)
         W.host_applied = ha;
-        if (lane == 0) { A.hdr->apply = ha; st_relaxed_sys(&A.lctrl->apply_off[A.me], ha); }
+        if (lane == 0) { A.hdr->apply = ha; apus_st_relaxed_sys(&A.lctrl->apply_off[A.me], ha); }
     }
     return stopf != 0;
 }
@@ -1917,11 +1917,11 @@ __device__ __forceinline__ void f_poll(const apus_devctx_t *__restrict__ cx, con
         const uint64_t spec_a = (R.old_end == A.L) ? 0 : R.old_end;
         const uint64_t spec_lo = (spec_a & ~15ull) + 16ull * (uint64_t)(lane - 4);
         uint4 spec = make_uint4(0, 0, 0, 0);
-        if (lane == 0) ld_acquire_sys_2x64(&A.ctrl->pub_end, x0, x1);
+        if (lane == 0) apus_ld_acquire_sys_2x64(&A.ctrl->pub_end, x0, x1);
         else if (lane == 1) ld_relaxed_sys_2x64(&A.ctrl->pub_csum, x0, x1);
         else if (lane == 2) ld_relaxed_sys_2x64(A.ctrl->pub_commit, x0, x1);
-        else if (lane == 3) x0 = ld_relaxed_sys(&A.ctrl->hb);
-        else if (lane < 16 && spec_lo + 16 <= A.L) spec = ld_relaxed_sys_v4(A.entries + spec_lo);
+        else if (lane == 3) x0 = apus_ld_relaxed_sys(&A.ctrl->hb);
+        else if (lane < 16 && spec_lo + 16 <= A.L) spec = apus_ld_relaxed_sys_v4(A.entries + spec_lo);
         const uint64_t e = __shfl_sync(0xffffffffu, x0, 0), cumt = __shfl_sync(0xffffffffu, x1, 0);
         const uint64_t csum = __shfl_sync(0xffffffffu, x0, 1), start = __shfl_sync(0xffffffffu, x1, 1);
         p = tail_pub_decode(e, cumt, csum, start, cx->term);
@@ -1946,14 +1946,14 @@ __device__ __forceinline__ void f_poll(const apus_devctx_t *__restrict__ cx, con
         uint64_t fe;
         if (cx->target != ~0ull && fin_read(A.ctrl, cx->target, lane, fe) &&
             R.acked >= fe && (R.old_end == A.L || (R.applied == R.old_end && c == R.old_end))) { done = 1; cum_seen = R.acked; break; }
-        if (hbw != W.last_hb) { W.last_hb = hbw; W.last_hb_t = globaltimer_ns(); if (lane == 0) st_relaxed_sys(&A.hw->hb_seen, hbw); }
+        if (hbw != W.last_hb) { W.last_hb = hbw; W.last_hb_t = globaltimer_ns(); if (lane == 0) apus_st_relaxed_sys(&A.hw->hb_seen, hbw); }
         if ((++W.spins & 0xffu) == 0 && f_housekeeping(cx, A, R, W, lane)) { done = 1; cum_seen = R.acked; break; }
     }
     // early ack: the tail publish was observed with acquire semantics (or its certificate verified), so every
     // entry up to it is resident and visible here (invariant I2); the reply bytes follow behind the ack word
     // unless APUS_F_FENCED_ACK asks for them first
     if (lane == 0) {
-        if (!done && !(A.flags & APUS_FLAG_FENCED_ACK) && cum_seen > R.acked) st_relaxed_sys(&A.lctrl->ack[A.me], cum_seen);
+        if (!done && !(A.flags & APUS_FLAG_FENCED_ACK) && cum_seen > R.acked) apus_st_relaxed_sys(&A.lctrl->ack[A.me], cum_seen);
         S->end_seen = p.end; S->cum_seen = cum_seen; S->commit_seen = c; S->done = done;
         S->cert = (cum_seen > R.acked) ? p.cert : 0u; S->cert_start = p.start;
     }
@@ -1977,7 +1977,7 @@ __device__ __forceinline__ void f_ack_index(const apus_devctx_t *__restrict__ cx
             const uint64_t j = j0 + (uint64_t)q * nthr;
             w[q] = 0;
             // (a self-certified publish names its one entry itself: its index word may still be in flight)
-            if (j < n) w[q] = S->cert ? (uint32_t)S->cert_start : ld_relaxed_sys_u32(&A.index[(uint32_t)(R.acked + 1 + j) & cx->idx_mask]);
+            if (j < n) w[q] = S->cert ? (uint32_t)S->cert_start : apus_ld_relaxed_sys_u32(&A.index[(uint32_t)(R.acked + 1 + j) & cx->idx_mask]);
         }
 #pragma unroll
         for (int q = 0; q < FIDX; q++) {
@@ -1992,9 +1992,9 @@ __device__ __forceinline__ void f_ack_index(const apus_devctx_t *__restrict__ cx
     __syncthreads();
     if (S->head_j) {
         // poll_config_entries (dare_server.c:2163-2170): remember the head this entry carries
-        const uint32_t w = ld_relaxed_sys_u32(&A.index[(uint32_t)(R.acked + S->head_j) & cx->idx_mask]);
+        const uint32_t w = apus_ld_relaxed_sys_u32(&A.index[(uint32_t)(R.acked + S->head_j) & cx->idx_mask]);
         const uint64_t off = (uint64_t)(w & ~APUS_IDX_HEAD_FLAG);
-        R.pend_val = ld_relaxed_sys_u64_any(A.entries, off + E_DATA);
+        R.pend_val = apus_ld_u64_any(A.entries, off + E_DATA);
         R.pend_end = (off + APUS_HDR_BYTES == A.L) ? 0 : off + APUS_HDR_BYTES;
     }
     R.old_end = end_seen;
@@ -2036,7 +2036,7 @@ __device__ __forceinline__ void f_ack_walk(const FollowerAt &A, FollowerShared *
                 const uint8_t *e = win + (off - lo16);
                 const uint32_t ty = e[E_TYPE];
                 const uint32_t ln = (uint32_t)e[E_DATA] | ((uint32_t)e[E_DATA + 1] << 8);
-                const uint32_t es = entry_stride(ty, ln);
+                const uint32_t es = apus_entry_stride(ty, ln);
                 if (A.L - off < es) { next = 0; wrapped = true; break; }              // ghost: entry continues at 0
                 if (off + es > hi) { next = off; break; }                            // entry crosses the window
                 if (ty == T_HEAD) {                                                  // poll_config_entries (dare_server.c:2163-2170)
@@ -2062,7 +2062,7 @@ __device__ __forceinline__ void f_ack_walk(const FollowerAt &A, FollowerShared *
         const uint64_t next = S->next;
         if (n == 0 && next == R.old_end) {
             // no progress possible inside this window: protocol error
-            if (tid == 0) st_relaxed_sys(&A.hw->error, APUS_KERR_BAD_ENTRY);
+            if (tid == 0) apus_st_relaxed_sys(&A.hw->error, APUS_KERR_BAD_ENTRY);
             R.old_end = end_seen;
             break;
         }
@@ -2070,7 +2070,7 @@ __device__ __forceinline__ void f_ack_walk(const FollowerAt &A, FollowerShared *
         walked += n;
         R.old_end = next;
     }
-    if (R.acked + walked != cum_seen && tid == 0) st_relaxed_sys(&A.hw->error, APUS_KERR_COUNT_MISMATCH);
+    if (R.acked + walked != cum_seen && tid == 0) apus_st_relaxed_sys(&A.hw->error, APUS_KERR_COUNT_MISMATCH);
 }
 
 // either mode, the batch is persisted: the ack word (APUS_F_FENCED_ACK: only now, behind a fence over the reply bytes),
@@ -2082,7 +2082,7 @@ __device__ __forceinline__ void f_persist(const FollowerAt &A, FollowerRep &R, u
     if (tid == 0) {
         if (A.flags & APUS_FLAG_FENCED_ACK) {
             __threadfence_system();                      // reply bytes before the ack word
-            st_relaxed_sys(&A.lctrl->ack[A.me], R.acked);   // the word the leader's quorum ranking polls
+            apus_st_relaxed_sys(&A.lctrl->ack[A.me], R.acked);   // the word the leader's quorum ranking polls
         }
         A.hdr->end = end_seen; A.hdr->old_end = R.old_end;
         A.ctrl->acked = R.acked;
@@ -2107,13 +2107,13 @@ __device__ __forceinline__ void f_follow_commit(const FollowerAt &A, FollowerRep
 {
     if (R.old_end == A.L || R.applied == R.old_end || commit_seen == R.applied) return;
     const uint64_t from = R.applied;
-    const uint64_t held = ring_dist(from, R.old_end, A.L);          // bytes I hold beyond `applied`
-    uint64_t want = ring_dist(from, commit_seen, A.L);
+    const uint64_t held = apus_ring_dist(from, R.old_end, A.L);          // bytes I hold beyond `applied`
+    uint64_t want = apus_ring_dist(from, commit_seen, A.L);
     uint64_t to = commit_seen;
     if (want > held) { want = held; to = R.old_end; }             // the leader clamps the same way (dare_ibv_rc.c:1783-1787)
     if (!want) return;
     if (R.pend_end != A.L) {
-        const uint64_t dh = ring_dist(from, R.pend_end, A.L);
+        const uint64_t dh = apus_ring_dist(from, R.pend_end, A.L);
         if (dh > 0 && dh <= want) {
             // the HEAD entry is committed: adopt the head it carries (dare_server.c:2166-2169, 2182-2186)
             if (tid == 0) { A.hdr->head = R.pend_val; A.ctrl->pend_head_end = A.L; }
@@ -2125,11 +2125,11 @@ __device__ __forceinline__ void f_follow_commit(const FollowerAt &A, FollowerRep
         A.hdr->commit = R.applied;              // what this replica knows committed AND holds (I4)
         if (!(A.flags & (APUS_FLAG_HOST_APPLY | APUS_FLAG_DEVICE_APPLY))) {
             A.hdr->apply = R.applied;           // library use: nothing replays the log on the host
-            st_relaxed_sys(&A.lctrl->apply_off[A.me], R.applied);
+            apus_st_relaxed_sys(&A.lctrl->apply_off[A.me], R.applied);
         }
         if (A.flags & APUS_FLAG_DEVICE_APPLY) cons_publish(A.ctrl, R.applied, R.acked);
         // the host may replay [its apply, applied): everything before `applied` is committed and held here
-        st_relaxed_sys_2x64(&A.hw->commit_off, R.applied, R.acked);
+        apus_st_relaxed_sys_2x64(&A.hw->commit_off, R.applied, R.acked);
     }
     R.last_progress = globaltimer_ns();
 }
@@ -2145,7 +2145,7 @@ __device__ void follower_main(const apus_devctx_t *__restrict__ cx)
                           cx->region + cx->entries_off, cx->peer[cx->leader_idx] + cx->entries_off,
                           reinterpret_cast<const uint32_t *>(cx->region + APUS_INDEX_OFF), cx->hw, cx->log_len, cx->flags, cx->idx};
     FollowerRep R = {hdr->old_end, ctrl->acked, hdr->apply, ctrl->pend_head_val, ctrl->pend_head_end, globaltimer_ns()};
-    FollowerPoll W = {0, false, hdr->apply, ld_relaxed_sys(&ctrl->hb), globaltimer_ns(), globaltimer_ns() >> 8, 0, 0};
+    FollowerPoll W = {0, false, hdr->apply, apus_ld_relaxed_sys(&ctrl->hb), globaltimer_ns(), globaltimer_ns() >> 8, 0, 0};
 
     for (;;) {
         if (tid < 32) f_poll(cx, A, S, R, W, tid);
@@ -2178,17 +2178,27 @@ extern "C" size_t apus_kernel_smem_bytes(void)
     return a > b ? a : b;
 }
 
-extern "C" cudaError_t apus_launch_roles(const apus_role_t *d_roles, int n_roles, cudaStream_t stream)
+/* load the replica kernel on the current device and set its shared-memory size, once per device.  Under lazy module
+ * loading the first launch would load it, and a load may wait for the kernels running on the device: a resident
+ * consumer (apus_consumer_attach) never ends by itself, so attach loads it first. */
+extern "C" cudaError_t apus_kernels_load(void)
 {
     static bool attr_set[64] = {false};
     int dev = 0;
     cudaGetDevice(&dev);
-    const size_t smem = apus_kernel_smem_bytes();
     if (dev < 64 && !attr_set[dev]) {
-        cudaError_t e = cudaFuncSetAttribute(apus_replica_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        cudaError_t e = cudaFuncSetAttribute(apus_replica_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                             (int)apus_kernel_smem_bytes());
         if (e != cudaSuccess) return e;
         attr_set[dev] = true;
     }
-    apus_replica_kernel<<<n_roles, APUS_KERNEL_THREADS, smem, stream>>>(d_roles);
+    return cudaSuccess;
+}
+
+extern "C" cudaError_t apus_launch_roles(const apus_role_t *d_roles, int n_roles, cudaStream_t stream)
+{
+    cudaError_t e = apus_kernels_load();
+    if (e != cudaSuccess) return e;
+    apus_replica_kernel<<<n_roles, APUS_KERNEL_THREADS, apus_kernel_smem_bytes(), stream>>>(d_roles);
     return cudaGetLastError();
 }

@@ -37,6 +37,7 @@
 #ifndef APUS_LAYOUT_H
 #define APUS_LAYOUT_H
 
+#include <stddef.h>
 #include <stdint.h>
 
 #define APUS_MAX_SERVERS      13
@@ -258,12 +259,19 @@ typedef struct apus_hostwords {
     uint32_t pad2[31];
     volatile uint64_t host_apply;        /* host -> follower kernel (APUS_FLAG_HOST_APPLY): offset up to which the
                                             application has replayed the log (dare_server.c:1939-1962) */
-    uint64_t pad3[15];
+    volatile uint64_t consumer_stop;     /* host -> resident consumer (apus_consumer_attach): detach and destroy bump it;
+                                            the consumer ends once it differs from the value it was attached under */
+    uint64_t pad3[14];
     volatile uint64_t heartbeat;         /* kernel liveness (debug) */
     volatile uint64_t error;             /* kernel-detected protocol error code */
     volatile uint64_t leader_suspect;    /* follower kernel -> host: 1 + term whose leader stopped sending heartbeats */
     volatile uint64_t hb_seen;           /* follower kernel -> host: last heartbeat word observed */
 } apus_hostwords_t;
+#ifdef __cplusplus
+static_assert(offsetof(apus_hostwords_t, stop) == 256 && offsetof(apus_hostwords_t, host_apply) == 384 &&
+              offsetof(apus_hostwords_t, consumer_stop) == 392 && offsetof(apus_hostwords_t, heartbeat) == 512 &&
+              sizeof(apus_hostwords_t) == 544, "the resident consumers' stop word takes a spare word: no offset moves");
+#endif
 
 #define APUS_FLAG_FENCED_ACK 0x1u
 #define APUS_FLAG_STATS      0x2u

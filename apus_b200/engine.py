@@ -55,6 +55,12 @@ class Stats(C.Structure):
                                    "lat_samples", "auto_heads", "entries_published")] + [("phase_ns", u64 * 8), ("turn_ns", u64 * 8)]
 
 
+class ConsumerView(C.Structure):
+    """apus_consumer_view_t: what a resident consumer kernel (include/apus_consumer.cuh) takes by value"""
+    _fields_ = [("entries", vp), ("log_len", u64), ("index", vp), ("idx_mask", u32), ("pad", u32), ("rec", vp),
+                ("cur", vp), ("error", vp), ("status", vp), ("stop", vp), ("stop_epoch", u64)]
+
+
 ConsumeStatus = namedtuple("ConsumeStatus", "cursor next_idx need_stride error")
 WaitStatus = namedtuple("WaitStatus", "outcome available")
 FenceStatus = namedtuple("FenceStatus", "outcome index")
@@ -110,6 +116,8 @@ SIGNATURES = {
     "apus_consume_seed": (C.c_int, [vp, u64, u64]),
     "apus_read_fence": (C.c_int, [vp, u32, vp, vp, vp]),
     "apus_read_fence_status": (C.c_int, [vp, p64, p64]),
+    "apus_consumer_attach": (C.c_int, [vp, vp, C.POINTER(ConsumerView)]),
+    "apus_consumer_detach": (C.c_int, [vp]),
     "apus_leader_suspect": (u64, [vp]),
     "apus_last_commit_ns": (u64, [vp]),
     "apus_ctl_read": (C.c_int, [vp, vp]),
@@ -478,6 +486,21 @@ class Replica:
         o, i = u64(), u64()
         _ck(lib().apus_read_fence_status(self.h, C.byref(o), C.byref(i)), "apus_read_fence_status")
         return FenceStatus(int(o.value), int(i.value))
+
+    def consumer_attach(self, stream=None):
+        """Attach a resident consumer (apus_consumer_attach), in the roles consume_device accepts: consume work enqueued
+        before has run when this returns.  `stream`: the stream its kernel will be launched on (default: the current
+        stream of this replica's device).  Returns the ConsumerView to pass to that kernel by value.  Until
+        consumer_detach(), consume_device*, consume_wait and consume_mark are refused."""
+        s = self._stream(stream)
+        v = ConsumerView()
+        _ck(lib().apus_consumer_attach(self.h, s.cuda_stream, C.byref(v)), "apus_consumer_attach")
+        return v
+
+    def consumer_detach(self):
+        """Ask the resident consumer to end and wait for the stream it was attached with (apus_consumer_detach); the
+        stream-ordered calls then continue from the cursor it left"""
+        _ck(lib().apus_consumer_detach(self.h), "apus_consumer_detach")
 
     def wait_committed_on_stream(self, ticket, stream=None):
         """make `stream` (default: the current stream of the leader's device) wait until `ticket` is committed"""

@@ -431,6 +431,39 @@ int  apus_read_fence(apus_replica_t *r, uint32_t timeout_us, uint64_t *index, ui
 /* the pinned words the latest fence that ran wrote: its outcome (UINT64_MAX before any fence has run) and its read
  * index (0 unless it ended READY) */
 int  apus_read_fence_status(apus_replica_t *r, uint64_t *outcome, uint64_t *index);
+/* Resident consumers: an application's own persistent kernel applies committed entries in place, from the log, beside
+ * the replica kernels (include/apus_consumer.cuh is its device API).  The view holds the device addresses that API
+ * needs; the application passes it to its kernel by value. */
+typedef struct apus_consumer_view {
+    const uint8_t  *entries;      /* the log ring (device memory) ... */
+    uint64_t        log_len;      /* ... and its length in bytes */
+    const uint32_t *index;        /* the offset index: the offset of entry idx is index[idx & idx_mask] (high bit: HEAD) */
+    uint32_t        idx_mask;
+    uint32_t        pad;
+    const uint64_t *rec;          /* consumer record {committed-and-held offset, entries held}: 16 B, acquired */
+    uint64_t       *cur;          /* cursor {offset, idx of the next entry}: 16 B, stored with a release */
+    uint64_t       *error;        /* sticky APUS_CONSUME_BAD_IDX of the consume state (device memory) */
+    uint64_t       *status;       /* the pinned words apus_consume_status reads: cursor, next idx, need_stride, error */
+    const uint64_t *stop;         /* pinned stop word: the consumer ends once it no longer holds stop_epoch */
+    uint64_t        stop_epoch;
+} apus_consumer_view_t;
+/* Attach a resident consumer to a replica the consume calls accept (APUS_F_DEVICE_APPLY on a follower; any role with
+ * APUS_F_APPLY_ANY_ROLE).  It synchronises the consume stream, so that consume work enqueued before it has run and the
+ * cursor stands where that work left it, then fills *out.  `stream` (a cudaStream_t on the replica's GPU, NULL = the
+ * legacy default stream) is the stream the application launches its consumer kernel on.  While attached:
+ *   - the resident consumer alone moves the cursor: apus_consume_device*, apus_consume_wait and apus_consume_mark
+ *     return APUS_ERROR with nothing enqueued (apus_read_fence stays accepted; it never moves the cursor);
+ *   - apus_replicas_stop, apus_replica_set_role and the release points of consume waits do not stop it: it keeps
+ *     polling its record through a take-over;
+ *   - a snapshot takes the position from apus_consumer_position in the application's own kernel, at a point where its
+ *     state is consistent; apus_consume_seed accepts it as it accepts a mark.
+ * APUS_ERROR where the consume calls refuse the replica, for a null `out`, and when a consumer is attached already. */
+int  apus_consumer_attach(apus_replica_t *r, void *stream, apus_consumer_view_t *out);
+/* Ask the resident consumer to end (its stop word moves) and synchronise the stream it was attached with.  Consume
+ * calls, waits and marks are accepted again and continue from the cursor it left.  APUS_ERROR when none is attached.
+ * apus_replica_destroy does the same for an attached replica before it frees anything: a consumer kernel that ignored
+ * the stop word would keep both calls waiting. */
+int  apus_consumer_detach(apus_replica_t *r);
 /* failure detector: 0 while the leader's heartbeats arrive, else 1 + the term whose leader fell silent */
 uint64_t apus_leader_suspect(apus_replica_t *follower);
 /* %globaltimer (ns) of the leader kernel's latest commit (device clock; step timing of resident kernels) */
