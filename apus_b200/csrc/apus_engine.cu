@@ -198,6 +198,10 @@ struct apus_replica {
     uint64_t cons_enqueued;       /* consume, wait and mark enqueues so far (under cons_mu): a seed needs none */
     int      attached;            /* a resident consumer moves the cursor (apus_consumer_attach; under cons_mu) ... */
     cudaStream_t attach_stream;   /* ... launched on this stream */
+    /* resident submitter (apus_submitter_attach): it alone writes the ring while attached */
+    int      sub_attached;
+    cudaStream_t sub_stream;      /* the stream it was launched on */
+    apus_submitter_state_t *sub_st;   /* device: its state, followed by pay_end[ring_slots] */
     apus_replica *live_next;      /* the process's live replicas (g_live, under g_live_mu) */
 };
 
@@ -248,6 +252,23 @@ static void consumer_stop(apus_replica *r)
     r->attached = 0;
 }
 
+/* end the attached resident submitter: move its stop word and wait for the stream it was launched on */
+static void submitter_stop(apus_replica *r)
+{
+    __atomic_fetch_add(&r->hw->submitter_stop, 1ull, __ATOMIC_SEQ_CST);
+    cudaStreamSynchronize(r->sub_stream);
+    r->sub_attached = 0;
+}
+
+/* the calls that write the submission ring: a resident submitter, while attached, alone writes it */
+static int ring_writer_gate(const apus_replica *r, const char *what)
+{
+    if (!r) return fail("null argument");
+    if (r->sub_attached)
+        return fail("%s: a resident submitter is attached (apus_submitter_detach first): it alone writes the ring", what);
+    return APUS_OK;
+}
+
 static int ensure_host_ring(apus_replica *r)
 {
     /* device ring: the pinned staging copy of the ring is only needed when the HOST submits (lazily allocated:
@@ -278,6 +299,8 @@ static int leader_ring_init(apus_replica *r)
         CK(cudaMemset(r->sub_tail_dev, 0, 128));
         CK(cudaHostAlloc(&r->sub_tail_stage, 64, cudaHostAllocPortable));
         CK(cudaMalloc(&r->pack_blk, APUS_PACK_BLK_WORDS * sizeof(uint64_t) * apus_pack_blocks(r->ring_slots)));
+        /* a resident submitter's state, allocated with the ring: apus_submitter_attach allocates nothing */
+        CK(cudaMalloc(&r->sub_st, sizeof(apus_submitter_state_t) + 8ull * r->ring_slots));
         CK(apus_batch_load());
     }
     return APUS_OK;
@@ -436,6 +459,7 @@ extern "C" void apus_replica_destroy(apus_replica_t *r)
         StageLock cl(&r->cons_mu);
         if (r->attached) consumer_stop(r);
     }
+    if (r->sub_attached) submitter_stop(r);             /* it writes the ring and reads the pinned words */
     if (r->in_flight && r->hw) {
         r->hw->stop = 1;
         cudaEventSynchronize(r->launch_owner ? r->launch_owner->ev_stop : r->ev_stop);
@@ -473,6 +497,7 @@ extern "C" void apus_replica_destroy(apus_replica_t *r)
     for (cudaEvent_t e : {r->ev_copy[0], r->ev_copy[1], r->ev_cons[0], r->ev_cons[1], r->ev_fence})
         if (e) cudaEventDestroy(e);
     if (r->cons_st) cudaFree(r->cons_st);
+    if (r->sub_st) cudaFree(r->sub_st);
     if (r->cons_stream) cudaStreamDestroy(r->cons_stream);
     if (r->stream) cudaStreamDestroy(r->stream);
     if (r->copy_stream) cudaStreamDestroy(r->copy_stream);
@@ -657,7 +682,7 @@ extern "C" int apus_replicas_stop(apus_replica_t **rs, int n)
 extern "C" uint8_t apus_synth_byte(uint32_t seed, uint64_t req_id, uint32_t k) { return synth_byte(seed, req_id, k); }
 
 /* Where the data image of a request goes: inline in its slot (<= APUS_SLOT_INLINE bytes) or into the payload byte
- * ring (slot_place: apus_slot.h).  pay_end[ticket & mask] = the pay_head counter after that ticket's image.  Returns
+ * ring (slot_place: include/apus_slot_format.h).  pay_end[ticket & mask] = the pay_head counter after that ticket's image.  Returns
  * the type_off word; *ppos = ring position of an external image.  APUS_RETRY when the payload ring has no room. */
 static inline int place_image(apus_replica *r, uint8_t type, uint32_t nb, uint64_t consumed, uint64_t *head_io,
                               uint32_t *type_off_out, uint64_t *ppos)
@@ -771,7 +796,7 @@ static int ring_flush(apus_replica *r)
 extern "C" int apus_submit(apus_replica_t *r, uint8_t type, uint16_t connection_id, uint64_t req_id,
                            const void *cmd, uint16_t len, uint64_t *ticket)
 {
-    if (!r) return fail("null argument");
+    if (ring_writer_gate(r, "apus_submit") != APUS_OK) return APUS_ERROR;
     if (!is_leader(r)) return fail("submit on a follower (proxy.c:235 only submits when is_leader())");
     if (len && !cmd) return fail("null payload");
     int rc = ring_put(r, type, connection_id, req_id, cmd, len);
@@ -786,6 +811,7 @@ extern "C" int apus_submit_batch(apus_replica_t *r, uint32_t n, const uint8_t *t
                                  size_t stride, uint64_t *first_ticket)
 {
     if (!r || !types || !conns || !req_ids || !lens) return fail("null argument");
+    if (ring_writer_gate(r, "apus_submit_batch") != APUS_OK) return APUS_ERROR;
     if (!is_leader(r)) return fail("submit on a follower");
     uint64_t t0 = r->submitted + 1;
     /* all or nothing: remember the ring state */
@@ -928,7 +954,7 @@ extern "C" int apus_submit_uniform(apus_replica_t *r, uint32_t n, uint8_t type, 
                                    uint64_t first_req_id, uint16_t len, const void *payloads, size_t stride,
                                    uint64_t *first_ticket)
 {
-    if (!r) return fail("null argument");
+    if (ring_writer_gate(r, "apus_submit_uniform") != APUS_OK) return APUS_ERROR;
     if (!is_leader(r)) return fail("submit on a follower");
     if (len && !payloads) return fail("null payload");
     if (n == 0) return APUS_OK;
@@ -975,7 +1001,7 @@ extern "C" int apus_submit_uniform(apus_replica_t *r, uint32_t n, uint8_t type, 
 extern "C" int apus_submit_synth(apus_replica_t *r, uint32_t n, uint8_t type, uint16_t connection_id,
                                  uint64_t first_req_id, uint16_t len, uint32_t seed, uint64_t *first_ticket)
 {
-    if (!r) return fail("null argument");
+    if (ring_writer_gate(r, "apus_submit_synth") != APUS_OK) return APUS_ERROR;
     if (!is_leader(r)) return fail("submit on a follower");
     if (r->cfg.ring_mode != APUS_RING_DEVICE) return fail("apus_submit_synth needs the device submission ring");
     if (type == APUS_NOOP || type == APUS_CONFIG || type == APUS_HEAD) return fail("apus_submit_synth: request types only");
@@ -1071,7 +1097,7 @@ extern "C" int apus_submit_device(apus_replica_t *r, uint32_t n, const uint8_t *
                                   const uint64_t *req_ids, const uint16_t *lens, const void *payloads, size_t stride,
                                   void *stream, uint64_t *first_ticket)
 {
-    if (!r) return fail("null argument");
+    if (ring_writer_gate(r, "apus_submit_device") != APUS_OK) return APUS_ERROR;
     if (!is_leader(r)) return fail("submit on a follower");
     if (r->cfg.ring_mode != APUS_RING_DEVICE) return fail("apus_submit_device needs the device submission ring");
     if (n == 0) return APUS_OK;
@@ -1089,7 +1115,7 @@ extern "C" int apus_submit_device_packed(apus_replica_t *r, uint32_t n, const ui
                                          const uint16_t *connection_ids, const uint64_t *req_ids, const uint64_t *offsets,
                                          const void *values, uint64_t values_bytes, void *stream, uint64_t *first_ticket)
 {
-    if (!r) return fail("null argument");
+    if (ring_writer_gate(r, "apus_submit_device_packed") != APUS_OK) return APUS_ERROR;
     if (!is_leader(r)) return fail("submit on a follower");
     if (r->cfg.ring_mode != APUS_RING_DEVICE) return fail("apus_submit_device_packed needs the device submission ring");
     if (n == 0) return APUS_OK;
@@ -1107,8 +1133,17 @@ extern "C" int apus_submit_device_packed(apus_replica_t *r, uint32_t n, const ui
 extern "C" int apus_device_submit_status(apus_replica_t *r, uint64_t *rejected, uint64_t *first_rejected_ticket)
 {
     if (!r) return fail("null argument");
-    if (rejected) *rejected = r->hw->dev_rejected;
-    if (first_rejected_ticket) *first_rejected_ticket = r->hw->dev_first_rejected;
+    uint64_t n = r->hw->dev_rejected, first = r->hw->dev_first_rejected;
+    if (r->sub_attached) {                               /* ... and what the resident submitter has counted so far */
+        DeviceGuard g(r->cfg.device);
+        apus_submitter_state_t s;
+        CK(cudaMemcpyAsync(&s, r->sub_st, sizeof s, cudaMemcpyDeviceToHost, r->copy_stream));
+        CK(cudaStreamSynchronize(r->copy_stream));
+        n += s.rejected;
+        if (!first && s.rejected) first = s.first_rejected;
+    }
+    if (rejected) *rejected = n;
+    if (first_rejected_ticket) *first_rejected_ticket = first;
     return APUS_OK;
 }
 
@@ -1160,18 +1195,18 @@ extern "C" const volatile uint64_t *apus_committed_word(apus_replica_t *r)
 
 extern "C" int apus_submit_defer(apus_replica_t *r, int defer)
 {
-    if (!r) return fail("null argument");
+    if (ring_writer_gate(r, "apus_submit_defer") != APUS_OK) return APUS_ERROR;
     r->defer = defer;
     return APUS_OK;
 }
 extern "C" int apus_submit_flush(apus_replica_t *r)
 {
-    if (!r) return fail("null argument");
+    if (ring_writer_gate(r, "apus_submit_flush") != APUS_OK) return APUS_ERROR;
     return ring_flush(r);
 }
 extern "C" int apus_submit_release(apus_replica_t *r, uint64_t ticket)
 {
-    if (!r) return fail("null argument");
+    if (ring_writer_gate(r, "apus_submit_release") != APUS_OK) return APUS_ERROR;
     if (ticket > r->submitted) return fail("release beyond what was submitted");
     int rc = ring_push(r);
     if (rc != APUS_OK) return rc;
@@ -1219,6 +1254,7 @@ extern "C" int apus_closed_loop(apus_replica_t *r, uint32_t n, uint16_t payload_
                                 uint64_t first_req_id, uint32_t *lat_ns)
 {
     if (!r || !lat_ns) return fail("null argument");
+    if (ring_writer_gate(r, "apus_closed_loop") != APUS_OK) return APUS_ERROR;
     if (!is_leader(r)) return fail("submit on a follower");
     uint8_t *buf = (uint8_t *)malloc(payload_len ? payload_len : 1);
     if (!buf) return fail("out of memory");
@@ -1513,6 +1549,71 @@ extern "C" int apus_consumer_detach(apus_replica_t *r)
     return APUS_OK;
 }
 
+/* ---- resident submitters: an application's kernel writes the leader's HBM ring itself -------------------------- */
+extern "C" int apus_submitter_attach(apus_replica_t *r, void *stream, apus_submitter_view_t *out)
+{
+    if (!r || !out) return fail("null argument");
+    if (!is_leader(r)) return fail("apus_submitter_attach: a resident submitter writes the leader's ring (this is a follower)");
+    if (r->cfg.ring_mode != APUS_RING_DEVICE) return fail("apus_submitter_attach needs the device submission ring");
+    if (r->sub_attached) return fail("apus_submitter_attach: a resident submitter is attached already (one per leader)");
+    DeviceGuard g(r->cfg.device);
+    /* detach synchronises this stream: it must be the queue the submitter runs on, on the leader's GPU */
+    int sdev = -1;
+    CK(cudaStreamGetDevice((cudaStream_t)stream, &sdev));
+    if (sdev != r->cfg.device)
+        return fail("apus_submitter_attach: the stream is on device %d, the leader on device %d", sdev, r->cfg.device);
+    /* everything the host has submitted reaches the ring and the doorbell first: the submitter's turns start there */
+    if (ring_flush(r) != APUS_OK) return APUS_ERROR;
+    CK(cudaStreamSynchronize(r->copy_stream));
+    CK(apus_kernels_load());                             /* no lazy load of ours may wait for the submitter from here on */
+    apus_submitter_state_t s;
+    memset(&s, 0, sizeof s);
+    s.submitted = r->submitted; s.pay_head = r->pay_head; s.wrap_next = r->wrap_next ? 1 : 0;
+    s.consumed = r->hw->consumed; s.first_rejected = ~0ull;
+    CK(cudaMemcpyAsync(r->sub_st, &s, sizeof s, cudaMemcpyHostToDevice, r->copy_stream));
+    CK(cudaMemcpyAsync(r->sub_st + 1, r->pay_end, 8ull * r->ring_slots, cudaMemcpyHostToDevice, r->copy_stream));
+    CK(cudaStreamSynchronize(r->copy_stream));
+    apus_submitter_view_t v;
+    memset(&v, 0, sizeof v);
+    v.slots = reinterpret_cast<uint8_t *>(r->ring_desc_dev);
+    v.pay = r->ring_pay_dev;
+    v.doorbell = r->sub_tail_dev;
+    v.ring_slots = r->ring_slots; v.ring_bytes = r->ring_bytes;
+    v.state = r->sub_st;
+    v.pay_end = reinterpret_cast<uint64_t *>(r->sub_st + 1);
+    v.consumed = const_cast<const uint64_t *>(&r->hw_dev->consumed);
+    v.committed = const_cast<const uint64_t *>(&r->hw_dev->committed_tickets);
+    v.stop = const_cast<const uint64_t *>(&r->hw_dev->submitter_stop);
+    v.stop_epoch = r->hw->submitter_stop;
+    r->sub_attached = 1;
+    r->sub_stream = (cudaStream_t)stream;
+    *out = v;
+    return APUS_OK;
+}
+
+extern "C" int apus_submitter_detach(apus_replica_t *r)
+{
+    if (!r) return fail("null argument");
+    if (!r->sub_attached) return fail("apus_submitter_detach: no resident submitter is attached");
+    DeviceGuard g(r->cfg.device);
+    submitter_stop(r);
+    /* hand the ring back: the doorbell P is what the leader may read; reservations past it are dropped */
+    apus_submitter_state_t s;
+    uint64_t P = 0;
+    CK(cudaMemcpyAsync(&P, r->sub_tail_dev, 8, cudaMemcpyDeviceToHost, r->copy_stream));
+    CK(cudaMemcpyAsync(&s, r->sub_st, sizeof s, cudaMemcpyDeviceToHost, r->copy_stream));
+    CK(cudaMemcpyAsync(r->pay_end, r->sub_st + 1, 8ull * r->ring_slots, cudaMemcpyDeviceToHost, r->copy_stream));
+    CK(cudaStreamSynchronize(r->copy_stream));
+    r->submitted = r->flushed = r->belled = P;
+    r->pay_head = r->pay_flushed = P ? r->pay_end[(P - 1) & (r->ring_slots - 1)] : 0;
+    r->wrap_next = 1;                                    /* a dropped reservation may have moved the payload counter */
+    if (s.rejected) {
+        if (!r->hw->dev_first_rejected) r->hw->dev_first_rejected = s.first_rejected;
+        r->hw->dev_rejected += s.rejected;
+    }
+    return APUS_OK;
+}
+
 extern "C" uint64_t apus_leader_suspect(apus_replica_t *r) { return r ? r->hw->leader_suspect : 0; }
 extern "C" uint64_t apus_last_commit_ns(apus_replica_t *r) { return r ? r->hw->last_commit_ns : 0; }
 
@@ -1525,6 +1626,10 @@ extern "C" int apus_get_stats(apus_replica_t *r, apus_stats_t *out)
     CK(cudaStreamSynchronize(r->copy_stream));
     memset(out, 0, sizeof *out);
     out->tickets_submitted = r->submitted;
+    if (r->sub_attached) {                               /* the resident submitter's published tickets: the doorbell */
+        CK(cudaMemcpyAsync(&out->tickets_submitted, r->sub_tail_dev, 8, cudaMemcpyDeviceToHost, r->copy_stream));
+        CK(cudaStreamSynchronize(r->copy_stream));
+    }
     out->tickets_consumed = c.consumed;
     out->tickets_committed = c.committed_tickets;
     out->entries_acked = c.acked;
@@ -2006,6 +2111,9 @@ extern "C" int apus_replica_disconnect(apus_replica_t *r, uint8_t peer_idx)
 extern "C" int apus_replica_set_role(apus_replica_t *r, uint8_t leader_idx, uint64_t term)
 {
     if (!r || leader_idx >= r->cfg.group_size) return fail("bad argument");
+    if (r->sub_attached)
+        return fail("apus_replica_set_role: a resident submitter is attached (apus_submitter_detach first): it does not "
+                    "follow a take-over");
     if ((r->cfg.flags & APUS_F_DEVICE_APPLY) && !(r->cfg.flags & APUS_F_APPLY_ANY_ROLE))
         return fail("a replica with device consumers (APUS_F_DEVICE_APPLY) keeps its role");
     if (r->in_flight) return fail("stop the kernel first");

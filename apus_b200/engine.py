@@ -61,6 +61,12 @@ class ConsumerView(C.Structure):
                 ("cur", vp), ("error", vp), ("status", vp), ("stop", vp), ("stop_epoch", u64)]
 
 
+class SubmitterView(C.Structure):
+    """apus_submitter_view_t: what a resident submitter kernel (include/apus_submitter.cuh) takes by value"""
+    _fields_ = [("slots", vp), ("pay", vp), ("doorbell", vp), ("ring_slots", u32), ("ring_bytes", u32), ("state", vp),
+                ("pay_end", vp), ("consumed", vp), ("committed", vp), ("stop", vp), ("stop_epoch", u64)]
+
+
 ConsumeStatus = namedtuple("ConsumeStatus", "cursor next_idx need_stride error")
 WaitStatus = namedtuple("WaitStatus", "outcome available")
 FenceStatus = namedtuple("FenceStatus", "outcome index")
@@ -118,6 +124,8 @@ SIGNATURES = {
     "apus_read_fence_status": (C.c_int, [vp, p64, p64]),
     "apus_consumer_attach": (C.c_int, [vp, vp, C.POINTER(ConsumerView)]),
     "apus_consumer_detach": (C.c_int, [vp]),
+    "apus_submitter_attach": (C.c_int, [vp, vp, C.POINTER(SubmitterView)]),
+    "apus_submitter_detach": (C.c_int, [vp]),
     "apus_leader_suspect": (u64, [vp]),
     "apus_last_commit_ns": (u64, [vp]),
     "apus_ctl_read": (C.c_int, [vp, vp]),
@@ -501,6 +509,21 @@ class Replica:
         """Ask the resident consumer to end and wait for the stream it was attached with (apus_consumer_detach); the
         stream-ordered calls then continue from the cursor it left"""
         _ck(lib().apus_consumer_detach(self.h), "apus_consumer_detach")
+
+    def submitter_attach(self, stream=None):
+        """Attach a resident submitter to this leader (apus_submitter_attach; APUS_RING_DEVICE only): everything the
+        host submitted has reached the ring when this returns.  `stream`: the stream its kernel will be launched on
+        (default: the current stream of this replica's device).  Returns the SubmitterView to pass to that kernel by
+        value.  Until submitter_detach(), every call that writes the ring, and set_role, is refused."""
+        s = self._stream(stream)
+        v = SubmitterView()
+        _ck(lib().apus_submitter_attach(self.h, s.cuda_stream, C.byref(v)), "apus_submitter_attach")
+        return v
+
+    def submitter_detach(self):
+        """Ask the resident submitter to end, wait for its stream and hand the ring back to the host
+        (apus_submitter_detach): the next host ticket follows the last one it published"""
+        _ck(lib().apus_submitter_detach(self.h), "apus_submitter_detach")
 
     def wait_committed_on_stream(self, ticket, stream=None):
         """make `stream` (default: the current stream of the leader's device) wait until `ticket` is committed"""

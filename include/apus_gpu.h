@@ -464,6 +464,55 @@ int  apus_consumer_attach(apus_replica_t *r, void *stream, apus_consumer_view_t 
  * apus_replica_destroy does the same for an attached replica before it frees anything: a consumer kernel that ignored
  * the stop word would keep both calls waiting. */
 int  apus_consumer_detach(apus_replica_t *r);
+/* Resident submitters: an application's own persistent kernel, on the leader's GPU, reserves tickets, writes slots and
+ * payload images straight into the leader's HBM submission ring and rings the doorbell, without a host call
+ * (include/apus_submitter.cuh is its device API; the slot format is include/apus_slot_format.h).  The submitter's state
+ * lives in device memory: reservations take tickets and payload space in one order under its lock. */
+typedef struct apus_submitter_state {
+    uint64_t lock;                /* 0 = free; taken with a CAS by the reserving thread */
+    uint64_t submitted;           /* tickets handed out (reserved) so far */
+    uint64_t pay_head;            /* payload bytes handed out so far (monotone; position = % ring_bytes) */
+    uint64_t wrap_next;           /* 1: the next external image carries APUS_SLOT_WRAP */
+    uint64_t consumed;            /* the leader's consumed tickets as last read over PCIe (a lower bound) */
+    uint64_t rejected;            /* requests written as NOOPs ... */
+    uint64_t first_rejected;      /* ... and the lowest ticket among them (UINT64_MAX = none) */
+    uint64_t pad;
+} apus_submitter_state_t;
+typedef struct apus_submitter_view {
+    uint8_t        *slots;        /* the leader's HBM slot ring: ring_slots slots of 128 B (apus_slot_t) */
+    uint8_t        *pay;          /* ... and its payload ring of ring_bytes bytes */
+    uint64_t       *doorbell;     /* the device doorbell the leader kernel reads: tickets readable so far */
+    uint32_t        ring_slots;   /* power of two */
+    uint32_t        ring_bytes;
+    apus_submitter_state_t *state;
+    uint64_t       *pay_end;      /* [ticket % ring_slots]: the payload counter after that ticket (device memory) */
+    const uint64_t *consumed;     /* pinned: tickets the leader kernel has taken from the ring */
+    const uint64_t *committed;    /* pinned: tickets committed (the word apus_committed_word gives) */
+    const uint64_t *stop;         /* pinned stop word: the submitter ends once it no longer holds stop_epoch */
+    uint64_t        stop_epoch;
+} apus_submitter_view_t;
+/* Attach a resident submitter to a leader created with APUS_RING_DEVICE.  It pushes and rings everything the host has
+ * submitted, waits for that to reach the ring, copies the ring accounting (tickets handed out, the payload counter,
+ * pay_end of the unconsumed tickets) into the submitter's device state and fills *out.  `stream` (a cudaStream_t on
+ * the leader's GPU, NULL = the legacy default stream) is the stream the application launches its submitter on.  While
+ * attached:
+ *   - the submitter alone writes the ring: apus_submit, apus_submit_batch, _uniform, _synth, _device, _device_packed,
+ *     apus_submit_defer, _flush, _release and apus_closed_loop return APUS_ERROR with nothing written;
+ *   - apus_replica_set_role on this replica returns APUS_ERROR (a submitter does not follow a take-over: detach first);
+ *   - apus_replicas_stop leaves it attached: its reservations and commit waits then end at their timeouts;
+ *   - reads stay accepted: apus_committed_tickets, apus_wait_committed, apus_stream_wait_committed, apus_get_stats
+ *     (tickets_submitted counts the published device tickets) and apus_device_submit_status (which counts the requests
+ *     the submitter wrote as NOOPs).
+ * APUS_ERROR for a null replica or `out`, on a follower, on a host-mapped ring, for a stream of another device, and when
+ * a submitter is attached already. */
+int  apus_submitter_attach(apus_replica_t *leader, void *stream, apus_submitter_view_t *out);
+/* Ask the resident submitter to end (its stop word moves), synchronise the stream it was attached with, and hand the
+ * ring back to the host: what was published -- the doorbell P -- becomes the host's count of submitted tickets, the
+ * payload counter becomes the one after ticket P, and the next host image carries APUS_SLOT_WRAP.  Reservations past P
+ * were never visible to the leader: they are dropped, and the host hands their ticket numbers out again (P + 1 is the
+ * next ticket).  A dropped reservation's requests that were written as NOOPs stay counted.  apus_replica_destroy does
+ * the same stop before it frees anything.  APUS_ERROR when none is attached. */
+int  apus_submitter_detach(apus_replica_t *leader);
 /* failure detector: 0 while the leader's heartbeats arrive, else 1 + the term whose leader fell silent */
 uint64_t apus_leader_suspect(apus_replica_t *follower);
 /* %globaltimer (ns) of the leader kernel's latest commit (device clock; step timing of resident kernels) */
