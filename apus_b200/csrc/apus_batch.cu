@@ -7,7 +7,7 @@
  *   consume  apus_consume_device / apus_consume_device_packed: head, count, scan, copy and tail
  *   wait     apus_consume_wait: one warp between consume calls, until enough entries are committed past the cursor
  *   mark     apus_consume_mark: one thread writes the consumer position, for a snapshot of the application's state
- *   fence    apus_read_fence: one warp until this replica's state can answer a linearizable read (apus_fence.h)
+ *   fence    apus_read_fence: one warp until this replica's state can answer a linearizable read (apus_reader.cuh)
  *
  * apus_engine.cu checks the arguments, accounts ring space, and brackets each enqueue below in the caller's stream
  * order.  The batch layouts are apus_layout.h; the slot format is apus_slot.h; the device helpers shared with the
@@ -21,6 +21,7 @@
 #include "apus_slot.h"
 #include "apus_dev.h"
 #include "apus_fence.h"
+#include "apus_reader.cuh"
 
 // ---------------------------------------------------------------------------------
 // block scans: the packing and the consume kernels run blocks of the same size
@@ -537,14 +538,15 @@ __global__ void apus_consume_mark_kernel(const apus_ctrl_t *ctrl, const apus_con
 }
 
 // ---------------------------------------------------------------------------------
-// READ FENCES (apus_read_fence): one warp on the consume stream; lane 0 takes the three steps of apus_fence.h.
+// READ FENCES (apus_read_fence): one warp on the consume stream; lane 0 takes the three steps of apus_reader.cuh, the
+// definitions a resident reader takes too.
 //   1. K: the entries-committed word of the leader's consumer record (apus_cons_read's acquire), which its commit warp
 //      publishes only under APUS_F_APPLY_ANY_ROLE (cons_on == 2); otherwise, or with the leader not mapped, NOT_LEADER.
 //   2. after K (the acquire orders the loads below after it): the SID word of every member this replica maps; fewer
 //      than N/2 + 1 at term <= t ends NOT_LEADER (rf_confirmed).
 //   3. this replica's own record, polled as a consume wait polls (wait_backoff) until rf_ready: held >= K, and the
 //      entry the offset index names for idx `held` carries idx `held` (else it is another lap's: poll again) and a term
-//      >= t.  The header is read idx, term, idx, so that a term torn from an entry of a later lap is not taken.
+//      >= t.
 // F = held.  N + 2 loads of other replicas' words (the leader's cons_on and record, the SIDs), one local poll.  It
 // writes the caller's index (READY only) and outcome words and two pinned status words, nothing the replica kernels read.
 // ---------------------------------------------------------------------------------
@@ -554,39 +556,27 @@ __global__ void apus_read_fence_kernel(apus_fence_args_t a)
     const uint64_t t0 = apus_globaltimer_ns();
     uint64_t F = 0;
     uint32_t why = APUS_WAIT_NOT_LEADER;
-    const apus_ctrl_t *lead = NULL;
+    const uint8_t *lead = NULL;
 #pragma unroll
     for (uint32_t i = 0; i < APUS_MAX_SERVERS; i++)
-        if (i == a.leader) lead = reinterpret_cast<const apus_ctrl_t *>(a.member[i]);
-    if (lead && apus_ld_relaxed_sys(&lead->cons_on) == 2) {
-        uint64_t k_off, K;
-        apus_cons_read(lead->cons_rec, k_off, K);
-        uint32_t counted = 0;
-#pragma unroll
-        for (uint32_t i = 0; i < APUS_MAX_SERVERS; i++)
-            if (i < a.n && a.member[i])
-                counted += rf_member_counts(1, apus_ld_relaxed_sys(a.member[i] + APUS_CTL_OFF + offsetof(apus_ctlwords_t, sid)),
-                                            a.term);
-        if (rf_confirmed(counted, a.n)) {
-            const apus_ctrl_t *own = reinterpret_cast<const apus_ctrl_t *>(a.region);
-            const uint32_t *index = reinterpret_cast<const uint32_t *>(a.region + APUS_INDEX_OFF);
-            const uint8_t *entries = a.region + a.entries_off;
-            uint64_t t_rel = t0;
-            uint32_t sleep = APUS_WAIT_SLEEP_MIN_NS;
-            for (;;) {
-                uint64_t held_off, held, e_idx = 0, e_term = 0;
-                apus_cons_read(own->cons_rec, held_off, held);
-                if (held && held >= K) {
-                    const uint64_t off = apus_ld_relaxed_sys_u32(&index[(uint32_t)held & a.idx_mask]) & ~APUS_IDX_HEAD_FLAG;
-                    if (off + APUS_HDR_BYTES <= a.log_len) {
-                        e_idx = apus_ld_u64_any(entries, off + E_IDX);
-                        e_term = apus_ld_u64_any(entries, off + E_TERM);
-                        if (apus_ld_u64_any(entries, off + E_IDX) != e_idx) e_idx = 0;
-                    }
-                }
-                if (rf_ready(held, K, e_idx, e_term, a.term)) { F = held; why = APUS_WAIT_READY; break; }
-                if (wait_backoff(a.hw, a.epoch, t0, a.timeout_ns, t_rel, sleep, why)) break;
+        if (i == a.leader) lead = a.member[i];
+    uint64_t K;
+    uint32_t mask;
+    if (apus_fence_take_k(lead, APUS_REGION_CONS_ON, APUS_REGION_CONS_REC, K) &&
+        apus_fence_confirm(a.member, a.n, APUS_REGION_SID, a.term, mask)) {
+        const apus_ctrl_t *own = reinterpret_cast<const apus_ctrl_t *>(a.region);
+        const uint32_t *index = reinterpret_cast<const uint32_t *>(a.region + APUS_INDEX_OFF);
+        const uint8_t *entries = a.region + a.entries_off;
+        uint64_t t_rel = t0;
+        uint32_t sleep = APUS_WAIT_SLEEP_MIN_NS;
+        for (;;) {
+            uint64_t held;
+            if (apus_fence_ready(entries, index, a.idx_mask, a.log_len, own->cons_rec, K, a.term, held)) {
+                F = held;
+                why = APUS_WAIT_READY;
+                break;
             }
+            if (wait_backoff(a.hw, a.epoch, t0, a.timeout_ns, t_rel, sleep, why)) break;
         }
     }
     if (why == APUS_WAIT_READY) *(volatile uint64_t *)a.index = F;

@@ -202,6 +202,12 @@ struct apus_replica {
     int      sub_attached;
     cudaStream_t sub_stream;      /* the stream it was launched on */
     apus_submitter_state_t *sub_st;   /* device: its state, followed by pay_end[ring_slots] */
+    /* resident reader (apus_reader_attach): the pinned block it reads its role and the peers' regions from.  The
+     * member words change under g_live_mu */
+    apus_reader_block_t *rb;      /* pinned + mapped, allocated at create */
+    apus_reader_block_t *rb_dev;
+    int      reader_attached;
+    cudaStream_t reader_stream;   /* the stream it was launched on */
     apus_replica *live_next;      /* the process's live replicas (g_live, under g_live_mu) */
 };
 
@@ -258,6 +264,33 @@ static void submitter_stop(apus_replica *r)
     __atomic_fetch_add(&r->hw->submitter_stop, 1ull, __ATOMIC_SEQ_CST);
     cudaStreamSynchronize(r->sub_stream);
     r->sub_attached = 0;
+}
+
+/* end the attached resident reader: move its stop word and wait for the stream it was launched on */
+static void reader_stop(apus_replica *r)
+{
+    __atomic_fetch_add(&r->hw->reader_stop, 1ull, __ATOMIC_SEQ_CST);
+    cudaStreamSynchronize(r->reader_stream);
+    r->reader_attached = 0;
+}
+
+/* the role word of the reader block: the SID this replica knows, [TERM|L|IDX] (dare_server.h:46-61) */
+static inline uint64_t role_sid(const apus_replica *r) { return (r->cfg.term << 9) | (1ull << 8) | r->cfg.leader_idx; }
+
+/* Clear member word i of r's reader block (under g_live_mu), then wait until no fence that may have read the old word
+ * still reads that region: the host's half of the handshake of include/apus_reader.cuh.  A busy word is odd only across
+ * one fence's N + 2 remote loads.  Without an attached reader no fence runs (detach synchronised its stream). */
+static void reader_forget(apus_replica *r, int i)
+{
+    if (!r->rb || !r->rb->member[i]) return;
+    r->rb->member[i] = 0;
+    __sync_synchronize();
+    if (!r->reader_attached) return;
+    for (int s = 0; s < APUS_READER_SLOTS; s++) {
+        const uint64_t b = r->rb->busy[s];
+        if (b & 1)
+            while (r->rb->busy[s] == b) _mm_pause();
+    }
 }
 
 /* the calls that write the submission ring: a resident submitter, while attached, alone writes it */
@@ -369,6 +402,11 @@ static int replica_init(apus_replica *r, const apus_config_t *cfg, uint64_t log_
         CK(cudaMemcpy(r->region + APUS_CTL_OFF, &w, sizeof w, cudaMemcpyHostToDevice));
     }
     r->peer_ptr[cfg->server_idx] = r->region;
+    CK(cudaHostAlloc(&r->rb, sizeof(apus_reader_block_t), cudaHostAllocMapped | cudaHostAllocPortable));
+    memset((void *)r->rb, 0, sizeof(apus_reader_block_t));
+    r->rb->role = role_sid(r);
+    r->rb->member[cfg->server_idx] = (uint64_t)(uintptr_t)r->region;
+    CK(cudaHostGetDevicePointer(&r->rb_dev, r->rb, 0));
     return APUS_OK;
 }
 
@@ -442,6 +480,7 @@ extern "C" void apus_replica_destroy(apus_replica_t *r)
             for (int i = 0; i < APUS_MAX_SERVER_COUNT; i++)
                 if (i != q->cfg.server_idx && !q->peer_is_ipc[i] && q->peer_ptr[i] == (void *)r->region) {
                     q->peer_ptr[i] = NULL;
+                    reader_forget(q, i);
                     maps = true;
                 }
             if (!maps || !q->fences) continue;
@@ -460,6 +499,7 @@ extern "C" void apus_replica_destroy(apus_replica_t *r)
         if (r->attached) consumer_stop(r);
     }
     if (r->sub_attached) submitter_stop(r);             /* it writes the ring and reads the pinned words */
+    if (r->reader_attached) reader_stop(r);             /* it reads the regions, the pinned words and the block */
     if (r->in_flight && r->hw) {
         r->hw->stop = 1;
         cudaEventSynchronize(r->launch_owner ? r->launch_owner->ev_stop : r->ev_stop);
@@ -502,6 +542,7 @@ extern "C" void apus_replica_destroy(apus_replica_t *r)
     if (r->stream) cudaStreamDestroy(r->stream);
     if (r->copy_stream) cudaStreamDestroy(r->copy_stream);
     if (r->hw) cudaFreeHost((void *)r->hw);
+    if (r->rb) cudaFreeHost((void *)r->rb);
     if (r->vmm_handle && g_drv.ok) {
         if (r->mc_region) { g_drv.MemUnmap((CUdeviceptr)r->mc_region, r->vmm_bytes); g_drv.MemAddressFree((CUdeviceptr)r->mc_region, r->vmm_bytes); }
         if (r->mc_handle) g_drv.MemRelease(r->mc_handle);
@@ -547,11 +588,19 @@ extern "C" int apus_replica_connect(apus_replica_t *r, uint8_t peer_idx, const a
                 return fail("cudaDeviceEnablePeerAccess: %s", cudaGetErrorString(e));
             cudaGetLastError();
         }
+        StageLock ll(&g_live_mu);
+        if (r->rb->member[peer_idx] != b.ptr) reader_forget(r, peer_idx);    /* another replica was mapped there */
         r->peer_ptr[peer_idx] = (void *)(uintptr_t)b.ptr;
         r->peer_is_ipc[peer_idx] = 0;
+        r->rb->member[peer_idx] = b.ptr;
     } else {
         void *p = NULL;
         if (r->vmm_handle) return fail("fabric-mode regions are shared between replicas of one process only");
+        StageLock ll(&g_live_mu);
+        if (r->reader_attached)
+            return fail("apus_replica_connect: a resident reader is attached, and readers do not read peers mapped "
+                        "through CUDA IPC (apus_reader_detach first)");
+        reader_forget(r, peer_idx);                      /* IPC-mapped peers are never entered */
         CK(cudaIpcOpenMemHandle(&p, b.ipc, cudaIpcMemLazyEnablePeerAccess));
         r->peer_ptr[peer_idx] = p;
         r->peer_is_ipc[peer_idx] = 1;
@@ -1549,6 +1598,61 @@ extern "C" int apus_consumer_detach(apus_replica_t *r)
     return APUS_OK;
 }
 
+/* ---- resident readers: an application's kernel runs read fences itself ---------------------------------------- */
+/* the offsets a reader view carries are part of the ABI: a reader compiled against an older header reads the same words */
+static_assert(APUS_REGION_CONS_REC == 896 && APUS_REGION_CONS_ON == 928 && APUS_REGION_SID == 1024,
+              "the words a fence reads in another region keep their offsets");
+static_assert(APUS_READER_SLOTS == sizeof(((apus_reader_block_t *)0)->busy) / 8 &&
+              APUS_MAX_SERVER_COUNT == sizeof(((apus_reader_block_t *)0)->member) / 8, "the reader block's arrays");
+
+extern "C" int apus_reader_attach(apus_replica_t *r, void *stream, apus_reader_view_t *out)
+{
+    if (consumer_gate(r, "apus_reader_attach", CONS_ANY_ROLE) != APUS_OK) return APUS_ERROR;
+    if (!out) return fail("null argument");
+    DeviceGuard g(r->cfg.device);
+    StageLock ll(&g_live_mu);                            /* connect and destroy change the member words under it */
+    if (r->reader_attached) return fail("apus_reader_attach: a resident reader is attached already (one per replica)");
+    for (int i = 0; i < APUS_MAX_SERVER_COUNT; i++)
+        if (r->peer_is_ipc[i] && r->peer_ptr[i])
+            return fail("apus_reader_attach: peer %d is mapped through CUDA IPC (readers are for groups hosted in one "
+                        "process)", i);
+    /* detach synchronises this stream: it must be the queue the reader runs on, on the replica's GPU */
+    int sdev = -1;
+    CK(cudaStreamGetDevice((cudaStream_t)stream, &sdev));
+    if (sdev != r->cfg.device)
+        return fail("apus_reader_attach: the stream is on device %d, the replica on device %d", sdev, r->cfg.device);
+    CK(apus_kernels_load());                             /* no lazy load of ours may wait for the reader from here on */
+    apus_reader_view_t v;
+    memset(&v, 0, sizeof v);
+    v.entries = r->region + r->entries_off;
+    v.log_len = r->log_len;
+    v.index = reinterpret_cast<const uint32_t *>(r->region + APUS_INDEX_OFF);
+    v.idx_mask = r->idx_cap - 1;
+    v.rec = reinterpret_cast<const uint64_t *>(r->region + offsetof(apus_ctrl_t, cons_rec));
+    v.role = const_cast<const uint64_t *>(&r->rb_dev->role);
+    v.busy = const_cast<uint64_t *>(r->rb_dev->busy);
+    v.member = const_cast<const uint64_t *>(r->rb_dev->member);
+    v.n = r->cfg.group_size;
+    v.own = r->cfg.server_idx;
+    v.on_off = APUS_REGION_CONS_ON; v.rec_off = APUS_REGION_CONS_REC; v.sid_off = APUS_REGION_SID;
+    v.release = const_cast<const uint64_t *>(&r->hw_dev->cons_wait_epoch);
+    v.stop = const_cast<const uint64_t *>(&r->hw_dev->reader_stop);
+    v.stop_epoch = r->hw->reader_stop;
+    r->reader_attached = 1;
+    r->reader_stream = (cudaStream_t)stream;
+    *out = v;
+    return APUS_OK;
+}
+
+extern "C" int apus_reader_detach(apus_replica_t *r)
+{
+    if (!r) return fail("null argument");
+    if (!r->reader_attached) return fail("apus_reader_detach: no resident reader is attached");
+    DeviceGuard g(r->cfg.device);
+    reader_stop(r);
+    return APUS_OK;
+}
+
 /* ---- resident submitters: an application's kernel writes the leader's HBM ring itself -------------------------- */
 extern "C" int apus_submitter_attach(apus_replica_t *r, void *stream, apus_submitter_view_t *out)
 {
@@ -2103,8 +2207,13 @@ extern "C" int apus_replica_disconnect(apus_replica_t *r, uint8_t peer_idx)
 {
     if (!r || peer_idx >= APUS_MAX_SERVER_COUNT) return fail("bad argument");
     if (r->in_flight) return fail("stop the kernel first");
-    /* the mapping itself is left alone (closing a handle whose exporter died is not worth the risk): nothing stores there any more */
-    if (peer_idx != r->cfg.server_idx) r->peer_ptr[peer_idx] = NULL;
+    /* the mapping itself is left alone (closing a handle whose exporter died is not worth the risk): nothing stores there
+     * any more, and no resident fence reads there once this returns */
+    if (peer_idx != r->cfg.server_idx) {
+        StageLock ll(&g_live_mu);
+        r->peer_ptr[peer_idx] = NULL;
+        reader_forget(r, peer_idx);
+    }
     return APUS_OK;
 }
 
@@ -2121,6 +2230,9 @@ extern "C" int apus_replica_set_role(apus_replica_t *r, uint8_t leader_idx, uint
     const bool was_leader = is_leader(r);
     r->cfg.leader_idx = leader_idx;
     r->cfg.term = term;
+    /* a resident fence takes t and L from here; the take-over's release below comes after this store */
+    r->rb->role = role_sid(r);
+    __sync_synchronize();
     if (!is_leader(r)) {
         if (!r->peer_ptr[leader_idx]) return fail("not connected to the new leader");
         /* the leader's adjustment already set end / old_end / the entry counter (and, for a joiner, head and commit):

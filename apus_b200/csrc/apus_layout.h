@@ -152,6 +152,21 @@ typedef struct apus_ctlwords {
     apus_vote_req_t vote_req[APUS_MAX_SERVERS];   /* [i] written by candidate i into everybody's block */
 } apus_ctlwords_t;
 
+/* the words a read fence reads in another replica's region, as byte offsets (apus_reader_view_t carries them) */
+#define APUS_REGION_CONS_ON  ((uint32_t)offsetof(apus_ctrl_t, cons_on))
+#define APUS_REGION_CONS_REC ((uint32_t)offsetof(apus_ctrl_t, cons_rec))
+#define APUS_REGION_SID      ((uint32_t)(APUS_CTL_OFF + offsetof(apus_ctlwords_t, sid)))
+
+/* Resident readers (apus_reader_attach): one pinned, mapped block per replica, kept current by the host (apus_gpu.h,
+ * include/apus_reader.cuh).  The busy words have a 128 B line to themselves, away from the words the host writes. */
+typedef struct apus_reader_block {
+    volatile uint64_t role;                           /* the SID this replica knows: term << 9 | 1 << 8 | leader idx */
+    uint64_t pad0[15];
+    volatile uint64_t member[APUS_MAX_SERVERS];       /* [i]: member i's region as mapped here (own at own idx; 0 = none) */
+    uint64_t pad1[3];
+    volatile uint64_t busy[32];                       /* [s]: odd while a fence of slot s reads other regions */
+} apus_reader_block_t;
+
 /* Sequencer shared by the leader's worker CTAs (device memory, gpu-scope atomics).
  * A worker CLAIMS the next slots of the submission ring (one compare-and-swap), builds its
  * tile in parallel with the others, but PLACES it in the log and PUBLISHES its tail strictly
@@ -240,7 +255,8 @@ typedef struct apus_hostwords {
                                             the consumer ends once it differs from the value it was attached under */
     volatile uint64_t submitter_stop;    /* host -> resident submitter (apus_submitter_attach): detach and destroy bump
                                             it, the same way */
-    uint64_t pad3[13];
+    volatile uint64_t reader_stop;       /* host -> resident reader (apus_reader_attach): detach and destroy bump it */
+    uint64_t pad3[12];
     volatile uint64_t heartbeat;         /* kernel liveness (debug) */
     volatile uint64_t error;             /* kernel-detected protocol error code */
     volatile uint64_t leader_suspect;    /* follower kernel -> host: 1 + term whose leader stopped sending heartbeats */
@@ -249,8 +265,8 @@ typedef struct apus_hostwords {
 #ifdef __cplusplus
 static_assert(offsetof(apus_hostwords_t, stop) == 256 && offsetof(apus_hostwords_t, host_apply) == 384 &&
               offsetof(apus_hostwords_t, consumer_stop) == 392 && offsetof(apus_hostwords_t, submitter_stop) == 400 &&
-              offsetof(apus_hostwords_t, heartbeat) == 512 && sizeof(apus_hostwords_t) == 544,
-              "the resident consumers' and submitters' stop words take spare words: no offset moves");
+              offsetof(apus_hostwords_t, reader_stop) == 408 && offsetof(apus_hostwords_t, heartbeat) == 512 && sizeof(apus_hostwords_t) == 544,
+              "the stop words of resident consumers, submitters and readers take spare words: no offset moves");
 #endif
 
 #define APUS_FLAG_FENCED_ACK 0x1u

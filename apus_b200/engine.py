@@ -67,6 +67,13 @@ class SubmitterView(C.Structure):
                 ("pay_end", vp), ("consumed", vp), ("committed", vp), ("stop", vp), ("stop_epoch", u64)]
 
 
+class ReaderView(C.Structure):
+    """apus_reader_view_t: what a resident reader kernel (include/apus_reader.cuh) takes by value"""
+    _fields_ = [("entries", vp), ("log_len", u64), ("index", vp), ("idx_mask", u32), ("pad", u32), ("rec", vp),
+                ("role", vp), ("busy", vp), ("member", vp), ("n", u32), ("own", u32), ("on_off", u32), ("rec_off", u32),
+                ("sid_off", u32), ("pad2", u32), ("release", vp), ("stop", vp), ("stop_epoch", u64)]
+
+
 ConsumeStatus = namedtuple("ConsumeStatus", "cursor next_idx need_stride error")
 WaitStatus = namedtuple("WaitStatus", "outcome available")
 FenceStatus = namedtuple("FenceStatus", "outcome index")
@@ -126,6 +133,8 @@ SIGNATURES = {
     "apus_consumer_detach": (C.c_int, [vp]),
     "apus_submitter_attach": (C.c_int, [vp, vp, C.POINTER(SubmitterView)]),
     "apus_submitter_detach": (C.c_int, [vp]),
+    "apus_reader_attach": (C.c_int, [vp, vp, C.POINTER(ReaderView)]),
+    "apus_reader_detach": (C.c_int, [vp]),
     "apus_leader_suspect": (u64, [vp]),
     "apus_last_commit_ns": (u64, [vp]),
     "apus_ctl_read": (C.c_int, [vp, vp]),
@@ -524,6 +533,20 @@ class Replica:
         """Ask the resident submitter to end, wait for its stream and hand the ring back to the host
         (apus_submitter_detach): the next host ticket follows the last one it published"""
         _ck(lib().apus_submitter_detach(self.h), "apus_submitter_detach")
+
+    def reader_attach(self, stream=None):
+        """Attach a resident reader (apus_reader_attach; F_DEVICE_APPLY | F_APPLY_ANY_ROLE, no peer mapped through CUDA
+        IPC).  `stream`: the stream its kernel will be launched on (default: the current stream of this replica's
+        device).  Returns the ReaderView to pass to that kernel by value.  Until reader_detach(), connecting a peer
+        through CUDA IPC is refused; everything else stays accepted."""
+        s = self._stream(stream)
+        v = ReaderView()
+        _ck(lib().apus_reader_attach(self.h, s.cuda_stream, C.byref(v)), "apus_reader_attach")
+        return v
+
+    def reader_detach(self):
+        """Ask the resident reader to end and wait for the stream it was attached with (apus_reader_detach)"""
+        _ck(lib().apus_reader_detach(self.h), "apus_reader_detach")
 
     def wait_committed_on_stream(self, ticket, stream=None):
         """make `stream` (default: the current stream of the leader's device) wait until `ticket` is committed"""

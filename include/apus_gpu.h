@@ -513,6 +513,51 @@ int  apus_submitter_attach(apus_replica_t *leader, void *stream, apus_submitter_
  * next ticket).  A dropped reservation's requests that were written as NOOPs stay counted.  apus_replica_destroy does
  * the same stop before it frees anything.  APUS_ERROR when none is attached. */
 int  apus_submitter_detach(apus_replica_t *leader);
+/* Resident readers: read fences that an application's own persistent kernel runs, with no host call per fence
+ * (include/apus_reader.cuh is its device API).  What a stream fence takes from the host when it is enqueued -- the term
+ * and leader, the peers' regions -- the reader reads from a pinned block the host keeps current: `role` holds the SID
+ * this replica knows (term << 9 | 1 << 8 | leader idx: one 8 B word, so that no fence sees a torn pair), `member[i]` the
+ * region of member i as this replica maps it (its own at its own index; 0 = not connected), and `busy[s]` is the
+ * sequence word of fencing slot s, odd while a fence of that slot reads other replicas' regions.  A fence runs in one
+ * slot at a time: fences that run at once use distinct slots. */
+#define APUS_READER_SLOTS 32
+typedef struct apus_reader_view {
+    const uint8_t  *entries;      /* this replica's log ring (device memory) ... */
+    uint64_t        log_len;      /* ... and its length in bytes */
+    const uint32_t *index;        /* the offset index (apus_consumer_view_t.index) */
+    uint32_t        idx_mask;
+    uint32_t        pad;
+    const uint64_t *rec;          /* this replica's consumer record {committed-and-held offset, entries held} */
+    const uint64_t *role;         /* pinned: the SID this replica knows (see above) */
+    uint64_t       *busy;         /* pinned: APUS_READER_SLOTS sequence words */
+    const uint64_t *member;       /* pinned: APUS_MAX_SERVER_COUNT region addresses */
+    uint32_t        n;            /* the group size */
+    uint32_t        own;          /* this replica's index */
+    uint32_t        on_off;       /* byte offsets inside a region: the consumer flag (2 = a record in every role), */
+    uint32_t        rec_off;      /* ... the consumer record */
+    uint32_t        sid_off;      /* ... and the SID word */
+    uint32_t        pad2;
+    const uint64_t *release;      /* pinned: the release epoch of consume waits and fences */
+    const uint64_t *stop;         /* pinned stop word: the reader ends once it no longer holds stop_epoch */
+    uint64_t        stop_epoch;
+} apus_reader_view_t;
+/* Attach a resident reader to a replica that stream fences accept (APUS_F_DEVICE_APPLY | APUS_F_APPLY_ANY_ROLE) and fill
+ * *out.  `stream` (a cudaStream_t on the replica's GPU, NULL = the legacy default stream) is the stream the application
+ * launches its reader kernel on.  A resident fence has the contract of apus_read_fence, except that t and L are what the
+ * role word holds when the fence begins, and that the reader's stop word ends it RELEASED too; it ends RELEASED at the
+ * release points of stream fences (apus_consume_wait_release, apus_replicas_stop, a take-over's apus_replica_set_role,
+ * destroy) and writes nothing to the status words apus_read_fence_status reads.  While attached:
+ *   - apus_replica_connect of a peer of another process (CUDA IPC) returns APUS_ERROR;
+ *   - stream fences, the consume calls and a resident consumer stay accepted: a reader never moves the cursor;
+ *   - apus_replica_set_role, stops and wait releases leave it attached, and set_role rewrites the role word first;
+ *   - apus_replica_disconnect and the destroy of a peer clear the peer's member word, then wait until no fence that
+ *     may have read the old word is still reading that peer's region.
+ * APUS_ERROR, with nothing written, where apus_read_fence refuses the replica, for a null `out`, a replica that maps a
+ * peer through CUDA IPC, a stream of another device, and when a reader is attached already. */
+int  apus_reader_attach(apus_replica_t *r, void *stream, apus_reader_view_t *out);
+/* Ask the resident reader to end (its stop word moves) and synchronise the stream it was attached with.
+ * apus_replica_destroy does the same before it frees anything.  APUS_ERROR when none is attached. */
+int  apus_reader_detach(apus_replica_t *r);
 /* failure detector: 0 while the leader's heartbeats arrive, else 1 + the term whose leader fell silent */
 uint64_t apus_leader_suspect(apus_replica_t *follower);
 /* %globaltimer (ns) of the leader kernel's latest commit (device clock; step timing of resident kernels) */
