@@ -4,16 +4,11 @@ include/apus_slot_format.h, their ctypes structures, and this module's own state
 (Placement), which the tests check against the header compiled as C.  Importing this module starts no CUDA context."""
 import ctypes as C
 import os
-import shutil
 import subprocess
-import tempfile
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-INCLUDE = os.path.join(ROOT, "include")
-SRC = os.path.join(HERE, "devicelogic", "header_probe.cu")
-WRITER_SRC = os.path.join(HERE, "hostlogic", "slot_writer.c")
-NVCC = ["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-I", INCLUDE]
+import device_build as DB
+
+WRITER_SRC = os.path.join(DB.HERE, "hostlogic", "slot_writer.c")
 
 NOOP, CSM, CONFIG, HEAD, CONNECT, SEND, CLOSE = 0, 1, 2, 3, 4, 5, 6
 ACCEPTED = (CSM, CONNECT, SEND, CLOSE)
@@ -55,28 +50,12 @@ class Out(C.Structure):
                 ("pad0", u64), ("pad1", u64)]
 
 
-def compile_so(outdir, extra=()):
-    """nvcc header_probe.cu into outdir/header_probe.so; returns (path, nvcc's output)"""
-    so = os.path.join(outdir, "header_probe.so")
-    p = subprocess.run(NVCC + ["-shared", "-Xcompiler", "-fPIC", *extra, "-o", so, SRC], capture_output=True, text=True,
-                       check=True)
-    return so, p.stdout + p.stderr
-
-
 def build_writer(outdir):
     """gcc slot_writer.c into outdir/slot_writer.so"""
     so = os.path.join(outdir, "slot_writer.so")
-    subprocess.run(["gcc", "-O2", "-std=gnu99", "-Wall", "-Werror", "-shared", "-fPIC", "-I", INCLUDE, "-o", so,
+    subprocess.run(["gcc", "-O2", "-std=gnu99", "-Wall", "-Werror", "-shared", "-fPIC", "-I", DB.INCLUDE, "-o", so,
                     WRITER_SRC], check=True)
     return so
-
-
-def _load(build):
-    tmp = tempfile.mkdtemp(prefix="header_probe_")
-    try:
-        return C.CDLL(build(tmp))                       # (the loaded library outlives its file)
-    finally:
-        shutil.rmtree(tmp, ignore_errors=True)
 
 
 _lib = None
@@ -87,7 +66,7 @@ def lib():
     """the compiled probe, loaded once per process"""
     global _lib
     if _lib is None:
-        L = _load(lambda d: compile_so(d)[0])
+        L = DB.load_kernel("header_probe")
         L.hp_copy.argtypes = [vp, vp, vp, u32, vp]
         L.hp_loads.argtypes = [vp, vp, vp, vp, vp]
         L.hp_consumer.argtypes = [vp, vp, u32, vp, u32, vp, u32, vp]
@@ -105,7 +84,7 @@ def writer():
     """the slot writer, built and loaded once per process"""
     global _writer
     if _writer is None:
-        W = _load(build_writer)
+        W = DB.load(build_writer)
         W.sw_put.restype = u32
         W.sw_put.argtypes = [vp, u32, vp, u64, u64, u32, u32, u16, u64, vp, u32]
         W.sw_reserve.restype = C.c_int

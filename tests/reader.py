@@ -2,16 +2,11 @@
 nvcc for sm_90a into a temporary directory against include/ alone, and a host handle per launch that keeps its fence
 log.  Importing this module starts no CUDA context: torch is loaded where it is used."""
 import ctypes as C
-import os
-import subprocess
-import tempfile
 import time
 from collections import namedtuple
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-SRC = os.path.join(HERE, "devicelogic", "resident_reads.cu")
-NVCC = ["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-I", os.path.join(ROOT, "include")]
+import device_build as DB
+
 END_STOP, END_TARGET, END_DEADLINE = 1, 2, 3
 LOG_WORDS = 12
 
@@ -27,14 +22,6 @@ class Args(C.Structure):
                 ("deadline_ns", u64), ("gap_ns", u64), ("begun", vp), ("out", vp), ("slot0", u32), ("has_cv", u32)]
 
 
-def compile_so(outdir, extra=()):
-    """nvcc resident_reads.cu into outdir/resident_reads.so; returns (path, nvcc's output)"""
-    so = os.path.join(outdir, "resident_reads.so")
-    p = subprocess.run(NVCC + ["-shared", "-Xcompiler", "-fPIC", *extra, "-o", so, SRC], capture_output=True, text=True,
-                       check=True)
-    return so, p.stdout + p.stderr
-
-
 _lib = None
 
 
@@ -42,8 +29,7 @@ def lib():
     """the compiled reader, loaded (and its kernel loaded into the context) once per process"""
     global _lib
     if _lib is None:
-        so, _ = compile_so(tempfile.mkdtemp(prefix="resident_reads_"))
-        L = C.CDLL(so)
+        L = DB.load_kernel("resident_reads")
         L.rd_launch.argtypes = [vp, vp, vp, C.c_uint, vp]
         L.rd_load.restype = C.c_int
         L.rd_args_size.restype = C.c_uint

@@ -3,15 +3,10 @@ with nvcc for sm_90a into a temporary directory against include/apus_consumer.cu
 that keeps its rows, its cursor log and its control words.  Importing this module starts no CUDA context: torch is
 loaded where it is used."""
 import ctypes as C
-import os
-import subprocess
-import tempfile
 import time
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-SRC = os.path.join(HERE, "devicelogic", "resident_rows.cu")
-NVCC = ["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-I", os.path.join(ROOT, "include")]
+import device_build as DB
+
 END_STOP, END_TARGET, END_BAD_IDX, END_FULL, END_DEADLINE = 1, 2, 3, 4, 5
 
 vp, u64, u32 = C.c_void_p, C.c_uint64, C.c_uint32
@@ -25,14 +20,6 @@ class Args(C.Structure):
                 ("ctl", vp), ("pos", vp), ("out", vp)]
 
 
-def compile_so(outdir, extra=()):
-    """nvcc resident_rows.cu into outdir/resident_rows.so; returns (path, nvcc's output)"""
-    so = os.path.join(outdir, "resident_rows.so")
-    p = subprocess.run(NVCC + ["-shared", "-Xcompiler", "-fPIC", *extra, "-o", so, SRC], capture_output=True, text=True,
-                       check=True)
-    return so, p.stdout + p.stderr
-
-
 _lib = None
 
 
@@ -40,8 +27,7 @@ def lib():
     """the compiled consumer, loaded (and its kernel loaded into the context) once per process"""
     global _lib
     if _lib is None:
-        so, _ = compile_so(tempfile.mkdtemp(prefix="resident_rows_"))
-        L = C.CDLL(so)
+        L = DB.load_kernel("resident_rows")
         L.rr_launch.argtypes = [vp, vp, vp]
         L.rr_load.restype = C.c_int
         L.rr_args_size.restype = C.c_uint

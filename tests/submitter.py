@@ -3,19 +3,12 @@ compiled with nvcc for sm_90a into a temporary directory against include/ alone,
 its request arrays and reads back the tickets it handed out, and the request streams and oracle orders the tests use.
 Importing this module starts no CUDA context: torch is loaded where it is used."""
 import ctypes as C
-import os
-import shutil
-import subprocess
-import tempfile
 
 import numpy as np
 
+import device_build as DB
 import streams as S
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-SRC = os.path.join(HERE, "devicelogic", "resident_submit.cu")
-NVCC = ["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-I", os.path.join(ROOT, "include")]
 WAIT, DROP_LAST = 1, 2                      # RS_WAIT, RS_DROP_LAST
 OK, TIMED_OUT, STOPPED, NEVER_FITS = 0, 1, 2, 3
 STEP_RESERVE, STEP_PUBLISH, STEP_WAIT = 1, 2, 3
@@ -32,14 +25,6 @@ class Args(C.Structure):
                 ("batch", u32), ("mode", u32), ("timeout_ns", u64), ("tickets", vp), ("lat_ns", vp), ("out", vp)]
 
 
-def compile_so(outdir, extra=()):
-    """nvcc resident_submit.cu into outdir/resident_submit.so; returns (path, nvcc's output)"""
-    so = os.path.join(outdir, "resident_submit.so")
-    p = subprocess.run(NVCC + ["-shared", "-Xcompiler", "-fPIC", *extra, "-o", so, SRC], capture_output=True, text=True,
-                       check=True)
-    return so, p.stdout + p.stderr
-
-
 _lib = None
 
 
@@ -48,12 +33,7 @@ def lib():
     global _lib
     if _lib is None:
         from apus_b200 import engine as E
-        tmp = tempfile.mkdtemp(prefix="resident_submit_")
-        try:
-            so, _ = compile_so(tmp)
-            L = C.CDLL(so)                              # (the loaded library outlives its file)
-        finally:
-            shutil.rmtree(tmp, ignore_errors=True)
+        L = DB.load_kernel("resident_submit")
         L.rs_launch.argtypes = [vp, vp, C.c_uint, vp]
         L.rs_load.restype = C.c_int
         L.rs_args_size.restype = C.c_uint

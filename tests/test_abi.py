@@ -117,12 +117,20 @@ def test_fence_status_words_take_spare_host_words():
 
 
 def test_null_replica_is_refused(built):
-    """every call that checks which replicas may consume refuses a null replica first, whatever its other arguments"""
+    """every call that checks which replicas may consume, and the attach and detach of every resident kernel, refuses a
+    null replica first, whatever its other arguments; an attach writes nothing to the view"""
     lib = built.load_library()
     buf = (C.c_uint64 * 16)()
     a = C.addressof(buf)
     w = [C.byref(C.c_uint64()) for _ in range(4)]
+    views = [built.ConsumerView(), built.SubmitterView(), built.ReaderView()]
     calls = {
+        "apus_consumer_attach": (None, C.byref(views[0])),
+        "apus_submitter_attach": (None, C.byref(views[1])),
+        "apus_reader_attach": (None, C.byref(views[2])),
+        "apus_consumer_detach": (),
+        "apus_submitter_detach": (),
+        "apus_reader_detach": (),
         "apus_consume_device": (1, a, a, a, a, a, a, 8, a, None),
         "apus_consume_device_packed": (1, a, a, a, a, a, a, 8, a, None),
         "apus_consume_status": (w[0], w[1], w[2], w[3]),
@@ -138,6 +146,8 @@ def test_null_replica_is_refused(built):
         assert name in built.EXPORTS, name
         assert getattr(lib, name)(None, *args) == built.APUS_ERROR, name
         assert lib.apus_last_error() == b"null argument", (name, lib.apus_last_error())
+    for v in views:
+        assert bytes(v) == bytes(C.sizeof(v)), type(v)
 
 
 def test_nm_shows_kernel_and_c_abi(built):
