@@ -211,7 +211,8 @@ struct apus_replica {
     apus_cons_state_t *cons_st;   /* consume state + APUS_CONS_BLK_WORDS per consume block (index-ring capacity / block size) */
     pthread_mutex_t cons_mu;      /* one enqueue at a time: the two events are shared by every caller */
     uint64_t cons_enqueued;       /* consume, wait and mark enqueues so far (under cons_mu): a seed needs none */
-    resident_t res[RES_KINDS];    /* an attached consumer alone moves the cursor, an attached submitter the ring */
+    resident_t res[RES_KINDS];    /* an attached consumer alone moves the cursor, an active submitter the ring */
+    int      sub_active;          /* the attached submitter holds the ring (0: none attached, or it is dormant) */
     apus_submitter_state_t *sub_st;   /* device: the resident submitter's state, followed by pay_end[ring_slots] */
     /* the pinned block a resident reader reads its role and the peers' regions from.  The member words change under
      * g_live_mu */
@@ -322,11 +323,11 @@ static void reader_forget(apus_replica *r, int i)
     }
 }
 
-/* the calls that write the submission ring: a resident submitter, while attached, alone writes it */
+/* the calls that write the submission ring: a resident submitter, while active, alone writes it */
 static int ring_writer_gate(const apus_replica *r, const char *what)
 {
     if (!r) return fail("null argument");
-    if (r->res[RES_SUBMITTER].attached)
+    if (r->sub_active)
         return fail("%s: a resident submitter is attached (apus_submitter_detach first): it alone writes the ring", what);
     return APUS_OK;
 }
@@ -665,6 +666,7 @@ static void fill_ctx(apus_replica *r, uint64_t target)
     c->lat_ns = r->d_lat;
 }
 
+static int submitter_hand_over(apus_replica *r);
 extern "C" int apus_replicas_launch(apus_replica_t **rs, int n, uint64_t target)
 {
     if (!rs || n < 1 || n > 64) return fail("bad replica list");
@@ -676,6 +678,11 @@ extern "C" int apus_replicas_launch(apus_replica_t **rs, int n, uint64_t target)
         if (!is_leader(rs[i]) && !rs[i]->peer_ptr[rs[i]->cfg.leader_idx]) return fail("follower not connected to its leader");
     }
     DeviceGuard g(owner->cfg.device);
+    /* a leader's dormant submitter takes the ring over before the kernel runs: the host's tickets come first */
+    for (int i = 0; i < n; i++)
+        if (is_leader(rs[i]) && rs[i]->res[RES_SUBMITTER].attached && !rs[i]->sub_active &&
+            submitter_hand_over(rs[i]) != APUS_OK)
+            return APUS_ERROR;
     apus_role_t roles[MAX_ROLES];
     int nroles = 0;
     for (int i = 0; i < n; i++) {
@@ -1661,23 +1668,49 @@ extern "C" int apus_reader_detach(apus_replica_t *r)
 }
 
 /* ---- resident submitters: an application's kernel writes the leader's HBM ring itself -------------------------- */
-extern "C" int apus_submitter_attach(apus_replica_t *r, void *stream, apus_submitter_view_t *out)
+/* The hand-over of a leader's ring from the host to its attached, dormant submitter (attach on a leader, and the
+ * first launch that runs a dormant one's replica as leader): everything the host has submitted reaches the ring and
+ * the doorbell, then the accounting words and pay_end reach the submitter's state, then the term it holds the ring in,
+ * and last the lock word, which the host has held since attach (APUS_SUBMITTER_HOST_HELD): each copy is complete
+ * before the next begins, and the reserving thread's CAS acquires the lock only once it reads the host's 0
+ * (include/apus_submitter.cuh).  While the host holds the lock no kernel thread holds it. */
+static int submitter_hand_over(apus_replica *r)
 {
-    if (!r || !out) return fail("null argument");
-    if (!is_leader(r)) return fail("apus_submitter_attach: a resident submitter writes the leader's ring (this is a follower)");
-    if (r->cfg.ring_mode != APUS_RING_DEVICE) return fail("apus_submitter_attach needs the device submission ring");
-    DeviceGuard g(r->cfg.device);
-    if (resident_attach_check(r, RES_SUBMITTER, stream) != APUS_OK) return APUS_ERROR;
-    /* everything the host has submitted reaches the ring and the doorbell first: the submitter's turns start there */
     if (ring_flush(r) != APUS_OK) return APUS_ERROR;
     CK(cudaStreamSynchronize(r->copy_stream));
     apus_submitter_state_t s;
     memset(&s, 0, sizeof s);
     s.submitted = r->submitted; s.pay_head = r->pay_head; s.wrap_next = r->wrap_next ? 1 : 0;
-    s.consumed = r->hw->consumed; s.first_rejected = ~0ull;
-    CK(cudaMemcpyAsync(r->sub_st, &s, sizeof s, cudaMemcpyHostToDevice, r->copy_stream));
+    s.consumed = r->hw->consumed; s.lead_term = r->cfg.term;
+    const size_t a = offsetof(apus_submitter_state_t, submitted), b = offsetof(apus_submitter_state_t, rejected);
+    CK(cudaMemcpyAsync((char *)r->sub_st + a, (const char *)&s + a, b - a, cudaMemcpyHostToDevice, r->copy_stream));
     CK(cudaMemcpyAsync(r->sub_st + 1, r->pay_end, 8ull * r->ring_slots, cudaMemcpyHostToDevice, r->copy_stream));
     CK(cudaStreamSynchronize(r->copy_stream));
+    CK(cudaMemcpyAsync(&r->sub_st->lead_term, &s.lead_term, 8, cudaMemcpyHostToDevice, r->copy_stream));
+    CK(cudaStreamSynchronize(r->copy_stream));
+    CK(cudaMemcpyAsync(&r->sub_st->lock, &s.lock, 8, cudaMemcpyHostToDevice, r->copy_stream));   /* the release: 0 */
+    CK(cudaStreamSynchronize(r->copy_stream));
+    r->sub_active = 1;
+    return APUS_OK;
+}
+
+extern "C" int apus_submitter_attach(apus_replica_t *r, void *stream, apus_submitter_view_t *out)
+{
+    if (!r || !out) return fail("null argument");
+    if (r->cfg.ring_mode != APUS_RING_DEVICE)
+        return fail("apus_submitter_attach needs the device submission ring%s",
+                    is_leader(r) ? "" : " (this is a follower on a host-mapped ring)");
+    DeviceGuard g(r->cfg.device);
+    if (resident_attach_check(r, RES_SUBMITTER, stream) != APUS_OK) return APUS_ERROR;
+    if (leader_ring_init(r) != APUS_OK) return APUS_ERROR;      /* a follower's ring: the view's words exist from now */
+    /* dormant, the lock held by the host, nothing reserved: no kernel of this submitter runs yet, so the whole state is
+     * written */
+    apus_submitter_state_t s;
+    memset(&s, 0, sizeof s);
+    s.lock = APUS_SUBMITTER_HOST_HELD; s.first_rejected = ~0ull; s.lead_term = APUS_SUBMITTER_DORMANT;
+    CK(cudaMemcpyAsync(r->sub_st, &s, sizeof s, cudaMemcpyHostToDevice, r->copy_stream));
+    CK(cudaStreamSynchronize(r->copy_stream));
+    if (is_leader(r) && submitter_hand_over(r) != APUS_OK) return APUS_ERROR;
     apus_submitter_view_t v;
     memset(&v, 0, sizeof v);
     v.slots = reinterpret_cast<uint8_t *>(r->ring_desc_dev);
@@ -1700,6 +1733,8 @@ extern "C" int apus_submitter_detach(apus_replica_t *r)
     if (!r) return fail("null argument");
     DeviceGuard g(r->cfg.device);
     if (resident_stop(r, RES_SUBMITTER) != APUS_OK) return APUS_ERROR;
+    if (!r->sub_active) return APUS_OK;                  /* dormant: the host has kept the ring */
+    r->sub_active = 0;
     /* hand the ring back: the doorbell P is what the leader may read; reservations past it are dropped */
     apus_submitter_state_t s;
     uint64_t P = 0;
@@ -1729,7 +1764,7 @@ extern "C" int apus_get_stats(apus_replica_t *r, apus_stats_t *out)
     CK(cudaStreamSynchronize(r->copy_stream));
     memset(out, 0, sizeof *out);
     out->tickets_submitted = r->submitted;
-    if (r->res[RES_SUBMITTER].attached) {                /* the resident submitter's published tickets: the doorbell */
+    if (r->sub_active) {                                 /* the resident submitter's published tickets: the doorbell */
         CK(cudaMemcpyAsync(&out->tickets_submitted, r->sub_tail_dev, 8, cudaMemcpyDeviceToHost, r->copy_stream));
         CK(cudaStreamSynchronize(r->copy_stream));
     }
@@ -2219,9 +2254,9 @@ extern "C" int apus_replica_disconnect(apus_replica_t *r, uint8_t peer_idx)
 extern "C" int apus_replica_set_role(apus_replica_t *r, uint8_t leader_idx, uint64_t term)
 {
     if (!r || leader_idx >= r->cfg.group_size) return fail("bad argument");
-    if (r->res[RES_SUBMITTER].attached)
-        return fail("apus_replica_set_role: a resident submitter is attached (apus_submitter_detach first): it does not "
-                    "follow a take-over");
+    if (r->sub_active)
+        return fail("apus_replica_set_role: a resident submitter holds this replica's ring (apus_submitter_detach "
+                    "first): an active submitter does not step down");
     if ((r->cfg.flags & APUS_F_DEVICE_APPLY) && !(r->cfg.flags & APUS_F_APPLY_ANY_ROLE))
         return fail("a replica with device consumers (APUS_F_DEVICE_APPLY) keeps its role");
     if (r->in_flight) return fail("stop the kernel first");
@@ -2246,6 +2281,13 @@ extern "C" int apus_replica_set_role(apus_replica_t *r, uint8_t leader_idx, uint
     if (leader_ring_init(r) != APUS_OK) return APUS_ERROR;
     r->submitted = r->flushed = r->belled = 0; r->pay_head = r->pay_flushed = 0;
     r->hw->sub_tail = 0; r->hw->consumed = 0; r->hw->committed_tickets = 0;
+    if (r->cfg.ring_mode == APUS_RING_DEVICE) {
+        /* the device doorbell too: a replica that led before left its last value there, and the kernel does not poll
+         * the stamps of a device ring.  An attached submitter is dormant here; the hand-over writes its state */
+        *r->sub_tail_stage = 0;
+        CK(cudaMemcpyAsync(r->sub_tail_dev, r->sub_tail_stage, 8, cudaMemcpyHostToDevice, r->copy_stream));
+        CK(cudaStreamSynchronize(r->copy_stream));
+    }
     apus_loghdr_t h; apus_ctrl_t c;
     if (own_read(r, APUS_HDR_OFF, &h, sizeof h) != APUS_OK || own_read(r, 0, &c, sizeof c) != APUS_OK) return APUS_ERROR;
     const uint64_t L = r->log_len, last = c.acked;

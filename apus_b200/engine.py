@@ -61,8 +61,15 @@ class ConsumerView(C.Structure):
                 ("cur", vp), ("error", vp), ("status", vp), ("stop", vp), ("stop_epoch", u64)]
 
 
+# a dormant submitter's apus_submitter_state_t (its replica has not led since attach): the host holds its lock word,
+# and lead_term names no term
+SUBMITTER_HOST_HELD, SUBMITTER_DORMANT = 2, (1 << 64) - 1
+
+
 class SubmitterView(C.Structure):
-    """apus_submitter_view_t: what a resident submitter kernel (include/apus_submitter.cuh) takes by value"""
+    """apus_submitter_view_t: what a resident submitter kernel (include/apus_submitter.cuh) takes by value.  `state`
+    points at apus_submitter_state_t: lock, submitted, pay_head, wrap_next, consumed, rejected, first_rejected and
+    lead_term (the term the submitter holds the ring in, SUBMITTER_DORMANT until then), eight 64-bit words"""
     _fields_ = [("slots", vp), ("pay", vp), ("doorbell", vp), ("ring_slots", u32), ("ring_bytes", u32), ("state", vp),
                 ("pay_end", vp), ("consumed", vp), ("committed", vp), ("stop", vp), ("stop_epoch", u64)]
 
@@ -520,17 +527,19 @@ class Replica:
         _ck(lib().apus_consumer_detach(self.h), "apus_consumer_detach")
 
     def submitter_attach(self, stream=None):
-        """Attach a resident submitter to this leader (apus_submitter_attach; APUS_RING_DEVICE only): everything the
-        host submitted has reached the ring when this returns.  `stream`: the stream its kernel will be launched on
-        (default: the current stream of this replica's device).  Returns the SubmitterView to pass to that kernel by
-        value.  Until submitter_detach(), every call that writes the ring, and set_role, is refused."""
+        """Attach a resident submitter to this replica (apus_submitter_attach; APUS_RING_DEVICE only).  On a leader it
+        is active at once: everything the host submitted has reached the ring when this returns, and until
+        submitter_detach() every call that writes the ring, and set_role, is refused.  On a follower it is dormant: its
+        reserves end NOT_LEADER and the host calls behave as without it, until the first launch that runs this replica
+        as leader hands the ring over.  `stream`: the stream its kernel will be launched on (default: the current
+        stream of this replica's device).  Returns the SubmitterView to pass to that kernel by value."""
         s = self._stream(stream)
         v = SubmitterView()
         _ck(lib().apus_submitter_attach(self.h, s.cuda_stream, C.byref(v)), "apus_submitter_attach")
         return v
 
     def submitter_detach(self):
-        """Ask the resident submitter to end, wait for its stream and hand the ring back to the host
+        """Ask the resident submitter to end, wait for its stream and, if it was active, hand the ring back to the host
         (apus_submitter_detach): the next host ticket follows the last one it published"""
         _ck(lib().apus_submitter_detach(self.h), "apus_submitter_detach")
 

@@ -173,6 +173,9 @@ int  apus_group_multicast(apus_replica_t **rs, int n);
  * the cumulative ticket target is reached -- leader: that many requests committed;
  * follower: that many entries acked and applied -- or when apus_replicas_stop()
  * is called.  target_tickets == UINT64_MAX runs until stopped (service mode).
+ * A leader with a dormant resident submitter hands its ring over to it first
+ * (apus_submitter_attach): the host's submissions so far come before the
+ * submitter's first ticket, and the host paths are refused from then on.
  * Asynchronous: returns after the launch. */
 int  apus_replicas_launch(apus_replica_t **rs, int n, uint64_t target_tickets);
 /* Wait for the launch that included `r` to finish; timeout_ms < 0 waits forever.
@@ -469,15 +472,18 @@ int  apus_consumer_detach(apus_replica_t *r);
  * (include/apus_submitter.cuh is its device API; the slot format is include/apus_slot_format.h).  The submitter's state
  * lives in device memory: reservations take tickets and payload space in one order under its lock. */
 typedef struct apus_submitter_state {
-    uint64_t lock;                /* 0 = free; taken with a CAS by the reserving thread */
+    uint64_t lock;                /* 0 = free; taken with a CAS by the reserving thread; APUS_SUBMITTER_HOST_HELD while
+                                     dormant: the host holds it, and releases it last in the hand-over */
     uint64_t submitted;           /* tickets handed out (reserved) so far */
     uint64_t pay_head;            /* payload bytes handed out so far (monotone; position = % ring_bytes) */
     uint64_t wrap_next;           /* 1: the next external image carries APUS_SLOT_WRAP */
     uint64_t consumed;            /* the leader's consumed tickets as last read over PCIe (a lower bound) */
     uint64_t rejected;            /* requests written as NOOPs ... */
     uint64_t first_rejected;      /* ... and the lowest ticket among them (UINT64_MAX = none) */
-    uint64_t pad;
+    uint64_t lead_term;           /* the term the submitter holds the ring in (APUS_SUBMITTER_DORMANT until then) */
 } apus_submitter_state_t;
+#define APUS_SUBMITTER_HOST_HELD 2ull
+#define APUS_SUBMITTER_DORMANT (~0ull)
 typedef struct apus_submitter_view {
     uint8_t        *slots;        /* the leader's HBM slot ring: ring_slots slots of 128 B (apus_slot_t) */
     uint8_t        *pay;          /* ... and its payload ring of ring_bytes bytes */
@@ -491,27 +497,35 @@ typedef struct apus_submitter_view {
     const uint64_t *stop;         /* pinned stop word: the submitter ends once it no longer holds stop_epoch */
     uint64_t        stop_epoch;
 } apus_submitter_view_t;
-/* Attach a resident submitter to a leader created with APUS_RING_DEVICE.  It pushes and rings everything the host has
- * submitted, waits for that to reach the ring, copies the ring accounting (tickets handed out, the payload counter,
- * pay_end of the unconsumed tickets) into the submitter's device state and fills *out.  `stream` (a cudaStream_t on
- * the leader's GPU, NULL = the legacy default stream) is the stream the application launches its submitter on.  While
- * attached:
+/* Attach a resident submitter to a replica created with APUS_RING_DEVICE, leader or follower, and fill *out.  `stream`
+ * (a cudaStream_t on the replica's GPU, NULL = the legacy default stream) is the stream the application launches its
+ * submitter on.  Attach allocates the replica's submission ring if it has none yet, so that the view stays valid through
+ * any number of take-overs.  A submitter is dormant or active:
+ *   - on a follower it starts dormant: apus_submitter_reserve returns APUS_SUBMITTER_NOT_LEADER at once and writes
+ *     nothing, apus_replica_set_role is accepted, and the host paths behave as with no submitter attached (a winner
+ *     submits its blank CONFIG through them before its first launch);
+ *   - it becomes active by the hand-over: everything the host has submitted is pushed and rung, the ring accounting
+ *     (tickets handed out, the payload counter, pay_end of the unconsumed tickets) is copied into its device state,
+ *     and then the term it holds the ring in.  On a leader attach makes the hand-over; a dormant submitter gets it from
+ *     the first apus_replicas_launch that runs its replica as leader, before that launch.
+ * While active:
  *   - the submitter alone writes the ring: apus_submit, apus_submit_batch, _uniform, _synth, _device, _device_packed,
  *     apus_submit_defer, _flush, _release and apus_closed_loop return APUS_ERROR with nothing written;
- *   - apus_replica_set_role on this replica returns APUS_ERROR (a submitter does not follow a take-over: detach first);
+ *   - apus_replica_set_role on this replica returns APUS_ERROR: an active submitter does not step down (detach first;
+ *     the replica may attach again once it follows, dormant; include/apus_submitter.cuh says why);
  *   - apus_replicas_stop leaves it attached: its reservations and commit waits then end at their timeouts;
  *   - reads stay accepted: apus_committed_tickets, apus_wait_committed, apus_stream_wait_committed, apus_get_stats
  *     (tickets_submitted counts the published device tickets) and apus_device_submit_status (which counts the requests
  *     the submitter wrote as NOOPs).
- * APUS_ERROR for a null replica or `out`, on a follower, on a host-mapped ring, for a stream of another device, and when
- * a submitter is attached already. */
+ * APUS_ERROR for a null replica or `out`, on a host-mapped ring (leader or follower), for a stream of another device,
+ * and when a submitter is attached already. */
 int  apus_submitter_attach(apus_replica_t *leader, void *stream, apus_submitter_view_t *out);
-/* Ask the resident submitter to end (its stop word moves), synchronise the stream it was attached with, and hand the
- * ring back to the host: what was published -- the doorbell P -- becomes the host's count of submitted tickets, the
+/* Ask the resident submitter to end (its stop word moves), synchronise the stream it was attached with, and, if it is
+ * active, hand the ring back to the host: what was published -- the doorbell P -- becomes the host's count of submitted tickets, the
  * payload counter becomes the one after ticket P, and the next host image carries APUS_SLOT_WRAP.  Reservations past P
  * were never visible to the leader: they are dropped, and the host hands their ticket numbers out again (P + 1 is the
- * next ticket).  A dropped reservation's requests that were written as NOOPs stay counted.  apus_replica_destroy does
- * the same stop before it frees anything.  APUS_ERROR when none is attached. */
+ * next ticket).  A dropped reservation's requests that were written as NOOPs stay counted.  A dormant submitter hands
+ * nothing back.  apus_replica_destroy does the same stop before it frees anything.  APUS_ERROR when none is attached. */
 int  apus_submitter_detach(apus_replica_t *leader);
 /* Resident readers: read fences that an application's own persistent kernel runs, with no host call per fence
  * (include/apus_reader.cuh is its device API).  What a stream fence takes from the host when it is enqueued -- the term
@@ -602,7 +616,9 @@ int  apus_ctl_adjust_follower(apus_replica_t *leader, uint8_t peer_idx, uint64_t
  * tail, submission ring); becoming follower adopts what the new leader's adjustment left (apus_ctl_view.adj_*).  With
  * APUS_F_APPLY_ANY_ROLE a new leader's device consumers go on from their cursor: the consume work enqueued before the
  * call runs first, then they may read up to the commit offset the leader adopted (the entries of earlier terms
- * committed with it). */
+ * committed with it).  A new leader's submission ring starts empty and its device doorbell at 0, however often it
+ * led before.  A dormant resident submitter stays attached and dormant; with an active one the call is refused
+ * (apus_submitter_attach). */
 int  apus_replica_set_role(apus_replica_t *r, uint8_t leader_idx, uint64_t term);
 /* leader: liveness counters of the followers (their kernels bump them while polling); a counter that stands still
  * is a follower that is gone (HB replies, dare_ibv_rc.c:912-958 -> fail_count -> check_failure_count) */

@@ -39,6 +39,30 @@
  * and reads the slots after it.  The turn wait acquires the previous publish, so a later doorbell value also covers the
  * earlier reservations' stores.  Commits are read with an acquire of the committed-tickets word (pinned, over PCIe).
  *
+ * Take-overs.  A submitter may be attached to a follower too (apus_submitter_attach): it is then dormant, and every
+ * reserve returns APUS_SUBMITTER_NOT_LEADER at once, writing nothing, while the host paths of that replica stay open.
+ * The first apus_replicas_launch that runs the replica as leader hands the ring over before the launch: the host's
+ * submissions (the winner's blank CONFIG) reach the ring, the accounting is copied into the state, lead_term becomes
+ * the term of that leadership, and the host releases the lock.  From then on reservations are OK and carry that term (res.term), and
+ * apus_submitter_leading returns it.  So one persistent kernel per replica, launched once, writes through any number of
+ * take-overs: it waits out NOT_LEADER on the followers and, after a take-over, compares the term of its reservations
+ * with the one it wrote under to decide what to resubmit.  The rows carry (conn, req_id); the engine removes no
+ * duplicates.
+ *
+ * An active submitter does not step down: apus_replica_set_role refuses its replica, and a deposed or stopped leader
+ * detaches its submitter before it rejoins as a follower (then attaches again, dormant).  The application's threads may
+ * be delayed without bound between reserve, put and publish, so a put or publish of an earlier leadership could land in
+ * the ring after a later hand-over, and nothing in the engine could fence it off: only the stop word, which detach
+ * moves and then waits for the submitter's stream, ends every such thread before the ring changes hands.
+ *
+ * The hand-over's memory order.  While dormant, the lock word holds APUS_SUBMITTER_HOST_HELD: the host holds the lock,
+ * so no kernel thread does, and a reserve's CAS fails on that value and ends NOT_LEADER.  The host writes the
+ * accounting words (submitted .. consumed) and pay_end in one copy, synchronises, writes lead_term in a copy of its
+ * own, synchronises, and only then writes 0 into the lock word: the release.  It writes the lock word at no other
+ * time once a kernel may run.  The reserving thread's CAS acquires the lock (atom.acquire.gpu) only once it reads
+ * that 0, so the accounting it then reads under the lock, and the term it reads after it, are the host's.  An active
+ * reservation's critical section is the one it was before the hand-over existed; the term is one load after unlock.
+ *
  * The L1 rule.  The submitter never reads ring bytes.  Its state (the lock, counters and pay_end) is read and written
  * only by the reserving thread under the lock, with volatile accesses that bypass L1, and the leader's words are read
  * with system-scope loads, which bypass L1 as well; an application that reads the ring itself must do the same.
@@ -58,6 +82,7 @@
 #define APUS_SUBMITTER_TIMED_OUT   1u
 #define APUS_SUBMITTER_STOPPED     2u   /* the stop word moved: apus_submitter_detach or apus_replica_destroy */
 #define APUS_SUBMITTER_NEVER_FITS  3u   /* reserve only: n is 0 or above ring_slots, or the bytes exceed ring_bytes */
+#define APUS_SUBMITTER_NOT_LEADER  4u   /* reserve only: the submitter is dormant (its replica has not led since attach) */
 
 typedef struct apus_submitter_res {
     uint64_t first_ticket;  /* tickets first_ticket .. first_ticket + n - 1 */
@@ -66,6 +91,7 @@ typedef struct apus_submitter_res {
     uint32_t wrap;          /* 1: the first external image carries APUS_SLOT_WRAP */
     uint32_t outcome;       /* APUS_SUBMITTER_*; the other fields are meaningful only for APUS_SUBMITTER_OK */
     uint32_t pad;
+    uint64_t term;          /* the term the submitter held the ring in when it made the reservation */
 } apus_submitter_res_t;
 
 // ---------------------------------------------------------------------------------
@@ -115,13 +141,15 @@ __device__ __forceinline__ bool apus_submitter_should_stop(const apus_submitter_
 // ---------------------------------------------------------------------------------
 // reserve: n consecutive tickets and ext_bytes of the payload ring, one thread
 // ---------------------------------------------------------------------------------
-__device__ __forceinline__ bool apus_submitter_lock(apus_submitter_state_t *s)
+// one try at the lock: the word it held (0: taken now; APUS_SUBMITTER_HOST_HELD: the submitter is dormant)
+__device__ __forceinline__ uint32_t apus_submitter_try_lock(apus_submitter_state_t *s)
 {
     uint32_t old;
     asm volatile("{ .reg .u64 o; atom.acquire.gpu.global.cas.b64 o, [%1], 0, 1; cvt.u32.u64 %0, o; }"
                  : "=r"(old) : "l"(&s->lock) : "memory");
-    return old == 0;
+    return old;
 }
+__device__ __forceinline__ bool apus_submitter_lock(apus_submitter_state_t *s) { return apus_submitter_try_lock(s) == 0; }
 __device__ __forceinline__ void apus_submitter_unlock(apus_submitter_state_t *s) { apus_st_release_gpu(&s->lock, 0); }
 
 // under the lock: room for the reservation in both rings, placed and accounted; false when there is none now
@@ -153,22 +181,39 @@ __device__ __forceinline__ bool apus_submitter_try_reserve(const apus_submitter_
     return true;
 }
 
+// the term the submitter holds the ring in, or 0 while it is dormant
+__device__ __forceinline__ uint64_t apus_submitter_leading(const apus_submitter_view_t &v)
+{
+    const uint64_t t = apus_ld_relaxed_sys(&v.state->lead_term);
+    return t == APUS_SUBMITTER_DORMANT ? 0 : t;
+}
+
 // Reserve n consecutive tickets and ext_bytes payload-ring bytes (the sum of apus_submitter_ext_bytes of the n
-// requests), waiting while either ring is full, until the stop word moves or timeout_ns has passed.
+// requests), waiting while either ring is full, until the stop word moves or timeout_ns has passed.  A dormant
+// submitter gets APUS_SUBMITTER_NOT_LEADER at once, with nothing written.
 __device__ __forceinline__ apus_submitter_res_t apus_submitter_reserve(const apus_submitter_view_t &v, uint32_t n,
                                                                        uint64_t ext_bytes, uint64_t timeout_ns)
 {
     apus_submitter_res_t res;
-    res.first_ticket = 0; res.pos = 0; res.n = 0; res.wrap = 0; res.pad = 0;
+    res.first_ticket = 0; res.pos = 0; res.n = 0; res.wrap = 0; res.pad = 0; res.term = 0;
     res.outcome = APUS_SUBMITTER_NEVER_FITS;
     if (n == 0 || n > v.ring_slots || ext_bytes > v.ring_bytes) return res;
     apus_consumer_poll_t p = apus_consumer_poll_init();
     const uint64_t t0 = p.t_chk;
     for (;;) {
-        if (apus_submitter_lock(v.state)) {
+        const uint32_t held = apus_submitter_try_lock(v.state);
+        if (held == 0) {
             const bool ok = apus_submitter_try_reserve(v, n, ext_bytes, &res);
             apus_submitter_unlock(v.state);
-            if (ok) { res.outcome = APUS_SUBMITTER_OK; return res; }
+            if (ok) {
+                // after the acquire, so the host's term; outside the lock, which it does not lengthen
+                res.term = apus_ld_relaxed_sys(&v.state->lead_term);
+                res.outcome = APUS_SUBMITTER_OK;
+                return res;
+            }
+        } else if (held == APUS_SUBMITTER_HOST_HELD) {     // dormant: nothing taken, nothing written
+            res.outcome = APUS_SUBMITTER_NOT_LEADER;
+            return res;
         }
         if (apus_submitter_should_stop(v, p)) { res.outcome = APUS_SUBMITTER_STOPPED; return res; }
         if (apus_globaltimer_ns() - t0 >= timeout_ns) { res.outcome = APUS_SUBMITTER_TIMED_OUT; return res; }
